@@ -353,4 +353,28 @@ template <int N> PK_DEVICE void tma_store_wait_read_p(uint32_t pred) {
 
 PK_DEVICE void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
+// ---------------------------------------------------------------- PTX: shared-memory loads / stores
+// stores four 8 x 8 bf16 matrices; register i holds the thread's two elements of matrix i in the mma fragment layout (row lane / 4,
+// columns 2 * (lane % 4) + {0, 1}); lanes 8i .. 8i + 7 give the 16-byte row addresses of matrix i
+PK_DEVICE void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+PK_DEVICE uint4 lds_u32x4(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+PK_DEVICE float2 lds_f32x2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
+}
+PK_DEVICE void sts_f32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
+PK_DEVICE uint32_t bf16x2_max(uint32_t a, uint32_t b) {      // lane-wise max of two bf16 pairs (a NaN loses to a number)
+    uint32_t d;
+    asm("max.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+    return d;
+}
+
 }  // namespace pk

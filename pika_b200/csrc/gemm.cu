@@ -1,10 +1,14 @@
 // wgmma / TMA GEMM for sm_90a: C = epilogue(alpha * sum_p A_p * B_p^T).
 //
 // One persistent CTA per SM (ONE mode) or one 2-CTA cluster per pair of SMs (TWO mode), three warpgroups per CTA:
-//   warpgroup 0      TMA producer   (one converged warp: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
+//   warp 0           TMA producer   (one converged warp: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
+//   warps 1-3        epilogue       (bf16 C with the plain or LSE epilogue: take the finished C tile from shared memory, compute the
+//                                    row log-sum-exp partials, TMA-store it, hand it back; stage the next tile's bias)
 //   warpgroups 1, 2  consumers      (wgmma m64 x BN x k16 from shared-memory descriptors, fp32 accumulators in registers; each
-//                                    owns 64 rows of the 128-row tile, releases ring stages one k-block behind, then runs the fused
-//                                    epilogue: registers -> swizzled smem -> TMA store / TMA reduce-add)
+//                                    owns 64 rows of the 128-row tile, releases ring stages one k-block behind.  bf16 plain / LSE:
+//                                    alpha, bias, ReLU, bf16 rounding into the C tile with stmatrix, then straight on to the next
+//                                    tile's main loop.  EPI_FULL and f32 C: the whole epilogue, registers -> swizzled smem -> TMA store /
+//                                    TMA reduce-add, in 64-column chunks)
 // Tile 128 x BN x 64 per CTA (BN = 64 | 128 | 256).  TWO mode: the pair works on a 256 x 256 tile, each CTA on 128 of its rows; each
 // CTA loads its own A and HALF of B, and multicasts that half into both CTAs' rings, so B is read from L2 once per pair.  A ring stage
 // is refilled only when the consumers of both CTAs have released it.  Operands may be K-major or MN-major (wgrad / dgrad / P.V use the MN-major form so no
@@ -52,12 +56,16 @@ struct GemmParams {
     uint64_t pol_a, pol_b, pol_c;       // L2 eviction priorities of the three streams
 };
 
-template <int BN, bool TWO> struct GemmCfg {
+// EPI_WARPS: the epilogue runs on warps 1-3 from a whole BM x BN bf16 C tile in shared memory (bf16 C, EPI_PLAIN / EPI_LSE).
+// Otherwise the consumers stage 64-column chunks through two small buffers each.  The C tile costs BN = 256 its fourth ring stage.
+template <int BN, bool TWO, bool EPI_WARPS> struct GemmCfg {
     static constexpr int B_STAGE_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-    static constexpr int STAGES = BN == 256 ? 4 : (BN == 128 ? 6 : 8);
+    static constexpr int STAGES = BN == 256 ? (EPI_WARPS ? 3 : 4) : (BN == 128 ? 6 : 8);
     static constexpr int C_OFF = STAGES * STAGE_BYTES;
-    static constexpr int BAR_OFF = C_OFF + CONSUMERS * 2 * C_STAGE_BYTES;
+    static constexpr int C_BYTES = EPI_WARPS ? BM * BN * 2 : CONSUMERS * 2 * C_STAGE_BYTES;
+    static constexpr int BIAS_OFF = C_OFF + C_BYTES;                    // EPI_WARPS: the tile's BN bias values (f32)
+    static constexpr int BAR_OFF = BIAS_OFF + (EPI_WARPS ? BN * 4 : 0);
     static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;             // + barriers + alignment slack
     static constexpr int THREADS = 128 + CONSUMERS * 128;
     static constexpr int RELEASES = CONSUMERS * (TWO ? 2 : 1);         // arrivals that free a ring stage
@@ -93,13 +101,24 @@ template <int BN, bool A_MN, bool B_MN> PK_DEVICE void wgmma_tile(float (&acc)[B
 // EPI selects what the epilogue compiles in, so that the common case is straight-line code:
 //   EPI_PLAIN  alpha, bias, ReLU only      EPI_LSE  + per-row log-sum-exp partials (bf16 C)      EPI_FULL  + dropout / aux add / aux mask
 enum { EPI_PLAIN = 0, EPI_LSE = 1, EPI_FULL = 2 };
+// EPI_FULL and f32 C (wgrad, split-K reduce-add) keep the epilogue in the consumers: their K is long or they are off the joint's path,
+// so the tensor-pipe idle time it causes is small.
+template <bool CF32, int EPI> constexpr bool epi_warps() { return !CF32 && EPI != EPI_FULL; }
+
 template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI, bool TWO>
-__global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
-    using Cfg = GemmCfg<BN, TWO>;
+__global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
+    constexpr bool EW = epi_warps<CF32, EPI>();
+    static_assert(EPI != EPI_LSE || (EW && BN == 256), "the row log-sum-exp epilogue works on bf16 256-wide tiles");
+    using Cfg = GemmCfg<BN, TWO, EW>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
     uint64_t* empty_bar = full_bar + Cfg::STAGES;
+    // EW: the C tile is full (8 consumer warps have written it) / empty (3 epilogue warps have read it and staged the next bias)
+    uint64_t* c_full = empty_bar + Cfg::STAGES;
+    uint64_t* c_empty = c_full + 1;
+    const uint32_t ctile = smem_u32(smem + Cfg::C_OFF);                 // EW: [BN / 64][BM rows][128 B], TMA 128B swizzle
+    const uint32_t sbias = smem_u32(smem + Cfg::BIAS_OFF);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -116,6 +135,10 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full_bar[s], 1);              // the producer's expect_tx arrive
             mbar_init(&empty_bar[s], Cfg::RELEASES); // one arrive per consumer warpgroup (of both CTAs in TWO mode)
+        }
+        if (EW) {
+            mbar_init(c_full, CONSUMERS * 4);
+            mbar_init(c_empty, 3);
         }
         mbar_fence_init();
     }
@@ -191,6 +214,75 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
             }
         }
     }
+    if (EW && warp >= 1 && warp < 4) {
+        // ===================================================== epilogue warps: bias staging, TMA stores of the C tile, row LSE partials
+        const int et = threadIdx.x - 32;
+        const uint32_t store_pred = (threadIdx.x == 32) ? 1u : 0u;
+        uint32_t cph = 0;
+        for (int unit = worker; unit < num_units; unit += n_workers, cph ^= 1) {
+            const UnitCoord u = decode_unit(p, unit, out_tiles);
+            const int m0 = TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM, n0 = u.nb * BN;
+            // the consumers read the previous tile's bias before they marked C full, which this warp waited for
+            for (int c = et; c < BN; c += 96) sts_f32(sbias + c * 4, (p.bias != nullptr && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(c_empty);
+            mbar_wait(c_full, cph);
+#pragma unroll
+            for (int ch = 0; ch < BN / 64; ++ch)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (n0 + ch * 64 < p.N && m0 + h * 64 < p.M)
+                        tma_store_4d_hint_p(&p.c, smem + Cfg::C_OFF + ch * (BM * 128) + h * (64 * 128), n0 + ch * 64, m0 + h * 64, u.zb0, u.zb1,
+                                            p.pol_c, store_pred);
+            tma_store_commit_p(store_pred);
+            if constexpr (EPI == EPI_LSE) {
+                // (max * log2e, sum 2^(x * log2e - max)) of each row's rounded values, one max pass and one sum pass over shared memory.
+                // A lane pair shares a row: lane bit 0 picks the column half.  Rows go 16 per warp per round, so the last round is
+                // warp-uniform and the pair's merge can shuffle.  The two halves start 4 chunks apart: no bank conflicts.
+                constexpr float L2E = 1.4426950408889634f;
+                const int half = lane & 1;
+                const int nvalid = p.N - n0 - half * 128;                 // N % 8 == 0: a 16-byte chunk is valid as a whole
+                const int rot = half * 4;
+                for (int r = (et >> 5) * 16 + (lane >> 1); r < BM; r += 48) {
+                    const uint32_t rowa = ctile + half * (2 * BM * 128) + r * 128;
+                    uint32_t mx[4] = {0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u};   // bf16 -inf pairs
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int g = (j & 7) ^ rot;
+                        if ((j >> 3) * 64 + g * 8 < nvalid) {
+                            const uint4 v = lds_u32x4(rowa + (j >> 3) * (BM * 128) + ((g ^ (r & 7)) << 4));
+                            mx[0] = bf16x2_max(mx[0], v.x); mx[1] = bf16x2_max(mx[1], v.y);
+                            mx[2] = bf16x2_max(mx[2], v.z); mx[3] = bf16x2_max(mx[3], v.w);
+                        }
+                    }
+                    const uint32_t m2 = bf16x2_max(bf16x2_max(mx[0], mx[1]), bf16x2_max(mx[2], mx[3]));
+                    const float m = fmaxf(bf16lo(m2), bf16hi(m2)) * L2E;
+                    float s[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int g = (j & 7) ^ rot;
+                        if ((j >> 3) * 64 + g * 8 < nvalid) {
+                            const uint4 v = lds_u32x4(rowa + (j >> 3) * (BM * 128) + ((g ^ (r & 7)) << 4));
+                            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                            for (int q = 0; q < 4; ++q)
+                                s[q] += ex2_approx(fmaf(bf16lo(w[q]), L2E, -m)) + ex2_approx(fmaf(bf16hi(w[q]), L2E, -m));
+                        }
+                    }
+                    const float sum = (s[0] + s[1]) + (s[2] + s[3]);
+                    const float mo = __shfl_xor_sync(0xffffffffu, m, 1);
+                    const float so = __shfl_xor_sync(0xffffffffu, sum, 1);
+                    const float mm = fmaxf(m, mo);
+                    // a half (or tile) with no column below N is an empty partial (max = -inf, sum = 0), which the merges ignore
+                    const float st = (mm == -INFINITY) ? 0.f : sum * ex2_approx(m - mm) + so * ex2_approx(mo - mm);
+                    if (half == 0 && m0 + r < p.M)
+                        *reinterpret_cast<float2*>(p.row_lse + ((size_t)u.nb * (size_t)p.M + (size_t)(m0 + r)) * 2) = make_float2(mm, st);
+                }
+            }
+            tma_store_wait_read_p<0>(store_pred);      // the TMA has read the tile: the consumers may overwrite it
+        }
+        if (store_pred) tma_store_wait<0>();
+    }
     if (warp >= 4) {
     // ===================================================== consumers: MMA + epilogue for rows [wg * 64, wg * 64 + 64) of each tile
     setmaxnreg_inc<232>();
@@ -216,6 +308,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
     int stage = 0;
     uint32_t phase = 0;
     uint32_t chunk_ctr = 0;
+    uint32_t cph = 0;                                  // EW: parity of the C tile's barriers
     // a stage is released to this CTA's producer and, in TWO mode, to the peer's (whose multicast writes into this CTA's ring)
     auto release = [&](int s) {
         if (et == 0) { mbar_arrive(&empty_bar[s]); if (TWO) mbar_arrive_remote(&empty_bar[s], rank ^ 1u); }
@@ -243,7 +336,35 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
         wgmma_fence_acc(acc);
         if (prev >= 0) release(prev);
 
-        // ---------------------------------------------- epilogue
+        if constexpr (EW) {
+            // ------------------------------------------ alpha, bias, ReLU, RN to bf16 into the C tile; the epilogue warps take it from there
+            mbar_wait(c_empty, cph);
+            // stmatrix.x4 per pair of 8-column blocks (2q, 2q + 1): matrices (rows r0 | r0 + 8) x (block 2q | 2q + 1); lane -> row address
+            const int mi = lane >> 3;
+            const uint32_t row_addr = ctile + (uint32_t)(wg * 64 + w4 * 16 + (lane & 7) + ((mi & 1) << 3)) * 128;
+#pragma unroll
+            for (int q = 0; q < BN / 16; ++q) {
+                uint32_t r[4];
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int blk = 2 * q + i;
+                    const float2 bs = lds_f32x2(sbias + (blk * 8 + cq) * 4);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        r[2 * i + h] = pack_bf16x2(fmaxf(fmaf(acc[blk * 4 + 2 * h], p.alpha, bs.x), relu_floor),
+                                                   fmaxf(fmaf(acc[blk * 4 + 2 * h + 1], p.alpha, bs.y), relu_floor));
+                }
+                const int blk = 2 * q + (mi >> 1);
+                stmatrix_x4(row_addr + (blk >> 3) * (BM * 128) + (((blk & 7) ^ (lane & 7)) << 4), r[0], r[1], r[2], r[3]);
+            }
+            fence_proxy_async_smem();                  // the TMA store reads these bytes through the async proxy
+            __syncwarp();
+            if (lane == 0) mbar_arrive(c_full);
+            cph ^= 1;
+            continue;
+        }
+
+        // ---------------------------------------------- epilogue (EPI_FULL, f32 C)
         const int zb0 = u.zb0, zb1 = u.zb1;
         const int m0 = (TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM) + wg * 64;
         const int n0 = u.nb * BN;
@@ -259,7 +380,6 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
             }
             lin_row[h] = ((uint64_t)(zb1 * p.zb0 + zb0) * (uint64_t)p.M + (uint64_t)mrow[h]) * (uint64_t)p.N;
         }
-        float lse_m[2] = {-INFINITY, -INFINITY}, lse_s[2] = {0.f, 0.f};   // running row max (log2 units) and sum over this thread's columns
         constexpr int n_chunks = BN / CH;
 #pragma unroll
         for (int ch = 0; ch < n_chunks; ++ch) {
@@ -304,19 +424,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
                     if (CF32) {
                         *reinterpret_cast<float2*>(dst) = make_float2(x[0], x[1]);
                     } else {
-                        const uint32_t w = pack_bf16x2(x[0], x[1]);
-                        *reinterpret_cast<uint32_t*>(dst) = w;
-                        if (EPI == EPI_LSE) {
-                            // online log-sum-exp over the ROUNDED values (what the consumer of C will read); N % 8 == 0, so an 8-column
-                            // block is valid or invalid as a whole, and block 0 of a chunk is always valid (the running max is finite)
-                            const float kill = (ncol < p.N) ? 0.f : -INFINITY;
-                            const float v0 = bf16lo(w) + kill, v1 = bf16hi(w) + kill;
-                            const float m_new = fmaxf(lse_m[h], fmaxf(v0, v1) * 1.4426950408889634f);
-                            const float e0 = ex2_approx(fmaf(v0, 1.4426950408889634f, -m_new));
-                            const float e1 = ex2_approx(fmaf(v1, 1.4426950408889634f, -m_new));
-                            lse_s[h] = fmaf(lse_s[h], ex2_approx(lse_m[h] - m_new), e0 + e1);
-                            lse_m[h] = m_new;
-                        }
+                        *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(x[0], x[1]);
                     }
                 }
             }
@@ -327,25 +435,8 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO>::THREADS, 1) gemm_wgmma_kerne
             tma_store_commit_p(store_pred);
             ++chunk_ctr;
         }
-        if (!CF32 && EPI == EPI_LSE) {
-            // merge the four column partials of each row (the quad of lanes that share it); a tile whose columns lie entirely beyond N
-            // contributes an empty partial (max = -inf, sum = 0), which the merge on the consumer side ignores
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-#pragma unroll
-                for (int o = 1; o <= 2; o <<= 1) {
-                    const float mo = __shfl_xor_sync(0xffffffffu, lse_m[h], o);
-                    const float so = __shfl_xor_sync(0xffffffffu, lse_s[h], o);
-                    const float mm = fmaxf(lse_m[h], mo);
-                    lse_s[h] = (mm == -INFINITY) ? 0.f : lse_s[h] * ex2_approx(lse_m[h] - mm) + so * ex2_approx(mo - mm);
-                    lse_m[h] = mm;
-                }
-                if ((lane & 3) == 0 && mrow[h] < p.M)
-                    *reinterpret_cast<float2*>(p.row_lse + ((size_t)u.nb * (size_t)p.M + (size_t)mrow[h]) * 2) = make_float2(lse_m[h], lse_s[h]);
-            }
-        }
     }
-    if (store_pred) tma_store_wait<0>();
+    if (!EW && store_pred) tma_store_wait<0>();
     }
     // the peer may still arrive on this CTA's barriers: neither CTA of a pair leaves before both are done
     if (TWO) cluster_sync_all();
@@ -426,7 +517,7 @@ int encode_tiled_bf16_3d(CUtensorMap* out, const void* ptr, const unsigned long 
 
 template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI, bool TWO>
 static int launch_gemm_e(const GemmParams& gp, int workers, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, TWO>;
+    using Cfg = GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>;
     auto kern = gemm_wgmma_kernel<A_MN, B_MN, BN, CF32, EPI, TWO>;
     static bool configured = false;
     if (!configured) {
@@ -444,6 +535,19 @@ static int launch_gemm_e(const GemmParams& gp, int workers, cudaStream_t stream)
         attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
+        // a GPC whose SM count is odd cannot host a pair on every SM: launch no more persistent pairs than can be resident at once,
+        // or the extra ones would run as a second wave after the others finished all their tiles
+        static int max_pairs = -1;
+        if (max_pairs < 0) {
+            int n = 0;
+            PK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+            PK_CHECK_ARG(n > 0, "gemm: no 2-CTA cluster of the pair kernel fits on this device");
+            max_pairs = n;
+        }
+        if (workers > max_pairs) {
+            workers = max_pairs;
+            cfg.gridDim = dim3(2 * workers);
+        }
         PK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, gp));
     } else {
         kern<<<workers, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(gp);
@@ -491,8 +595,9 @@ struct GemmPlan { int bn; bool two; };
 static GemmPlan plan_gemm(long long M, long long N, int block_n, int two_sm_req) {
     GemmPlan pl;
     pl.bn = block_n ? block_n : (N <= 64 ? 64 : (N <= 128 ? 128 : 256));
-    // PK_GEMM_2SM=1 lets the automatic choice pick the pair kernel.  Off by default: on an H100 (400 W limit) it made the joint's fc2
-    // forward 45.3 ms against 37.8 ms on single CTAs and the train step 201 ms against 174 ms (bench.py, B=32, T=1000, U=150, V=6000)
+    // PK_GEMM_2SM=1 lets the automatic choice pick the pair kernel.  Off by default: on an H100 80GB HBM3 (700 W limit), with the
+    // epilogue on its own warps, it took 31.2 ms on the joint's fc2 forward with row LSE against 28.0 ms on single CTAs, 27.5 against
+    // 20.6 ms on the fc2 dgrad and 34.8 against 20.9 ms on the fc2 wgrad (scripts/gemm_lab.py fc2, one run each)
     static int use_2sm = -1;
     if (use_2sm < 0) use_2sm = env_int("PK_GEMM_2SM", 0);
     static int min_tiles = -1;               // smallest number of 256 x 256 tiles handed to the pair kernel
