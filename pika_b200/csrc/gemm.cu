@@ -2,13 +2,14 @@
 //
 // One persistent CTA per SM (ONE mode) or one 2-CTA cluster per pair of SMs (TWO mode), three warpgroups per CTA:
 //   warp 0           TMA producer   (one converged warp: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warps 1-3        epilogue       (bf16 C with the plain or LSE epilogue: take the finished C tile from shared memory, compute the
-//                                    row log-sum-exp partials, TMA-store it, hand it back; stage the next tile's bias)
+//   warps 1-3        epilogue       (bf16 C with the plain or LSE epilogue: TMA-store the finished C tile from shared memory, hand it
+//                                    back; stage the next tile's bias)
 //   warpgroups 1, 2  consumers      (wgmma m64 x BN x k16 from shared-memory descriptors, fp32 accumulators in registers; each
 //                                    owns 64 rows of the 128-row tile, releases ring stages one k-block behind.  bf16 plain / LSE:
 //                                    alpha, bias, ReLU, bf16 rounding into the C tile with stmatrix, then straight on to the next
-//                                    tile's main loop.  EPI_FULL and f32 C: the whole epilogue, registers -> swizzled smem -> TMA store /
-//                                    TMA reduce-add, in 64-column chunks)
+//                                    tile's main loop.  LSE: the row max comes from the registers being rounded; the exp-sum reads the
+//                                    warp's own rows of the C tile back while the next tile's wgmma run.  EPI_FULL and f32 C: the whole
+//                                    epilogue, registers -> swizzled smem -> TMA store / TMA reduce-add, in 64-column chunks)
 // Tile 128 x BN x 64 per CTA (BN = 64 | 128 | 256).  TWO mode: the pair works on a 256 x 256 tile, each CTA on 128 of its rows; each
 // CTA loads its own A and HALF of B, and multicasts that half into both CTAs' rings, so B is read from L2 once per pair.  A ring stage
 // is refilled only when the consumers of both CTAs have released it.  Operands may be K-major or MN-major (wgrad / dgrad / P.V use the MN-major form so no
@@ -56,7 +57,7 @@ struct GemmParams {
     uint64_t pol_a, pol_b, pol_c;       // L2 eviction priorities of the three streams
 };
 
-// EPI_WARPS: the epilogue runs on warps 1-3 from a whole BM x BN bf16 C tile in shared memory (bf16 C, EPI_PLAIN / EPI_LSE).
+// EPI_WARPS: warps 1-3 TMA-store a whole BM x BN bf16 C tile from shared memory (bf16 C, EPI_PLAIN / EPI_LSE).
 // Otherwise the consumers stage 64-column chunks through two small buffers each.  The C tile costs BN = 256 its fourth ring stage.
 template <int BN, bool TWO, bool EPI_WARPS> struct GemmCfg {
     static constexpr int B_STAGE_BYTES = BN * BK * 2;
@@ -114,7 +115,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
     uint64_t* empty_bar = full_bar + Cfg::STAGES;
-    // EW: the C tile is full (8 consumer warps have written it) / empty (3 epilogue warps have read it and staged the next bias)
+    // EW: the C tile is full (8 consumer warps have written it) / empty (its TMA store has read it, the epilogue warps have staged the next bias)
     uint64_t* c_full = empty_bar + Cfg::STAGES;
     uint64_t* c_empty = c_full + 1;
     const uint32_t ctile = smem_u32(smem + Cfg::C_OFF);                 // EW: [BN / 64][BM rows][128 B], TMA 128B swizzle
@@ -215,7 +216,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         }
     }
     if (EW && warp >= 1 && warp < 4) {
-        // ===================================================== epilogue warps: bias staging, TMA stores of the C tile, row LSE partials
+        // ===================================================== epilogue warps: bias staging, TMA stores of the C tile
         const int et = threadIdx.x - 32;
         const uint32_t store_pred = (threadIdx.x == 32) ? 1u : 0u;
         uint32_t cph = 0;
@@ -235,50 +236,6 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
                         tma_store_4d_hint_p(&p.c, smem + Cfg::C_OFF + ch * (BM * 128) + h * (64 * 128), n0 + ch * 64, m0 + h * 64, u.zb0, u.zb1,
                                             p.pol_c, store_pred);
             tma_store_commit_p(store_pred);
-            if constexpr (EPI == EPI_LSE) {
-                // (max * log2e, sum 2^(x * log2e - max)) of each row's rounded values, one max pass and one sum pass over shared memory.
-                // A lane pair shares a row: lane bit 0 picks the column half.  Rows go 16 per warp per round, so the last round is
-                // warp-uniform and the pair's merge can shuffle.  The two halves start 4 chunks apart: no bank conflicts.
-                constexpr float L2E = 1.4426950408889634f;
-                const int half = lane & 1;
-                const int nvalid = p.N - n0 - half * 128;                 // N % 8 == 0: a 16-byte chunk is valid as a whole
-                const int rot = half * 4;
-                for (int r = (et >> 5) * 16 + (lane >> 1); r < BM; r += 48) {
-                    const uint32_t rowa = ctile + half * (2 * BM * 128) + r * 128;
-                    uint32_t mx[4] = {0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u};   // bf16 -inf pairs
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int g = (j & 7) ^ rot;
-                        if ((j >> 3) * 64 + g * 8 < nvalid) {
-                            const uint4 v = lds_u32x4(rowa + (j >> 3) * (BM * 128) + ((g ^ (r & 7)) << 4));
-                            mx[0] = bf16x2_max(mx[0], v.x); mx[1] = bf16x2_max(mx[1], v.y);
-                            mx[2] = bf16x2_max(mx[2], v.z); mx[3] = bf16x2_max(mx[3], v.w);
-                        }
-                    }
-                    const uint32_t m2 = bf16x2_max(bf16x2_max(mx[0], mx[1]), bf16x2_max(mx[2], mx[3]));
-                    const float m = fmaxf(bf16lo(m2), bf16hi(m2)) * L2E;
-                    float s[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int g = (j & 7) ^ rot;
-                        if ((j >> 3) * 64 + g * 8 < nvalid) {
-                            const uint4 v = lds_u32x4(rowa + (j >> 3) * (BM * 128) + ((g ^ (r & 7)) << 4));
-                            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                            for (int q = 0; q < 4; ++q)
-                                s[q] += ex2_approx(fmaf(bf16lo(w[q]), L2E, -m)) + ex2_approx(fmaf(bf16hi(w[q]), L2E, -m));
-                        }
-                    }
-                    const float sum = (s[0] + s[1]) + (s[2] + s[3]);
-                    const float mo = __shfl_xor_sync(0xffffffffu, m, 1);
-                    const float so = __shfl_xor_sync(0xffffffffu, sum, 1);
-                    const float mm = fmaxf(m, mo);
-                    // a half (or tile) with no column below N is an empty partial (max = -inf, sum = 0), which the merges ignore
-                    const float st = (mm == -INFINITY) ? 0.f : sum * ex2_approx(m - mm) + so * ex2_approx(mo - mm);
-                    if (half == 0 && m0 + r < p.M)
-                        *reinterpret_cast<float2*>(p.row_lse + ((size_t)u.nb * (size_t)p.M + (size_t)(m0 + r)) * 2) = make_float2(mm, st);
-                }
-            }
             tma_store_wait_read_p<0>(store_pred);      // the TMA has read the tile: the consumers may overwrite it
         }
         if (store_pred) tma_store_wait<0>();
@@ -313,6 +270,44 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
     auto release = [&](int s) {
         if (et == 0) { mbar_arrive(&empty_bar[s]); if (TWO) mbar_arrive_remote(&empty_bar[s], rank ^ 1u); }
     };
+    // EPI_LSE: (max * log2e, sum 2^(x * log2e - max)) of each row's rounded values.  The max is taken in registers while the tile is
+    // rounded; the sum of the tile the warp wrote last is read back from its own 16 rows of the C tile in LSE_SLICES slices, one
+    // per k-block of the next tile while its wgmma run (the rest after that main loop; a worker's last tile after its unit loop).
+    // Those reads come before the warp's stmatrix of the next tile in program order, and the TMA store only reads: no barrier
+    // beyond a __syncwarp is needed before the C tile is overwritten.  Lane quad lane / 4 owns rows r0 and r0 + 8 as in the
+    // accumulators; slice t is one 16-byte chunk of row r0 + 8 * (t >> 3), 64-column block (t >> 1) & 3, chunk 2 * (lane & 3) +
+    // (t & 1): each quarter warp reads all eight chunk positions of the swizzled rows, so the 16-byte loads are conflict-free.
+    constexpr float L2E = 1.4426950408889634f;
+    constexpr int LSE_SLICES = BN / 16;                // 16 rows x BN columns of bf16 over 32 lanes, 16 B each
+    bool lse_pending = false;                          // the previous tile's sums are still to be taken
+    float lse_m0 = 0.f, lse_m1 = 0.f, lse_s0 = 0.f, lse_s1 = 0.f;
+    int lse_row = 0, lse_nb = 0, lse_nvalid = 0;       // global row of r0, N tile, valid columns of the pending tile
+    const uint32_t lse_addr = ctile + (uint32_t)(wg * 64 + r0) * 128;
+    auto lse_slice = [&](int t) {
+        const int j = (t >> 1) & 3, g = (lane & 3) * 2 + (t & 1);
+        if (j * 64 + g * 8 < lse_nvalid) {             // N % 8 == 0: a 16-byte chunk is valid as a whole
+            const bool hi = (t >> 3) != 0;
+            const uint4 v = lds_u32x4(lse_addr + (hi ? 8 * 128 : 0) + j * (BM * 128) + ((g ^ (lane >> 2)) << 4));
+            const float nm = hi ? -lse_m1 : -lse_m0;
+            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+            float s = 0.f;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) s += ex2_approx(fmaf(bf16lo(w[q]), L2E, nm)) + ex2_approx(fmaf(bf16hi(w[q]), L2E, nm));
+            if (hi) lse_s1 += s; else lse_s0 += s;
+        }
+    };
+    auto lse_finish = [&]() {
+        lse_s0 += __shfl_xor_sync(0xffffffffu, lse_s0, 1);
+        lse_s1 += __shfl_xor_sync(0xffffffffu, lse_s1, 1);
+        lse_s0 += __shfl_xor_sync(0xffffffffu, lse_s0, 2);
+        lse_s1 += __shfl_xor_sync(0xffffffffu, lse_s1, 2);
+        // a tile with no column below N is an empty partial (max = -inf, sum = 0), which the merges ignore
+        float* dst = p.row_lse + ((size_t)lse_nb * (size_t)p.M + (size_t)lse_row) * 2;
+        if ((lane & 3) == 0 && lse_row < p.M) *reinterpret_cast<float2*>(dst) = make_float2(lse_m0, lse_m0 == -INFINITY ? 0.f : lse_s0);
+        if ((lane & 3) == 0 && lse_row + 8 < p.M)
+            *reinterpret_cast<float2*>(dst + 16) = make_float2(lse_m1, lse_m1 == -INFINITY ? 0.f : lse_s1);
+        lse_pending = false;
+    };
     for (int unit = worker; unit < num_units; unit += n_workers) {
         const UnitCoord u = decode_unit(p, unit, out_tiles);
         const int k_iters = min(k_iters_total, (u.split + 1) * p.iters_per_split) - u.split * p.iters_per_split;
@@ -329,6 +324,10 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
             wgmma_fence_acc(acc);
             wgmma_wait<1>();                           // the previous k-block's products are done: its stage may be refilled
             if (prev >= 0) release(prev);
+            // after the release, not before the wait: with a 3-stage ring, a stage handed back late stalls its refill
+            if constexpr (EPI == EPI_LSE) {
+                if (lse_pending && k < LSE_SLICES) lse_slice(k);
+            }
             prev = stage;
             if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
         }
@@ -337,8 +336,19 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         if (prev >= 0) release(prev);
 
         if constexpr (EW) {
+            if constexpr (EPI == EPI_LSE) {
+                if (lse_pending) {
+                    for (int t = k_iters; t < LSE_SLICES; ++t) lse_slice(t);
+                    lse_finish();
+                }
+            }
             // ------------------------------------------ alpha, bias, ReLU, RN to bf16 into the C tile; the epilogue warps take it from there
             mbar_wait(c_empty, cph);
+            // LSE: every lane's reads of the previous tile come before any lane's stmatrix below.  Nothing else orders them: c_empty
+            // only says that the TMA store has read the tile.
+            if constexpr (EPI == EPI_LSE) __syncwarp();
+            const int nvalid = p.N - u.nb * BN;
+            uint32_t mx[2] = {0xFF80FF80u, 0xFF80FF80u};  // LSE: bf16 -inf pairs, the running max of rows r0 and r0 + 8
             // stmatrix.x4 per pair of 8-column blocks (2q, 2q + 1): matrices (rows r0 | r0 + 8) x (block 2q | 2q + 1); lane -> row address
             const int mi = lane >> 3;
             const uint32_t row_addr = ctile + (uint32_t)(wg * 64 + w4 * 16 + (lane & 7) + ((mi & 1) << 3)) * 128;
@@ -353,14 +363,30 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
                     for (int h = 0; h < 2; ++h)
                         r[2 * i + h] = pack_bf16x2(fmaxf(fmaf(acc[blk * 4 + 2 * h], p.alpha, bs.x), relu_floor),
                                                    fmaxf(fmaf(acc[blk * 4 + 2 * h + 1], p.alpha, bs.y), relu_floor));
+                    // columns >= N hold zeros from the zero-filled B rows, not logits
+                    if (EPI == EPI_LSE && blk * 8 < nvalid) { mx[0] = bf16x2_max(mx[0], r[2 * i]); mx[1] = bf16x2_max(mx[1], r[2 * i + 1]); }
                 }
                 const int blk = 2 * q + (mi >> 1);
                 stmatrix_x4(row_addr + (blk >> 3) * (BM * 128) + (((blk & 7) ^ (lane & 7)) << 4), r[0], r[1], r[2], r[3]);
             }
             fence_proxy_async_smem();                  // the TMA store reads these bytes through the async proxy
-            __syncwarp();
+            __syncwarp();                              // LSE: and so does this warp's exp-sum, from other lanes' stmatrix
             if (lane == 0) mbar_arrive(c_full);
             cph ^= 1;
+            if constexpr (EPI == EPI_LSE) {
+                // max is exact and x * log2e is monotonic: the same m as a max over the rounded tile in shared memory
+                float x0 = fmaxf(bf16lo(mx[0]), bf16hi(mx[0])), x1 = fmaxf(bf16lo(mx[1]), bf16hi(mx[1]));
+                x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 1));
+                x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 1));
+                x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, 2));
+                x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
+                lse_m0 = x0 * L2E; lse_m1 = x1 * L2E;
+                lse_s0 = 0.f; lse_s1 = 0.f;
+                lse_row = (TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM) + wg * 64 + r0;
+                lse_nb = u.nb;
+                lse_nvalid = nvalid;
+                lse_pending = true;
+            }
             continue;
         }
 
@@ -434,6 +460,13 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
             else tma_store_4d_hint_p(&p.c, sbuf, nc0, m0, zb0, zb1, p.pol_c, store_pred);
             tma_store_commit_p(store_pred);
             ++chunk_ctr;
+        }
+    }
+    if constexpr (EPI == EPI_LSE) {                    // the last tile has no next main loop to hide its sums in
+        if (lse_pending) {
+#pragma unroll
+            for (int t = 0; t < LSE_SLICES; ++t) lse_slice(t);
+            lse_finish();
         }
     }
     if (!EW && store_pred) tma_store_wait<0>();
