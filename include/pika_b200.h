@@ -304,13 +304,25 @@ int pk_beam_advance_lm(const float* logits, int ldv, const float* row_lse, float
  *   fwd: gx f32 [B,U,4H] = x W_ih^T + b_ih + b_hh; w_hh bf16 [4H,H]; out [B,U,H] (f32|bf16);
  *        gates_save f32 [U,B,4H], cs f32 [U,B,H] are kept for the backward.
  *   bwd: dout [B,U,H] -> dG bf16 [U,B,4H] (gradient w.r.t. the pre-activation gates, time-major).
- *   ws : pk_lstm_seq_workspace_bytes(H) bytes of scratch (grid barrier + hidden-state exchange).
+ *   ws : pk_lstm_seq_workspace_bytes(H) bytes of zero-initialised scratch (grid barrier + hidden-state exchange).
  */
 long long pk_lstm_seq_workspace_bytes(int H);
 int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, float* gates_save, float* cs, int B,
                     int U, int H, void* ws, void* stream);
 int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const float* cs, const void* w_hh_bf16, void* dG_bf16,
                     int B, int U, int H, void* ws, void* stream);
+/* Ragged, (bi)directional form (the LSTM encoder over pack_padded_sequence batches; trainer/model/transducer.py:38-44,82-86).
+ * n_dir = 2 runs both directions of a bidirectional layer in one launch of 2 * H/8 CTAs; n_dir = 1 with reverse = 1 runs one
+ * direction backwards in time.  Per direction d (buffers stacked along a leading n_dir axis): gx f32 [B,U,4H], w_hh bf16 [4H,H],
+ * gates_save f32 [U,B,4H], cs f32 [U,B,H], dG bf16 [U,B,4H]; out / dout [B,U,ldo], direction d at columns [d*H, (d+1)*H).
+ * lens: int32 [B] on the device, or NULL (every sequence runs all U steps).  Sequence b with length L_b is processed at
+ * t = s (forward) or t = L_b - 1 - s (reverse) for steps s < L_b, from a zero state; the kernel runs max_b L_b steps.
+ * Outputs and dG rows at t >= L_b are written as zeros.  ws: pk_lstm_seq_workspace_bytes(n_dir * H) bytes, zero-initialised.
+ * pk_lstm_seq_fwd / _bwd are the lens = NULL, n_dir = 1, reverse = 0, ldo = H case. */
+int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, int ldo, float* gates_save, float* cs,
+                       const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream);
+int pk_lstm_seq_bwd_ex(const void* dout, int dtype, int ldo, const float* gates_save, const float* cs, const void* w_hh_bf16,
+                       void* dG_bf16, const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * MBR training step helpers (trainer/train_transducer_mbr_bmuf_otfaug.py:197-235): the joint is evaluated only

@@ -1,7 +1,8 @@
 // Persistent LSTM layer kernels: the whole time recurrence (forward, and back-propagation through time)
 // runs inside ONE cooperative launch instead of two launches per step.
 //
-// Replaces cuDNN's nn.LSTM recurrence (trainer/model/transducer.py:56-61,95) for the prediction net.
+// Replaces cuDNN's nn.LSTM recurrence for the prediction net (trainer/model/transducer.py:56-61,95) and for the LSTM encoder
+// (:38-44,82-86): ragged lengths (packed sequences), reverse direction, and both directions of a layer in one launch.
 //
 // Work split: the hidden units are sharded across the CTAs (HJ = 8 units per CTA -> H/8 = 128 CTAs for
 // H = 1024, one per SM).  A CTA keeps its slice of the recurrent weights resident in shared memory for all U
@@ -60,11 +61,13 @@ PK_DEVICE void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "
 // they remove) -- the hardware cluster barrier gathers the cn CTAs of a cluster, ONE
 // thread per cluster does the mode-1 handshake on the global counter (128 -> 16 serialised atomics on one line), a second cluster
 // barrier releases the peers.  Causality chains through the cluster-scope and gpu-scope release/acquire pairs.  PK_LSTM_BARRIER selects.
-PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, int mode, uint32_t cn, uint32_t cr) {
+// ``nct`` = CTAs that meet at this barrier: the CTAs of one direction (a bidirectional launch keeps one counter per direction, so
+// the two recurrences never wait on each other).
+PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, int mode, uint32_t cn, uint32_t cr, unsigned int nct) {
     if (mode == 3 && cn > 1) {
         cluster_sync_all();
         if (cr == 0 && threadIdx.x == 0) {
-            const unsigned int target = (gridDim.x / cn) * step_index;
+            const unsigned int target = (nct / cn) * step_index;
             asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
             unsigned int seen;
             do {
@@ -74,7 +77,7 @@ PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, int 
         cluster_sync_all();
         return;
     }
-    const unsigned int target = gridDim.x * step_index;
+    const unsigned int target = nct * step_index;
     __syncthreads();
     if (threadIdx.x == 0) {
         if (mode == 0) {
@@ -95,13 +98,50 @@ PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, int 
 }
 PK_DEVICE float sigm(float x) { return 1.f / (1.f + __expf(-x)); }
 
+// Per-launch sequence lengths into len_s[32] (rows >= B get 0; lens == NULL: every row runs all U steps, clamped to [0, U]);
+// returns the number of steps of this launch, max_b L_b.  Called by every thread before the first __syncthreads.
+PK_DEVICE void load_lens(const int* lens, int B, int U, int* len_s, int* steps_s) {
+    if (threadIdx.x < 32) {
+        int L = 0;
+        if ((int)threadIdx.x < B) L = lens ? min(max(lens[threadIdx.x], 0), U) : U;
+        len_s[threadIdx.x] = L;
+        int m = L;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if (threadIdx.x == 0) *steps_s = m;
+    }
+}
+
+// Directions.  A launch of n_dir * H/8 CTAs runs n_dir independent recurrences: CTAs [d*H/8, (d+1)*H/8) are direction d, with
+// their own W_hh block, gate buffers, exchange buffer and barrier counter (clusters never straddle two directions: the cluster
+// size divides H/8).  Direction 1 of a bidirectional launch, or a single-direction launch with ``reverse`` set, runs backwards in
+// time: sequence b with length L_b processes step s at time t = L_b - 1 - s.  The forward direction processes t = s.  Both run only
+// while s < L_b, from a zero state.
+struct LsDir {
+    int d;          // buffer index (0 .. n_dir-1)
+    bool rev;       // runs backwards in time
+    int j0;         // first hidden unit of this CTA
+    unsigned nct;   // CTAs of this direction
+};
+PK_DEVICE LsDir ls_dir(int H, int reverse) {
+    LsDir r;
+    r.nct = (unsigned)(H / LS_HJ);
+    r.d = (int)(blockIdx.x / r.nct);
+    r.rev = gridDim.x > r.nct ? r.d == 1 : reverse != 0;
+    r.j0 = (int)(blockIdx.x - r.d * r.nct) * LS_HJ;
+    return r;
+}
+
 // ------------------------------------------------------------------------------------------ forward
-// gx [B,U,4H] f32 (input projection + both biases); w_hh bf16 [4H,H]; out (T) [B,U,H]; hx bf16 [2,32,H] exchange;
-// gates_save f32 [U,B,4H] (post-activation i,f,g,o), cs f32 [U,B,H].
+// Per direction d: gx [B,U,4H] f32 (input projection + both biases); w_hh bf16 [4H,H]; out (T) [B,U,ldo], columns [d*H, (d+1)*H);
+// hx bf16 [2,32,H] exchange; gates_save f32 [U,B,4H] (post-activation i,f,g,o), cs f32 [U,B,H]; the n_dir blocks of gx, w_hh,
+// gates_save, cs and hx are stacked, and the barrier counters are 128 B apart.  Outputs at t >= L_b are written as exact zeros;
+// gates_save / cs at those positions are left untouched.
 template <typename T>
 __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float* __restrict__ gx, const __nv_bfloat16* __restrict__ w_hh,
-                                                                     T* __restrict__ out, __nv_bfloat16* hx, float* __restrict__ gates_save,
-                                                                     float* __restrict__ cs, int B, int Bt, int U, int H, unsigned int* counter, int bar_mode) {
+                                                                     T* __restrict__ out, int ldo, __nv_bfloat16* hx, float* __restrict__ gates_save,
+                                                                     float* __restrict__ cs, const int* __restrict__ lens, int B, int Bt, int U,
+                                                                     int H, int reverse, unsigned int* counter, int bar_mode) {
     // B = sequences of this launch (<= 32); Bt = sequences of the whole batch: gates_save / cs are time-major [U, Bt, .] and the
     // caller passes them already offset to this launch's first sequence (batches larger than 32 run as independent launches)
     extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -110,7 +150,17 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float
     __nv_bfloat16* h_s = w_s + 32 * P;                                           // [32][P]: h_{t-1}
     float* g_s = reinterpret_cast<float*>(h_s + 32 * P);                         // [32][33]
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int j0 = blockIdx.x * LS_HJ;
+    const LsDir dir = ls_dir(H, reverse);
+    const int j0 = dir.j0;
+    gx += (long long)dir.d * Bt * U * 4 * H;
+    w_hh += (long long)dir.d * 4 * H * H;
+    out += dir.d * H;
+    hx += (long long)dir.d * 2 * LS_MB * H;
+    gates_save += (long long)dir.d * U * Bt * 4 * H;
+    cs += (long long)dir.d * U * Bt * H;
+    counter += dir.d * 32;
+    __shared__ int len_s[LS_MB], steps_s;
+    load_lens(lens, B, U, len_s, &steps_s);
     const int vec_per_row = H / 8;
     for (int i = tid; i < 32 * vec_per_row; i += LS_THREADS) {
         const int r = i / vec_per_row, v = i - r * vec_per_row;
@@ -128,18 +178,21 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float
     const uint16_t cmask = (uint16_t)((1u << cn) - 1u);
     __syncthreads();
     if (cn > 1) cluster_sync_all();                                              // every peer's barrier exists before the first multicast
-    for (int t = 0; t < U; ++t) {
+    const int S = steps_s, L = len_s[cb];
+    for (int s = 0; s < S; ++s) {
+        const bool active = s < L;
+        const int t = dir.rev ? L - 1 - s : s;                                   // this row's time at step s
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
         // this step's input-projection terms do not depend on h_{t-1}: fetch them now so that their L2 / HBM latency hides behind the
         // all-gather and the product instead of sitting on the step's critical path
         float gx_i = 0.f, gx_f = 0.f, gx_g = 0.f, gx_o = 0.f;
-        if (cb < B) {
+        if (active) {
             const float* gxr = gx + ((long long)cb * U + t) * 4 * H + j0 + cj;
             gx_i = __ldg(gxr); gx_f = __ldg(gxr + H); gx_g = __ldg(gxr + 2 * H); gx_o = __ldg(gxr + 3 * H);
         }
-        if (t > 0) {
-            // all-gather of h_{t-1} (32 x H bf16) from L2 by the TMA engine: lane r of warp 0 copies row r
-            const __nv_bfloat16* src = hx + (long long)((t - 1) & 1) * LS_MB * H;
+        if (s > 0) {
+            // all-gather of the previous step's h (32 x H bf16) from L2 by the TMA engine: lane r of warp 0 copies row r
+            const __nv_bfloat16* src = hx + (long long)((s - 1) & 1) * LS_MB * H;
             // the CTAs of a cluster share the gather: each fetches 32 / cn of the rows and multicasts them to all cn (one L2 read per
             // cluster instead of one per CTA -- with 128 CTAs pulling the same 64 KB every step the L2 was the bottleneck)
             if (warp == 0) {
@@ -178,32 +231,38 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float
         g_s[(mt * 16 + g + 8) * 33 + nt * 8 + 2 * tq + 1] = acc[3];
         __syncthreads();
         // fused cell for (cb, j0 + cj); local gate rows: i = cj, f = 8 + cj, g = 16 + cj, o = 24 + cj
-        if (cb < B) {
+        if (active) {
             const float gi = sigm(g_s[cb * 33 + cj] + gx_i);
             const float gf = sigm(g_s[cb * 33 + 8 + cj] + gx_f);
             const float gg = tanhf(g_s[cb * 33 + 16 + cj] + gx_g);
             const float go = sigm(g_s[cb * 33 + 24 + cj] + gx_o);
             c_state = gf * c_state + gi * gg;
             const float hv = go * tanhf(c_state);
-            out[((long long)cb * U + t) * H + j0 + cj] = from_f32<T>(hv);
-            hx[(long long)(t & 1) * LS_MB * H + (long long)cb * H + j0 + cj] = __float2bfloat16_rn(hv);
+            out[((long long)cb * U + t) * ldo + j0 + cj] = from_f32<T>(hv);
+            hx[(long long)(s & 1) * LS_MB * H + (long long)cb * H + j0 + cj] = __float2bfloat16_rn(hv);
             float* gs = gates_save + ((long long)t * Bt + cb) * 4 * H + j0 + cj;
             gs[0] = gi; gs[H] = gf; gs[2 * H] = gg; gs[3 * H] = go;
             cs[((long long)t * Bt + cb) * H + j0 + cj] = c_state;
         } else {
-            hx[(long long)(t & 1) * LS_MB * H + (long long)cb * H + j0 + cj] = __float2bfloat16_rn(0.f);
+            hx[(long long)(s & 1) * LS_MB * H + (long long)cb * H + j0 + cj] = __float2bfloat16_rn(0.f);
+            if (cb < B) out[((long long)cb * U + s) * ldo + j0 + cj] = from_f32<T>(0.f);      // s >= L_b: a padded position
         }
-        if (t + 1 < U) grid_barrier(counter, (unsigned int)(t + 1), bar_mode, cn, cr);
+        if (s + 1 < S) grid_barrier(counter, (unsigned int)(s + 1), bar_mode, cn, cr, dir.nct);
     }
+    if (cb < B)
+        for (int t = S; t < U; ++t) out[((long long)cb * U + t) * ldo + j0 + cj] = from_f32<T>(0.f);     // past this launch's longest sequence
 }
 
 // ------------------------------------------------------------------------------------------ backward
-// dout (T) [B,U,H]; gates_save, cs as saved by the forward; w_hh bf16 [4H,H];
-// dG bf16 [U,B,4H] (gradient w.r.t. the pre-activation gates, time-major: feeds dW_ih / dW_hh / dx GEMMs).
+// Per direction d: dout (T) [B,U,ldo], columns [d*H, (d+1)*H); gates_save, cs as saved by the forward; w_hh bf16 [4H,H];
+// dG bf16 [U,B,4H] (gradient w.r.t. the pre-activation gates, time-major: feeds dW_ih / dW_hh / dx GEMMs).  Rows of dG at
+// t >= L_b are written as zeros, so those GEMMs run over all U x B rows unmasked.  zrow: 4H zero bf16 values, the recurrent
+// input of a sequence's first backward step.
 template <typename T>
-__global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __restrict__ dout, const float* __restrict__ gates_save,
+__global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __restrict__ dout, int ldo, const float* __restrict__ gates_save,
                                                                      const float* __restrict__ cs, const __nv_bfloat16* __restrict__ w_hh,
-                                                                     __nv_bfloat16* dG, int B, int Bt, int U, int H, unsigned int* counter, int bar_mode) {
+                                                                     __nv_bfloat16* dG, const __nv_bfloat16* zrow, const int* __restrict__ lens,
+                                                                     int B, int Bt, int U, int H, int reverse, unsigned int* counter, int bar_mode) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
     const int G4 = 4 * H;
     const int PW = G4 + LS_PAD;                                                  // Wt_s pitch
@@ -214,7 +273,16 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __
     float* r_s = reinterpret_cast<float*>(d_s + 2 * 32 * PD);                    // [32][9] dh_rec
     __shared__ __align__(8) uint64_t q_bar[2];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int j0 = blockIdx.x * LS_HJ;
+    const LsDir dir = ls_dir(H, reverse);
+    const int j0 = dir.j0;
+    dout += dir.d * H;
+    gates_save += (long long)dir.d * U * Bt * G4;
+    cs += (long long)dir.d * U * Bt * H;
+    w_hh += (long long)dir.d * G4 * H;
+    dG += (long long)dir.d * U * Bt * G4;
+    counter += dir.d * 32;
+    __shared__ int len_s[LS_MB], steps_s;
+    load_lens(lens, B, U, len_s, &steps_s);
     for (int i = tid; i < G4 * LS_HJ; i += LS_THREADS) {
         const int r = i / LS_HJ, jj = i - r * LS_HJ;
         wt_s[jj * PW + r] = w_hh[(long long)r * H + j0 + jj];
@@ -230,27 +298,40 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __
     const uint16_t cmask = (uint16_t)((1u << cn) - 1u);
     __syncthreads();
     if (cn > 1) cluster_sync_all();                                              // every peer's barriers exist before the first multicast
-    for (int t = U - 1; t >= 0; --t) {
+    const int S = steps_s, L = len_s[cb];
+    if (cb < B)
+        for (int t = S; t < U; ++t) {                                            // past this launch's longest sequence
+            __nv_bfloat16* d = dG + ((long long)t * Bt + cb) * G4 + j0 + cj;
+            d[0] = d[H] = d[2 * H] = d[3 * H] = __float2bfloat16_rn(0.f);
+        }
+    // the recurrent input of row `lane` at step s comes from its step s + 1 (time t + 1 forward, t - 1 backwards in time), or is zero
+    // when s + 1 is past its length
+    const int Lr = len_s[lane];
+    for (int s = S - 1; s >= 0; --s) {
+        const bool active = s < L;
+        const int t = dir.rev ? L - 1 - s : s;
         for (int i = tid; i < 32 * 9; i += LS_THREADS) r_s[i] = 0.f;
         // saved forward values of this step: independent of the recurrent gradient, fetched before the product (latency off the critical path)
         float pgi = 0.f, pgf = 0.f, pgg = 0.f, pgo = 0.f, pc = 0.f, pcp = 0.f, pdo = 0.f;
-        if (cb < B) {
+        if (active) {
             const int j = j0 + cj;
+            const int tp = dir.rev ? t + 1 : t - 1;                              // the previous step's time
             const float* gs = gates_save + ((long long)t * Bt + cb) * G4 + j;
             pgi = __ldg(gs); pgf = __ldg(gs + H); pgg = __ldg(gs + 2 * H); pgo = __ldg(gs + 3 * H);
             pc = __ldg(cs + ((long long)t * Bt + cb) * H + j);
-            pcp = t > 0 ? __ldg(cs + ((long long)(t - 1) * Bt + cb) * H + j) : 0.f;
-            pdo = to_f32<T>(dout[((long long)cb * U + t) * H + j]);
+            pcp = s > 0 ? __ldg(cs + ((long long)tp * Bt + cb) * H + j) : 0.f;
+            pdo = to_f32<T>(dout[((long long)cb * U + t) * ldo + j]);
         }
-        if (t < U - 1) {
-            const __nv_bfloat16* src = dG + (long long)(t + 1) * Bt * G4;
+        if (s < S - 1) {
+            const int tn = dir.rev ? Lr - 2 - s : s + 1;
+            const __nv_bfloat16* src = s + 1 < Lr ? dG + ((long long)tn * Bt + lane) * G4 : zrow;
             auto issue = [&](int qtr) {                                          // warp 0: lane r copies row r of quarter `qtr`
                 if (warp == 0) {
                     fence_proxy_async_all();
                     if (lane == 0) mbar_arrive_expect_tx(&q_bar[qtr & 1], (uint32_t)B * (uint32_t)KQ * 2u);
                     __syncwarp();
                     __nv_bfloat16* dst = d_s + ((qtr & 1) * 32 + lane) * PD;
-                    const __nv_bfloat16* from = src + (long long)lane * G4 + qtr * KQ;
+                    const __nv_bfloat16* from = src + qtr * KQ;
                     if (lane < B) {
                         // cluster: each CTA fetches every cn-th row and multicasts it to all cn CTAs (every CTA needs the whole 256 KB
                         // row block each step: one L2 read per cluster instead of one per CTA)
@@ -298,7 +379,7 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __
             atomicAdd(&r_s[(mt * 16 + g + 8) * 9 + 2 * tq + 1], acc[3]);
         }
         __syncthreads();
-        if (cb < B) {
+        if (active) {
             const int j = j0 + cj;
             const float gi = pgi, gf = pgf, gg = pgg, go = pgo, c = pc, cp = pcp;
             const float dh = pdo + r_s[cb * 9 + cj];
@@ -310,8 +391,11 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __
             d[2 * H] = __float2bfloat16_rn(dc * gi * (1.f - gg * gg));
             d[3 * H] = __float2bfloat16_rn(dh * tc * go * (1.f - go));
             dc_state = dc * gf;
+        } else if (cb < B) {
+            __nv_bfloat16* d = dG + ((long long)s * Bt + cb) * G4 + j0 + cj;     // s >= L_b: a padded position
+            d[0] = d[H] = d[2 * H] = d[3 * H] = __float2bfloat16_rn(0.f);
         }
-        if (t > 0) grid_barrier(counter, (unsigned int)(U - t), bar_mode, cn, cr);
+        if (s > 0) grid_barrier(counter, (unsigned int)(S - s), bar_mode, cn, cr, dir.nct);
     }
 }
 }  // namespace pk
@@ -346,18 +430,25 @@ static int lstm_launch(const void* fn, int grid, int smem, void** args, cudaStre
     PK_CHECK_CUDA(cudaLaunchKernelExC(&cfg, fn, args));
     return 0;
 }
-static int lstm_seq_check(int B, int U, int H) {
+static int lstm_seq_check(int B, int U, int H, int n_dir) {
     PK_CHECK_ARG(B >= 1, "empty batch");
-    PK_CHECK_ARG(U >= 1 && H % 64 == 0 && H / LS_HJ <= num_sms(), "H must be a multiple of 64 with H/8 <= #SMs");
+    PK_CHECK_ARG(n_dir == 1 || n_dir == 2, "n_dir must be 1 or 2");
+    PK_CHECK_ARG(U >= 1 && H % 64 == 0 && n_dir * H / LS_HJ <= num_sms(), "H must be a multiple of 64 with n_dir * H/8 <= #SMs");
     return 0;
 }
-extern "C" long long pk_lstm_seq_workspace_bytes(int H) { return 2ll * LS_MB * H * 2 + 256; }
+// the cluster size is chosen once per (kernel flavour, n_dir, H): the grid and the shared memory per CTA both enter the occupancy.
+// Every grid is a multiple of 8 CTAs per direction, so a cluster of 8, 4 or 2 never straddles two directions.
+static int* lstm_cluster_slot(int (*cache)[2][64], int fl, int n_dir, int H) { return &cache[fl][n_dir - 1][(H / 64) & 63]; }
 
-/* ws: pk_lstm_seq_workspace_bytes(H): [barrier counter (256 B)] [hx bf16 2 x 32 x H] */
-extern "C" int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, float* gates_save, float* cs, int B,
-                               int U, int H, void* ws, void* stream) {
-    int rc = lstm_seq_check(B, U, H);
+extern "C" long long pk_lstm_seq_workspace_bytes(int H) { return 2ll * LS_MB * H * 2 + 256 + 4ll * H * 2; }
+
+/* ws: pk_lstm_seq_workspace_bytes(n_dir * H): [barrier counters, one per direction, 128 B apart (256 B)]
+ *     [hx bf16 n_dir x 2 x 32 x H] [4 * n_dir * H zero bf16 (never written)] */
+extern "C" int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, int ldo, float* gates_save, float* cs,
+                                  const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream) {
+    int rc = lstm_seq_check(B, U, H, n_dir);
     if (rc) return rc;
+    PK_CHECK_ARG(ldo >= n_dir * H, "ldo must be >= n_dir * H");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     unsigned int* counter = reinterpret_cast<unsigned int*>(ws);
     __nv_bfloat16* hx = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<unsigned char*>(ws) + 256);
@@ -367,31 +458,32 @@ extern "C" int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out
     PK_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const size_t es = out_dtype == PK_BF16 ? 2 : 4;
     int bar_mode = lstm_bar_mode();
+    const int grid = n_dir * H / LS_HJ;
+    static int cluster_f[2][2][64] = {};
     for (int b0 = 0; b0 < B; b0 += LS_MB) {                    // sequences are independent: 32 per cooperative launch
         int nb = B - b0 < LS_MB ? B - b0 : LS_MB, Bt = B;
         const float* gx_c = gx + (long long)b0 * U * 4 * H;
-        void* out_c = reinterpret_cast<unsigned char*>(out) + (size_t)b0 * U * H * es;
+        void* out_c = reinterpret_cast<unsigned char*>(out) + (size_t)b0 * U * ldo * es;
         float* gs_c = gates_save + (long long)b0 * 4 * H;
         float* cs_c = cs + (long long)b0 * H;
+        const int* lens_c = lens ? lens + b0 : nullptr;
         PK_CHECK_CUDA(cudaMemsetAsync(counter, 0, 256, st));
-        void* args[] = {(void*)&gx_c, (void*)&w, (void*)&out_c, (void*)&hx, (void*)&gs_c, (void*)&cs_c, (void*)&nb, (void*)&Bt, (void*)&U, (void*)&H,
-                        (void*)&counter, (void*)&bar_mode};
-        static int cluster_f[2] = {0, 0};                      // per kernel flavour (the cluster choice depends on the grid = H / 8 too:
-        static int grid_f[2] = {0, 0};                         //  re-evaluated when H changes)
-        const int fl = out_dtype == PK_BF16 ? 0 : 1;
-        if (grid_f[fl] != H / LS_HJ) { grid_f[fl] = H / LS_HJ; cluster_f[fl] = 0; }
-        rc = lstm_launch(fn, H / LS_HJ, smem, args, st, &cluster_f[fl]);
+        void* args[] = {(void*)&gx_c, (void*)&w, (void*)&out_c, (void*)&ldo, (void*)&hx, (void*)&gs_c, (void*)&cs_c, (void*)&lens_c, (void*)&nb,
+                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter, (void*)&bar_mode};
+        rc = lstm_launch(fn, grid, smem, args, st, lstm_cluster_slot(cluster_f, out_dtype == PK_BF16 ? 0 : 1, n_dir, H));
         if (rc) return rc;
         count_launch();
     }
     return 0;
 }
-extern "C" int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const float* cs, const void* w_hh_bf16, void* dG_bf16,
-                               int B, int U, int H, void* ws, void* stream) {
-    int rc = lstm_seq_check(B, U, H);
+extern "C" int pk_lstm_seq_bwd_ex(const void* dout, int dtype, int ldo, const float* gates_save, const float* cs, const void* w_hh_bf16,
+                                  void* dG_bf16, const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream) {
+    int rc = lstm_seq_check(B, U, H, n_dir);
     if (rc) return rc;
+    PK_CHECK_ARG(ldo >= n_dir * H, "ldo must be >= n_dir * H");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     unsigned int* counter = reinterpret_cast<unsigned int*>(ws);
+    const __nv_bfloat16* zrow = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<unsigned char*>(ws) + 256 + 2ll * LS_MB * n_dir * H * 2);
     const int G4 = 4 * H;
     const int smem = LS_HJ * (G4 + LS_PAD) * 2 + 2 * 32 * (G4 / 4 + LS_PAD) * 2 + 32 * 9 * 4;
     const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(w_hh_bf16);
@@ -399,21 +491,29 @@ extern "C" int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_s
     PK_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const size_t es = dtype == PK_BF16 ? 2 : 4;
     int bar_mode = lstm_bar_mode();
+    const int grid = n_dir * H / LS_HJ;
+    static int cluster_b[2][2][64] = {};
     for (int b0 = 0; b0 < B; b0 += LS_MB) {
         int nb = B - b0 < LS_MB ? B - b0 : LS_MB, Bt = B;
-        const void* dout_c = reinterpret_cast<const unsigned char*>(dout) + (size_t)b0 * U * H * es;
+        const void* dout_c = reinterpret_cast<const unsigned char*>(dout) + (size_t)b0 * U * ldo * es;
         const float* gs_c = gates_save + (long long)b0 * G4;
         const float* cs_c = cs + (long long)b0 * H;
         __nv_bfloat16* dg = reinterpret_cast<__nv_bfloat16*>(dG_bf16) + (long long)b0 * G4;
+        const int* lens_c = lens ? lens + b0 : nullptr;
         PK_CHECK_CUDA(cudaMemsetAsync(counter, 0, 256, st));
-        void* args[] = {(void*)&dout_c, (void*)&gs_c, (void*)&cs_c, (void*)&w, (void*)&dg, (void*)&nb, (void*)&Bt, (void*)&U, (void*)&H, (void*)&counter, (void*)&bar_mode};
-        static int cluster_b[2] = {0, 0};
-        static int grid_b[2] = {0, 0};
-        const int fl = dtype == PK_BF16 ? 0 : 1;
-        if (grid_b[fl] != H / LS_HJ) { grid_b[fl] = H / LS_HJ; cluster_b[fl] = 0; }
-        rc = lstm_launch(fn, H / LS_HJ, smem, args, st, &cluster_b[fl]);
+        void* args[] = {(void*)&dout_c, (void*)&ldo, (void*)&gs_c, (void*)&cs_c, (void*)&w, (void*)&dg, (void*)&zrow, (void*)&lens_c, (void*)&nb,
+                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter, (void*)&bar_mode};
+        rc = lstm_launch(fn, grid, smem, args, st, lstm_cluster_slot(cluster_b, dtype == PK_BF16 ? 0 : 1, n_dir, H));
         if (rc) return rc;
         count_launch();
     }
     return 0;
+}
+extern "C" int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, float* gates_save, float* cs, int B,
+                               int U, int H, void* ws, void* stream) {
+    return pk_lstm_seq_fwd_ex(gx, w_hh_bf16, out, out_dtype, H, gates_save, cs, nullptr, B, U, H, 1, 0, ws, stream);
+}
+extern "C" int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const float* cs, const void* w_hh_bf16, void* dG_bf16,
+                               int B, int U, int H, void* ws, void* stream) {
+    return pk_lstm_seq_bwd_ex(dout, dtype, H, gates_save, cs, w_hh_bf16, dG_bf16, nullptr, B, U, H, 1, 0, ws, stream);
 }

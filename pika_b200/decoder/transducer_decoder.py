@@ -237,7 +237,7 @@ class TransducerDecoder():
         dev = x.device if enc_out is None else enc_out.device
         assert dev.type == "cuda", "pika_b200 decodes on the GPU (there is no CPU fallback)"
         if enc_out is None:
-            enc = engine.encoder_forward_act(m.encoder, x).contiguous()          # [B, T', H]
+            enc = engine.model_encoder_forward_act(m, x, x_len).contiguous()     # [B, T', H] (packed over x_len: LSTM encoder)
         else:
             enc = engine._to_act(enc_out)
         B, Tenc, H = enc.shape

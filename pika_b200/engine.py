@@ -574,76 +574,150 @@ class EmbeddingFn(torch.autograd.Function):
         return None, None, None, None
 
 
+def _lstm_step_maps(lens, B, U, rev):
+    """Index maps of one direction's per-step path between time and processing step (step s of sequence b is time s, or
+    L_b - 1 - s in reverse).  Returns (src, dsrc, to_time), all int32 [U, B] indexed [step or time, b]:
+      src     -- row b*U + t of a [B*U, .] tensor that step s reads (clamped to t = 0 once the sequence has finished);
+      dsrc    -- the same, but B*U (a zero row) once the sequence has finished;
+      to_time -- row s*B + b of a step-major [U*B + 1, .] tensor that holds time t, or U*B (a zero row) for t >= L_b."""
+    r = torch.arange(U, dtype=torch.int32, device=lens.device).view(U, 1)
+    b = torch.arange(B, dtype=torch.int32, device=lens.device).view(1, B)
+    L = lens.view(1, B).clamp(0, U)
+    other = (L - 1 - r) if rev else r.expand(U, B)          # time of step r, or step of time r: the map is its own inverse
+    live = r < L
+    src = b * U + torch.where(live, other, torch.zeros_like(other))
+    dsrc = torch.where(live, b * U + other, torch.full_like(other, B * U))
+    to_time = torch.where(live, other * B + b, torch.full_like(other, U * B))
+    return src, dsrc, to_time
+
+
 class LstmLayerFn(torch.autograd.Function):
-    """One nn.LSTM layer (batch_first, zero initial state) over x [B,U,E]: the input projection is one
-    GEMM over all steps; each step is a recurrent GEMM (h_{t-1} W_hh^T) + a fused cell kernel."""
+    """One nn.LSTM layer (batch_first, zero initial state) over x [B,U,E] -> [B,U,n_dir*H], for n_dir = 1 or 2 directions (params:
+    w_ih, w_hh, b_ih, b_hh of each direction, direction 1 running backwards in time).  ``lens`` (int32 [B] on the device, or None):
+    the pack_padded_sequence lengths -- sequence b runs over its first L_b steps, its reverse direction starts at L_b - 1, and
+    outputs at t >= L_b are zero (pad_packed_sequence).  The input projection is one GEMM over all steps per direction; the
+    recurrence is one cooperative launch for both directions (lstm_seq.cu), or per step a recurrent GEMM + a fused cell kernel
+    (fp32-class mode, or shapes outside the persistent kernel's limits)."""
 
     @staticmethod
-    def forward(ctx, x, lstm, layer, w_ih, w_hh, b_ih, b_hh):
+    def forward(ctx, x, lens, *params):
         B, U, E = x.shape
-        H = w_hh.shape[1]
-        wih_parts = stage_weight(w_ih, cols_pad=E if E != w_ih.shape[1] else None)
-        whh_parts = stage_weight(w_hh)
-        bsum = torch.empty(4 * H, dtype=torch.float32, device=x.device)
-        K.add(b_ih.detach(), b_hh.detach(), bsum)
+        n_dir = len(params) // 4
+        dirs = [params[4 * d:4 * d + 4] for d in range(n_dir)]
+        H = dirs[0][1].shape[1]
+        G4 = 4 * H
+        wih_parts = [stage_weight(p[0], cols_pad=E if E != p[0].shape[1] else None) for p in dirs]
+        whh_parts = stage_weight([p[1] for p in dirs])                 # [n_dir*4H, H]
         x_parts = stage_act(x)
-        gx = torch.empty(B, U, 4 * H, dtype=torch.float32, device=x.device)
-        gemm_parts([[p.view(B * U, E) for p in x_parts]], [wih_parts], gx.view(B * U, 4 * H), bias=bsum)
-        out = _new((B, U, H), like=x)
-        gates = torch.empty(U, B, 4 * H, dtype=torch.float32, device=x.device)
-        cs = torch.empty(U, B, H, dtype=torch.float32, device=x.device)
+        gx = torch.empty(n_dir, B, U, G4, dtype=torch.float32, device=x.device)
+        for d, (w_ih, w_hh, b_ih, b_hh) in enumerate(dirs):
+            bsum = torch.empty(G4, dtype=torch.float32, device=x.device)
+            K.add(b_ih.detach(), b_hh.detach(), bsum)
+            gemm_parts([[p.view(B * U, E) for p in x_parts]], [wih_parts[d]], gx[d].view(B * U, G4), bias=bsum)
+        out = _new((B, U, n_dir * H), like=x)
+        gates = torch.empty(n_dir, U, B, G4, dtype=torch.float32, device=x.device)
+        cs = torch.empty(n_dir, U, B, H, dtype=torch.float32, device=x.device)
         ctx.persistent = (x.dtype == torch.bfloat16 and H % 64 == 0 and
-                          H // 8 <= torch.cuda.get_device_properties(x.device).multi_processor_count)      # any batch: 32 sequences per cooperative launch
+                          n_dir * H // 8 <= torch.cuda.get_device_properties(x.device).multi_processor_count)  # any batch: 32 sequences per cooperative launch
         if ctx.persistent:
-            # whole recurrence in one cooperative launch (pika_b200/csrc/lstm_seq.cu)
-            K.lstm_seq_fwd(gx, whh_parts[0], out, gates, cs)
-        gh = torch.empty(B, 4 * H, dtype=torch.float32, device=x.device)
-        for t in range(0 if not ctx.persistent else U, U):
-            if t > 0:
-                gemm_parts([stage_act_view(out[:, t - 1, :])], [whh_parts], gh, block_n=64)
-            K.lstm_cell_fwd(gx[:, t, :], gh if t > 0 else None, cs[t - 1] if t > 0 else None, cs[t], out[:, t, :], gates[t], B, H)
+            # whole recurrence of every direction in one cooperative launch (pika_b200/csrc/lstm_seq.cu)
+            K.lstm_seq_fwd_ex(gx, whh_parts[0], out, gates, cs, lens)
+        else:
+            for d in range(n_dir):
+                whh = [p[d * G4:(d + 1) * G4] for p in whh_parts]
+                out_d = out[:, :, d * H:(d + 1) * H]
+                if lens is None and d == 0:                           # step s is time s for every sequence
+                    gx_s, h_s = (lambda t: gx[d][:, t, :]), (lambda t: out_d[:, t, :])
+                else:
+                    src, _, _ = _lstm_step_maps(lens if lens is not None else _full_lens(B, U, x.device), B, U, d == 1)
+                    gxs = torch.empty(U * B, G4, dtype=torch.float32, device=x.device)
+                    K.gather_rows(gx[d].view(B * U, G4), src.view(-1), gxs)
+                    hs = _new((U * B + 1, H), like=x, zero=True)       # step-major; the last row stays zero
+                    gx_s, h_s = (lambda t: gxs[t * B:(t + 1) * B]), (lambda t: hs[t * B:(t + 1) * B])
+                gh = torch.empty(B, G4, dtype=torch.float32, device=x.device)
+                for t in range(U):
+                    if t > 0:
+                        gemm_parts([stage_act_view(h_s(t - 1))], [whh], gh, block_n=64)
+                    K.lstm_cell_fwd(gx_s(t), gh if t > 0 else None, cs[d][t - 1] if t > 0 else None, cs[d][t], h_s(t), gates[d][t], B, H)
+                if not (lens is None and d == 0):
+                    _, _, to_time = _lstm_step_maps(lens if lens is not None else _full_lens(B, U, x.device), B, U, d == 1)
+                    ho = _new((B * U, H), like=x)
+                    K.gather_rows(hs, to_time.t().contiguous().view(-1), ho)
+                    out_d.copy_(ho.view(B, U, H))
         ctx.save_for_backward(x, out, gates, cs)
         ctx.x_parts, ctx.wih_parts, ctx.whh_parts = x_parts, wih_parts, whh_parts
-        ctx.params = (w_ih, w_hh, b_ih, b_hh)
+        ctx.dirs, ctx.lens = dirs, lens
         return out
 
     @staticmethod
     def backward(ctx, dout):
         x, out, gates, cs = ctx.saved_tensors
-        w_ih, w_hh, b_ih, b_hh = ctx.params
+        lens, dirs = ctx.lens, ctx.dirs
+        n_dir = len(dirs)
         B, U, E = x.shape
-        H = w_hh.shape[1]
+        H = dirs[0][1].shape[1]
+        G4 = 4 * H
         dout = dout.contiguous()
-        dG = _new((U, B, 4 * H), like=out)                 # time-major: dG[t] is a contiguous [B,4H] matrix
-        dh_rec = torch.empty(B, H, dtype=torch.float32, device=x.device)
-        dc = [torch.empty(B, H, dtype=torch.float32, device=x.device) for _ in range(2)]
+        dG = _new((n_dir, U, B, G4), like=out)             # time-major: dG[d][t] is a contiguous [B,4H] matrix; zero at t >= L_b
         if ctx.persistent:
-            K.lstm_seq_bwd(dout, gates, cs, ctx.whh_parts[0], dG)
-        for t in range(U - 1 if not ctx.persistent else -1, -1, -1):
-            last = (t == U - 1)
-            K.lstm_cell_bwd(dout[:, t, :], None if last else dh_rec, None if last else dc[(t + 1) & 1], gates[t], cs[t],
-                            cs[t - 1] if t > 0 else None, dG[t], dc[t & 1], B, H)
-            if t > 0:
-                gemm_parts([stage_act_view(dG[t])], [ctx.whh_parts], dh_rec, b_mn=True, block_n=64)
-        dg_parts = stage_act(dG)                            # [U,B,4H]
-        out_parts = stage_act(out)                          # [B,U,H]
-        sel = dict(a_sel=(K.SEL_KZ, K.SEL_ZERO), b_sel=(K.SEL_KZ, K.SEL_ZERO))
-        # dW_hh = sum_{t>=1} dG[t]^T h[t-1]   (reduction over batch rows, batched over t)
-        if U > 1:
-            gemm_parts([[p[1:] for p in dg_parts]], [[p.permute(1, 0, 2)[:-1] for p in out_parts]], grad_of(w_hh),
-                       a_mn=True, b_mn=True, kz_count=U - 1, **sel)
+            K.lstm_seq_bwd_ex(dout, gates, cs, ctx.whh_parts[0], dG, lens)
         else:
-            grad_of(w_hh).zero_()
-        gemm_parts([dg_parts], [[p.permute(1, 0, 2) for p in ctx.x_parts]], grad_of(w_ih), a_mn=True, b_mn=True, kz_count=U, **sel)
-        K.colsum(dG.view(U * B, 4 * H), grad_of(b_ih))
-        grad_of(b_hh).copy_(b_ih.grad)
+            dh_rec = torch.empty(B, H, dtype=torch.float32, device=x.device)
+            dc = [torch.empty(B, H, dtype=torch.float32, device=x.device) for _ in range(2)]
+            for d in range(n_dir):
+                whh = [p[d * G4:(d + 1) * G4] for p in ctx.whh_parts]
+                dout_d = dout[:, :, d * H:(d + 1) * H]
+                if lens is None and d == 0:
+                    do_s, dg_s = (lambda t: dout_d[:, t, :]), (lambda t: dG[d][t])
+                else:
+                    # step-major copies; a finished sequence reads a zero gradient, so its dG rows and dc stay exactly zero
+                    _, dsrc, to_time = _lstm_step_maps(lens if lens is not None else _full_lens(B, U, x.device), B, U, d == 1)
+                    dz = torch.zeros(B * U + 1, H, dtype=dout.dtype, device=x.device)
+                    dz[:B * U].view(B, U, H).copy_(dout_d)
+                    dos = torch.empty(U * B, H, dtype=dout.dtype, device=x.device)
+                    K.gather_rows(dz, dsrc.view(-1), dos)
+                    dgs = _new((U * B + 1, G4), like=out, zero=True)
+                    do_s, dg_s = (lambda t: dos[t * B:(t + 1) * B]), (lambda t: dgs[t * B:(t + 1) * B])
+                for t in range(U - 1, -1, -1):
+                    last = (t == U - 1)
+                    K.lstm_cell_bwd(do_s(t), None if last else dh_rec, None if last else dc[(t + 1) & 1], gates[d][t], cs[d][t],
+                                    cs[d][t - 1] if t > 0 else None, dg_s(t), dc[t & 1], B, H)
+                    if t > 0:
+                        gemm_parts([stage_act_view(dg_s(t))], [whh], dh_rec, b_mn=True, block_n=64)
+                if not (lens is None and d == 0):
+                    K.gather_rows(dgs, to_time.view(-1), dG[d].view(U * B, G4))
+        dg_all = stage_act(dG)                              # [n_dir,U,B,4H]
+        out_parts = stage_act(out)                          # [B,U,n_dir*H]
+        sel = dict(a_sel=(K.SEL_KZ, K.SEL_ZERO), b_sel=(K.SEL_KZ, K.SEL_ZERO))
+        for d, (w_ih, w_hh, b_ih, b_hh) in enumerate(dirs):
+            dg_parts = [p[d] for p in dg_all]
+            h_parts = [p[:, :, d * H:(d + 1) * H].permute(1, 0, 2) for p in out_parts]       # [U,B,H]
+            # dW_hh = sum_t dG[t]^T h[t-1] (forward) or dG[t]^T h[t+1] (reverse), reduced over batch rows, batched over t;
+            # dG is zero past each length and h[L_b] is a zero output, so no masking
+            if U > 1:
+                a, b = ([p[1:] for p in dg_parts], [p[:-1] for p in h_parts]) if d == 0 else \
+                       ([p[:-1] for p in dg_parts], [p[1:] for p in h_parts])
+                gemm_parts([a], [b], grad_of(w_hh), a_mn=True, b_mn=True, kz_count=U - 1, **sel)
+            else:
+                grad_of(w_hh).zero_()
+            gemm_parts([dg_parts], [[p.permute(1, 0, 2) for p in ctx.x_parts]], grad_of(w_ih), a_mn=True, b_mn=True, kz_count=U, **sel)
+            K.colsum(dG[d].view(U * B, G4), grad_of(b_ih))
+            grad_of(b_hh).copy_(b_ih.grad)
         dx = None
         if ctx.needs_input_grad[0]:
+            # dx = sum_d dG_d W_ih_d: one GEMM over the directions' (A, B) pairs
             dx = torch.empty_like(x)
-            wb, wmn = dgrad_b(ctx.wih_parts)
-            gemm_parts([dg_parts], [wb], dx.permute(1, 0, 2), b_mn=wmn, a_sel=(K.SEL_ZB0, K.SEL_ZERO),
-                       b_sel=(K.SEL_ZERO, K.SEL_ZERO))
-        return dx, None, None, None, None, None, None
+            taps, wbs, wmn = [], [], True
+            for d in range(n_dir):
+                wb, wmn = dgrad_b(ctx.wih_parts[d])
+                taps.append([p[d] for p in dg_all])
+                wbs.append(wb)
+            gemm_parts(taps, wbs, dx.permute(1, 0, 2), b_mn=wmn, a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO))
+        return (dx, None) + (None,) * (4 * n_dir)
+
+
+def _full_lens(B, U, device):
+    return torch.full((B,), U, dtype=torch.int32, device=device)
 
 
 def stage_act_view(v):
@@ -906,8 +980,11 @@ def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None):
                   mask_input_scale=(1.0 / (1.0 - p) if p > 0 else 1.0) if fold else 0.0)
 
 
-def encoder_forward_act(enc, x):
-    """x [B,T,D] -> [B,T',H] in the activation dtype."""
+def encoder_forward_act(enc, x, x_len=None, t_out=None):
+    """x [B,T,D] -> [B,T',H] in the activation dtype.  An nn.LSTM encoder runs over the packed lengths ``x_len`` (see
+    lstm_encoder_forward_act); the TDNN-Transformer encoder ignores them, as the reference does (pack_seq is False)."""
+    if isinstance(enc, torch.nn.LSTM):
+        return lstm_encoder_forward_act(enc, x, x_len, t_out)
     training = enc.training
     B, T, D = x.shape
     C = enc.tdnn_nhid
@@ -932,6 +1009,51 @@ def encoder_forward(enc, x):
     return encoder_forward_act(enc, x).float()
 
 
+def _lstm_layer_params(lstm, l):
+    names = ["weight_ih_l%d", "weight_hh_l%d", "bias_ih_l%d", "bias_hh_l%d"]
+    sfx = ["", "_reverse"] if lstm.bidirectional else [""]
+    return [getattr(lstm, n % l + x) for x in sfx for n in names]
+
+
+def lstm_encoder_forward_act(lstm, x, x_len=None, t_out=None):
+    """The LSTM encoder (trainer/model/transducer.py:38-44,82-86): nn.LSTM (batch_first, optionally bidirectional) over
+    pack_padded_sequence(x, x_len, enforce_sorted=False), unpacked again: x [B,T,D] -> [B,T_out,n_dir*H] in the activation dtype,
+    zero at t >= x_len[b].  T_out = max(x_len), as pad_packed_sequence returns; a caller that knows it on the host passes ``t_out``
+    (the lengths are then not read back), otherwise it is read once.  ``x_len = None``: every sequence runs all T frames (the
+    reference's unpacked forward).  Lengths may come in any order.  nn.LSTM's inter-layer dropout runs in training mode only,
+    never after the last layer."""
+    if lstm.batch_first is not True or not lstm.bias or lstm.proj_size:
+        raise NotImplementedError("pika_b200: the LSTM encoder expects nn.LSTM(batch_first=True, bias=True, proj_size=0)")
+    B, T, D = x.shape
+    lens = None
+    if x_len is None:
+        t_out = T
+    else:
+        x_len = torch.as_tensor(x_len)
+        if x_len.shape != (B,):
+            raise ValueError("x_len must hold one length per sequence (%d), got shape %s" % (B, tuple(x_len.shape)))
+        if t_out is None or not x_len.is_cuda:
+            lo, hi = (int(v) for v in torch.stack((x_len.min(), x_len.max())).tolist())
+            if lo < 1 or hi > T:
+                raise ValueError("x_len must lie in [1, %d] (the frames of x); got [%d, %d]" % (T, lo, hi))
+            t_out = hi if t_out is None else t_out
+        if not 1 <= t_out <= T:
+            raise ValueError("t_out = %d must lie in [1, %d]" % (t_out, T))
+        lens = x_len.to(device=x.device, dtype=torch.int32).contiguous()
+    ld = (D + 7) // 8 * 8
+    h = _to_act(x[:, :t_out])
+    if ld != D:
+        hp = _new((B, t_out, ld), like=h, zero=True)
+        hp[:, :, :D] = h
+        h = hp
+    p = _drop(lstm.dropout, lstm.training)
+    for l in range(lstm.num_layers):
+        h = LstmLayerFn.apply(h, lens, *_lstm_layer_params(lstm, l))
+        if p > 0 and l < lstm.num_layers - 1:
+            h = DropoutFn.apply(h, p, _next_seed())
+    return h
+
+
 def prednet_forward_act(model, y):
     """y [B,U] int64 -> [B,U+1,H]: SOS(blank=0) prepend, embedding, LSTM stack with inter-layer dropout
     (trainer/model/transducer.py:90-95)."""
@@ -946,8 +1068,7 @@ def prednet_forward_act(model, y):
     lstm = model.decoder
     p = _drop(lstm.dropout, lstm.training)
     for l in range(lstm.num_layers):
-        h = LstmLayerFn.apply(h, lstm, l, getattr(lstm, "weight_ih_l%d" % l), getattr(lstm, "weight_hh_l%d" % l),
-                              getattr(lstm, "bias_ih_l%d" % l), getattr(lstm, "bias_hh_l%d" % l))
+        h = LstmLayerFn.apply(h, None, *_lstm_layer_params(lstm, l))
         if p > 0 and l < lstm.num_layers - 1:
             h = DropoutFn.apply(h, p, _next_seed())
     return h
@@ -974,9 +1095,18 @@ def conv_transformer_lm_forward_act(dec, src):
     return linear(hn, dec.linear_out.weight, dec.linear_out.bias).view(B, L, -1)
 
 
-def transducer_forward(model, x, y, softmax=True):
-    """Net.forward drop-in: -> [B,T',U+1,V] fp32 log-probs (softmax=True) or logits."""
-    enc = encoder_forward_act(model.encoder, x)
+def model_encoder_forward_act(model, x, x_len=None, t_out=None):
+    """The transducer's encoder as Net.forward runs it: over the packed lengths ``x_len`` when ``model.pack_seq`` (the LSTM
+    encoder; ``t_out`` = max(x_len) if the caller knows it on the host), over all frames otherwise."""
+    if getattr(model, "pack_seq", False):
+        return encoder_forward_act(model.encoder, x, x_len, t_out)
+    return encoder_forward_act(model.encoder, x)
+
+
+def transducer_forward(model, x, y, softmax=True, x_len=None, t_out=None):
+    """Net.forward drop-in: -> [B,T',U+1,V] fp32 log-probs (softmax=True) or logits.  ``x_len`` / ``t_out``: the packed lengths of
+    an LSTM encoder (lstm_encoder_forward_act); ignored by the TDNN-Transformer encoder."""
+    enc = model_encoder_forward_act(model, x, x_len, t_out)
     pred = prednet_forward_act(model, y)
     logits = JointFn.apply(enc, pred, model)
     V = model.fc2.weight.shape[0]
@@ -1005,9 +1135,10 @@ class LogSoftmaxFn(torch.autograd.Function):
         return out, None
 
 
-def transducer_loss(model, x, y, frame_lens, label_lens):
-    """Fused training path: costs [B] with gradients wired to every parameter."""
-    enc = encoder_forward_act(model.encoder, x)
+def transducer_loss(model, x, y, frame_lens, label_lens, x_len=None, t_out=None):
+    """Fused training path: costs [B] with gradients wired to every parameter.  ``x_len`` / ``t_out`` as in transducer_forward
+    (the trainer passes the encoder output lengths, which are also ``frame_lens``)."""
+    enc = model_encoder_forward_act(model, x, x_len, t_out)
     pred = prednet_forward_act(model, y)
     return JointLossFn.apply(enc, pred, model, y.int().contiguous(), frame_lens.int().contiguous(), label_lens.int().contiguous(),
                              torch.is_grad_enabled())

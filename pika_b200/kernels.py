@@ -349,6 +349,36 @@ def lstm_seq_bwd(dout, gates_save, cs, w_hh, dG):
                               _P(_lstm_scratch(H, dout.device)), _stream()), "pk_lstm_seq_bwd")
 
 
+def _lens_arg(lens, B):
+    if lens is None:
+        return ctypes.c_void_p(0)
+    assert lens.dtype == torch.int32 and lens.is_contiguous() and lens.numel() == B
+    return _P(lens)
+
+
+def lstm_seq_fwd_ex(gx, w_hh, out, gates_save, cs, lens=None, reverse=False):
+    """gx [n_dir,B,U,4H] f32; w_hh bf16 [n_dir*4H,H]; out [B,U,ldo] (a column-slice view is fine: direction d writes columns
+    [d*H, (d+1)*H) of it); gates_save [n_dir,U,B,4H], cs [n_dir,U,B,H]; lens int32 [B] or None."""
+    n_dir, B, U, G4 = gx.shape
+    H = G4 // 4
+    assert gx.is_contiguous() and w_hh.dtype == torch.bfloat16 and w_hh.is_contiguous() and w_hh.shape[0] == n_dir * G4
+    assert out.stride(2) == 1 and out.stride(0) == U * out.stride(1) and out.shape[-1] == n_dir * H
+    check(lib.pk_lstm_seq_fwd_ex(_P(gx), _P(w_hh), _P(out), _I(_dt(out)), _I(out.stride(1)), _P(gates_save), _P(cs), _lens_arg(lens, B),
+                                 _I(B), _I(U), _I(H), _I(n_dir), _I(int(reverse)), _P(_lstm_scratch(n_dir * H, gx.device)), _stream()),
+          "pk_lstm_seq_fwd_ex")
+
+
+def lstm_seq_bwd_ex(dout, gates_save, cs, w_hh, dG, lens=None, reverse=False):
+    """dout [B,U,ldo] (column-slice views as in lstm_seq_fwd_ex) -> dG bf16 [n_dir,U,B,4H]."""
+    n_dir, U, B, G4 = dG.shape
+    H = G4 // 4
+    assert dout.stride(2) == 1 and dout.stride(0) == U * dout.stride(1) and dout.shape[-1] == n_dir * H
+    assert dG.dtype == torch.bfloat16 and dG.is_contiguous() and w_hh.shape[0] == n_dir * G4
+    check(lib.pk_lstm_seq_bwd_ex(_P(dout), _I(_dt(dout)), _I(dout.stride(1)), _P(gates_save), _P(cs), _P(w_hh), _P(dG), _lens_arg(lens, B),
+                                 _I(B), _I(U), _I(H), _I(n_dir), _I(int(reverse)), _P(_lstm_scratch(n_dir * H, dout.device)), _stream()),
+          "pk_lstm_seq_bwd_ex")
+
+
 def gather_rows(src, idx, dst):
     rows, C = dst.shape
     check(lib.pk_gather_rows(_P(src), _P(idx), _P(dst), _I(_dt(src)), _L(rows), _I(C), _stream()), "pk_gather_rows")

@@ -2,9 +2,10 @@
 
 ``Net(opt, input_dim, output_dim)`` / ``forward(x, y, x_len, softmax)`` and the sub-module names
 ``encoder, embed, decoder, fc1, fc_gate, fc2`` (reached into by the decoder and the MBR trainer)
-are the reference's.  TDNN-Transformer encoder (``encoder_type != 'rnn'``) with either prediction net of the reference:
-the LSTM stack (``decoder_type == 'rnn'``) or the convolutional transformer (``'transformer'``,
-trainer/model/rnnt_conv_transformer_lm.py).
+are the reference's.  Either encoder of the reference: the LSTM (``encoder_type == 'rnn'``, optionally bidirectional,
+run over the packed lengths ``x_len``) or the TDNN-Transformer; and either prediction net: the LSTM stack
+(``decoder_type == 'rnn'``) or the convolutional transformer (``'transformer'``, trainer/model/rnnt_conv_transformer_lm.py).
+Modules are created in the reference's order, so ``torch.manual_seed(s); Net(...)`` draws the reference's initial weights.
 """
 import torch.nn as nn
 
@@ -20,11 +21,14 @@ class Net(nn.Module):
         self.hid_dim = opt.rnn_size
         self.local_rank = getattr(opt, "local_rank", 0)
         self.decoder_type = opt.decoder_type
-        if opt.encoder_type == "rnn":
-            raise NotImplementedError("pika_b200: only the TDNN-Transformer encoder is on the hot path")
-        self.encoder = encoder_tdnn(input_dim=input_dim, input_ctx=0, output_dim=self.hid_dim,
-                                    tdnn_nhid=1024, tdnn_layers=9)
-        self.pack_seq = False
+        if opt.encoder_type == "rnn":                  # trainer/model/transducer.py:35-44
+            self.encoder = nn.LSTM(input_size=input_dim, hidden_size=self.hid_dim // (2 if opt.brnn else 1), dropout=opt.dropout,
+                                   num_layers=opt.enc_layers, bidirectional=bool(opt.brnn), batch_first=True)
+            self.pack_seq = True
+        else:
+            self.encoder = encoder_tdnn(input_dim=input_dim, input_ctx=0, output_dim=self.hid_dim,
+                                        tdnn_nhid=1024, tdnn_layers=9)
+            self.pack_seq = False
         self.embed = nn.Embedding(output_dim + 1, opt.embd_dim, padding_idx=opt.padding_idx)
         if opt.decoder_type == "rnn":
             self.decoder = nn.LSTM(input_size=opt.embd_dim, hidden_size=self.hid_dim, dropout=opt.dropout,
@@ -37,9 +41,10 @@ class Net(nn.Module):
         self.fc2 = nn.Linear(self.hid_dim, output_dim)
 
     def forward(self, x, y, x_len=None, softmax=True):
-        """x [B,T,D] f32, y [B,U] int64 -> [B,T',U+1,V] log-probs (or logits if softmax=False)."""
+        """x [B,T,D] f32, y [B,U] int64 -> [B,T',U+1,V] log-probs (or logits if softmax=False).  With the LSTM encoder, x_len
+        packs the batch (T' = max(x_len)); the TDNN-Transformer encoder ignores it."""
         from pika_b200 import engine
-        return engine.transducer_forward(self, x, y, softmax)
+        return engine.transducer_forward(self, x, y, softmax, x_len=x_len)
 
     def clean_hidden(self):
         """interface kept from the reference"""

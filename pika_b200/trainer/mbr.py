@@ -128,7 +128,7 @@ def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, 
     nonblk, prob, dist, seq_grad, mbr_loss = nbest_risk(hyps, scores, tgt_cpu, al_cpu, blk)
 
     # ---- shared encoder forward; prediction net once on [reference ; hypotheses]
-    enc = engine.encoder_forward_act(model.encoder, feats)                       # [bsz, T', H], in the autograd graph
+    enc = engine.model_encoder_forward_act(model, feats, len_batch)              # [bsz, T', H], in the autograd graph
     Tp = enc.shape[1]
     u_ref = int(target.shape[1])
     u_hyp = max(len(h) for row in nonblk for h in row)

@@ -16,6 +16,12 @@ def encoder_out_lens(lens, lctx, rctx, stride):
     return l // stride + (l % stride != 0).to(l.dtype)
 
 
+def encoder_out_max(t_max, lctx, rctx, stride):
+    """max(encoder_out_lens) from the host-side longest input: the T_out of the packed LSTM encoder without a device read"""
+    l = t_max - lctx - rctx
+    return l // stride + (l % stride != 0)
+
+
 class TrainStep:
     def __init__(self, model, args, frontend, bmuf, optimizer, offset=None, scale=None, spec_augmentor=None):
         self.model, self.args, self.frontend, self.bmuf, self.opt = model, args, frontend, bmuf, optimizer
@@ -41,7 +47,8 @@ class TrainStep:
         self.opt.flat.zero_grad()                                         # optimizer.zero_grad()
         feats = self.features(batch)
         len_batch = encoder_out_lens(batch["n_frames"], a.model_lctx, a.model_rctx, a.model_stride)
-        costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"])
+        t_out = encoder_out_max(int(batch["t_max"]), a.model_lctx, a.model_rctx, a.model_stride)
+        costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out)
         engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1
         try:
             costs.sum().backward()

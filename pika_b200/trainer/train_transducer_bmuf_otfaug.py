@@ -54,9 +54,10 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
             else:
                 with torch.no_grad():
                     feats = step.features(batch)
-                    from .step import encoder_out_lens
+                    from .step import encoder_out_lens, encoder_out_max
                     tl = encoder_out_lens(batch["n_frames"], args.model_lctx, args.model_rctx, args.model_stride)
-                    costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"])
+                    t_out = encoder_out_max(int(batch["t_max"]), args.model_lctx, args.model_rctx, args.model_stride)
+                    costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
             loss = float(costs.sum().item())
         else:                                                 # empty batch (:100-101)
             loss = 0.0
