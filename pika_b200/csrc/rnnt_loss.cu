@@ -557,6 +557,12 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
     if (G > LAT_MAX_G) G = LAT_MAX_G;
     const int cpt = (U1 + G - 1) / G;
     PK_CHECK_ARG(cpt <= LAT_MAX_CPT, "U too large for the lattice kernel (U+1 <= 2048)");
+    static bool configured = false;                  // the two ping-pong diagonals exceed the default 48 KB from U+1 = 1534 on
+    if (!configured) {
+        PK_CHECK_CUDA(cudaFuncSetAttribute(rnnt_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           2 * 2 * (LAT_MAX_G * LAT_MAX_CPT + 2) * (int)sizeof(lat_t)));
+        configured = true;
+    }
     rnnt_lattice_kernel<<<B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
                                                      costs, gb, gl);
     PK_CHECK_LAUNCH(); count_launch();

@@ -211,10 +211,21 @@ def test_lstm_and_embedding():
 
 
 def test_joint_and_fused_loss():
+    _joint_and_fused_loss(128, 11, 4)         # the channel-sliced gate forward and the fused gate backward
+
+
+# each fallback of the gate kernels to the frame-major forward / two-pass backward: H % 32 != 0 (both), T < 8 (forward
+# only), U+1 > 160 (both)
+@pytest.mark.parametrize("H,T,U", [(200, 9, 4), (128, 5, 4), (128, 9, 170)])
+def test_joint_and_fused_loss_gate_fallbacks(H, T, U):
+    _joint_and_fused_loss(H, T, U)
+
+
+def _joint_and_fused_loss(H, T, U):
     from pika_b200 import engine as E
     import numpy as np
     from oracle import rnnt as orc
-    H, V, B, T, U = 128, 45, 2, 11, 4
+    V, B = 45, 2
 
     class M(nn.Module):
         pass
@@ -319,6 +330,10 @@ def test_fused_lse_joint_loss_matches_separate_first_pass():
     H, V, B, T, U = 128, 520, 3, 13, 5
     prev, was = E.get_precision(), E._FUSED_LSE
     E.set_precision("bf16")
+    # the weights and labels come from the global RNG: seed it, so that they do not depend on what earlier tests drew from it
+    # (on some draws the two first passes round a few bf16 gradient entries differently, which moves the joint's weight
+    # gradients by up to a few 1e-4 norm-relative, around the bound below)
+    torch.manual_seed(0)
     try:
         class M(nn.Module):
             pass
