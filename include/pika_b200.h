@@ -87,8 +87,6 @@ typedef struct {
     float aux_scale;
     int block_n;                      /* 0 = auto; else 64 | 128 | 256 */
     int k_splits;                     /* 0 = auto; 1 = off; >1 = split the reduction (plain f32 2-D C only) */
-    int two_sm;                       /* 0 = auto (single CTA unless PK_GEMM_2SM=1); 1 = pair kernel for 256-wide tiles when M > 128; -1 = never.  The pair is a
-                                         2-CTA cluster working on a 256 x 256 tile: each CTA loads half of B and multicasts it to both */
     float* row_lse;                   /* optional out [pk_gemm_row_lse_parts()][M][2] f32: per row and column group (max*log2(e),
                                          sum_j 2^(c_ij*log2(e) - max)) over the ROUNDED bf16 outputs -- the first pass of the fused
                                          log-softmax + RNN-T loss (pk_rnnt_loss_fwd_bwd_lse) computed while the logits tile is still in registers.
@@ -96,9 +94,8 @@ typedef struct {
 } pk_gemm_desc;
 
 int pk_gemm_bf16(const pk_gemm_desc* desc, void* stream);
-/* number of partials per row that pk_gemm_bf16 writes into row_lse for an [M, N] output with these block_n / two_sm settings:
- * one per N tile on both kernel flavours */
-int pk_gemm_row_lse_parts(long long M, long long N, int block_n, int two_sm);
+/* number of partials per row that pk_gemm_bf16 writes into row_lse for an [M, N] output with this block_n: one per N tile */
+int pk_gemm_row_lse_parts(long long M, long long N, int block_n);
 
 /* ------------------------------------------------------------------------------------------
  * RNN-T loss + gradient, fused with the log-softmax over V.
@@ -137,9 +134,6 @@ int pk_rnnt_loss_fwd_bwd_lse(const void* logits, int dtype, const int* labels, c
  * weight/activation staging for pk_gemm_bf16 (replaces the implicit casts of torch autocast-free fp32). */
 int pk_cast_split(const void* src, int src_dtype, long long ld_src, void* hi, void* lo, long long ld_dst,
                   long long rows, int cols, int cols_pad, float scale, void* stream);
-/* dst[c, r] = src[r, c] for a bf16 matrix [rows, cols]: K-major copies of staged weights for the dgrad GEMMs
- * (the reference relies on cuBLAS's transposed-operand modes, e.g. nn.Linear backward). */
-int pk_transpose_bf16(const void* src, long long ld_src, void* dst, long long ld_dst, int rows, int cols, void* stream);
 /* Fused unmasked multi-head self-attention, head dim 64, bf16 (pika_b200/csrc/attention_tc.cu):
  *   O = dropout(softmax(alpha * Q K^T)) V  per (batch, head)   -- MultiHeadedAttention.forward,
  *   trainer/model/modules/multi_headed_attn.py:199-223 (scale, softmax, dropout, context) and its autograd backward,
@@ -300,17 +294,13 @@ int pk_beam_advance_lm(const float* logits, int ldv, const float* row_lse, float
 
 /* ------------------------------------------------------------------------------------------
  * Persistent LSTM layer (pika_b200/csrc/lstm_seq.cu): the whole recurrence of one nn.LSTM layer in one
- * cooperative launch (trainer/model/transducer.py:56-61,95).  B <= 32 sequences, zero initial state.
+ * cooperative launch per 32 sequences (trainer/model/transducer.py:56-61,95), zero initial state.
  *   fwd: gx f32 [B,U,4H] = x W_ih^T + b_ih + b_hh; w_hh bf16 [4H,H]; out [B,U,H] (f32|bf16);
  *        gates_save f32 [U,B,4H], cs f32 [U,B,H] are kept for the backward.
  *   bwd: dout [B,U,H] -> dG bf16 [U,B,4H] (gradient w.r.t. the pre-activation gates, time-major).
  *   ws : pk_lstm_seq_workspace_bytes(H) bytes of zero-initialised scratch (grid barrier + hidden-state exchange).
  */
 long long pk_lstm_seq_workspace_bytes(int H);
-int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, float* gates_save, float* cs, int B,
-                    int U, int H, void* ws, void* stream);
-int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const float* cs, const void* w_hh_bf16, void* dG_bf16,
-                    int B, int U, int H, void* ws, void* stream);
 /* Ragged, (bi)directional form (the LSTM encoder over pack_padded_sequence batches; trainer/model/transducer.py:38-44,82-86).
  * n_dir = 2 runs both directions of a bidirectional layer in one launch of 2 * H/8 CTAs; n_dir = 1 with reverse = 1 runs one
  * direction backwards in time.  Per direction d (buffers stacked along a leading n_dir axis): gx f32 [B,U,4H], w_hh bf16 [4H,H],
@@ -318,7 +308,7 @@ int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const 
  * lens: int32 [B] on the device, or NULL (every sequence runs all U steps).  Sequence b with length L_b is processed at
  * t = s (forward) or t = L_b - 1 - s (reverse) for steps s < L_b, from a zero state; the kernel runs max_b L_b steps.
  * Outputs and dG rows at t >= L_b are written as zeros.  ws: pk_lstm_seq_workspace_bytes(n_dir * H) bytes, zero-initialised.
- * pk_lstm_seq_fwd / _bwd are the lens = NULL, n_dir = 1, reverse = 0, ldo = H case. */
+ * The prediction net's layer is the lens = NULL, n_dir = 1, reverse = 0, ldo = H case. */
 int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, int ldo, float* gates_save, float* cs,
                        const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream);
 int pk_lstm_seq_bwd_ex(const void* dout, int dtype, int ldo, const float* gates_save, const float* cs, const void* w_hh_bf16,

@@ -267,25 +267,6 @@ PK_DEVICE void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-PK_DEVICE void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)),
-        "r"(cta)
-        : "memory");
-}
-// TMA load written to the same shared-memory offset of every CTA in `mask`; each destination's mbarrier (same offset) gets the bytes
-PK_DEVICE void tma_load_4d_mc_hint_p(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3, uint16_t mask,
-                                     uint64_t pol, uint32_t pred) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %9, 0;\n\t"
-        "@q cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7, %8;\n\t}\n" ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask), "l"(pol), "r"(pred)
-        : "memory");
-}
 
 // ---------------------------------------------------------------- predicated single-lane issue
 // The producer warps run their loops CONVERGED (all 32 lanes wait on the barriers and compute the same addresses) and only the

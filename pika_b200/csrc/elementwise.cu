@@ -1059,30 +1059,6 @@ extern "C" int pk_cast_split(const void* src, int src_dtype, long long ld_src, v
     DONE();
 }
 
-// 64x64 bf16 tiles through shared memory; both the read and the write are 128-byte row segments.
-__global__ void transpose_bf16_kernel(const __nv_bfloat16* __restrict__ src, long long ld_src, __nv_bfloat16* __restrict__ dst,
-                                      long long ld_dst, int rows, int cols) {
-    __shared__ __nv_bfloat16 tile[64][66];
-    const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
-    const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;        // 256 threads: 64 x 4
-    for (int i = ty; i < 64; i += 4) {
-        const int r = r0 + i, c = c0 + tx;
-        tile[i][tx] = (r < rows && c < cols) ? src[(long long)r * ld_src + c] : __float2bfloat16(0.f);
-    }
-    __syncthreads();
-    for (int i = ty; i < 64; i += 4) {
-        const int c = c0 + i, r = r0 + tx;
-        if (c < cols && r < rows) dst[(long long)c * ld_dst + r] = tile[tx][i];
-    }
-}
-
-extern "C" int pk_transpose_bf16(const void* src, long long ld_src, void* dst, long long ld_dst, int rows, int cols, void* stream) {
-    PK_CHECK_ARG(rows > 0 && cols > 0 && ld_src >= cols && ld_dst >= rows, "bad shape");
-    dim3 grid((cols + 63) / 64, (rows + 63) / 64);
-    transpose_bf16_kernel<<<grid, 256, 0, STREAM(stream)>>>((const __nv_bfloat16*)src, ld_src, (__nv_bfloat16*)dst, ld_dst, rows, cols);
-    DONE();
-}
-
 /* BatchNorm1d over rows of x [rows, C].  stats_ws: pk_colstats_ws_floats(C) + 2*C floats of scratch. */
 extern "C" int pk_bn_fwd(const void* x, void* y, int dtype, long long rows, int C, const float* w, const float* b, float eps,
                          int train, float momentum, float* run_mean, float* run_var, float* mean, float* rstd, float* stats_ws,
@@ -1209,9 +1185,8 @@ static void launch_gate_fwd_sliced(const void* ex, const void* py, void* h, int 
 }
 extern "C" int pk_joint_gate_fwd(const void* ex, const void* py, void* h, int dtype, int B, int T_, int U1, int H, int ld_h, void* stream) {
     PK_CHECK_ARG(H % 8 == 0 && ld_h % 8 == 0 && ld_h >= H, "H, ld_h must be multiples of 8");
-    static const bool frame_major = getenv("PK_GATE_FWD_FRAME_MAJOR") && atoi(getenv("PK_GATE_FWD_FRAME_MAJOR")) != 0;      // A/B switch
     const int ui = (U1 + 31) / 32;
-    if (!frame_major && H % 32 == 0 && ui <= 5 && T_ >= 8) {
+    if (H % 32 == 0 && ui <= 5 && T_ >= 8) {
         cudaStream_t st = STREAM(stream);
 #define PK_GATE_CASE(N) case N: { PK_DISPATCH_T(dtype, (launch_gate_fwd_sliced<T, N>(ex, py, h, B, T_, U1, H, ld_h, st))); } break;
         switch (ui) { PK_GATE_CASE(1) PK_GATE_CASE(2) PK_GATE_CASE(3) PK_GATE_CASE(4) PK_GATE_CASE(5) }
@@ -1231,9 +1206,8 @@ static void launch_gate_bwd_fused(const void* ex, const void* py, const void* dh
 extern "C" int pk_joint_gate_bwd(const void* ex, const void* py, const void* dh, void* dex, void* dpy, int dtype, int B, int T_, int U1,
                                  int H, void* stream) {
     PK_CHECK_ARG(H % 8 == 0, "H must be a multiple of 8");
-    static const bool two_pass = getenv("PK_GATE_BWD_TWO_PASS") && atoi(getenv("PK_GATE_BWD_TWO_PASS")) != 0;      // A/B switch
     const int ui = (U1 + 31) / 32;
-    if (!two_pass && H % 32 == 0 && ui <= 5) {
+    if (H % 32 == 0 && ui <= 5) {
         cudaStream_t st = STREAM(stream);
 #define PK_GATE_CASE(N) case N: { PK_DISPATCH_T(dtype, (launch_gate_bwd_fused<T, N>(ex, py, dh, dex, dpy, B, T_, U1, H, st))); } break;
         switch (ui) { PK_GATE_CASE(1) PK_GATE_CASE(2) PK_GATE_CASE(3) PK_GATE_CASE(4) PK_GATE_CASE(5) }

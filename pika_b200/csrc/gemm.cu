@@ -1,6 +1,6 @@
 // wgmma / TMA GEMM for sm_90a: C = epilogue(alpha * sum_p A_p * B_p^T).
 //
-// One persistent CTA per SM (ONE mode) or one 2-CTA cluster per pair of SMs (TWO mode), three warpgroups per CTA:
+// One persistent CTA per SM, three warpgroups per CTA:
 //   warp 0           TMA producer   (one converged warp: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
 //   warps 1-3        epilogue       (bf16 C with the plain or LSE epilogue: TMA-store the finished C tile from shared memory, hand it
 //                                    back; stage the next tile's bias)
@@ -10,14 +10,11 @@
 //                                    tile's main loop.  LSE: the row max comes from the registers being rounded; the exp-sum reads the
 //                                    warp's own rows of the C tile back while the next tile's wgmma run.  EPI_FULL and f32 C: the whole
 //                                    epilogue, registers -> swizzled smem -> TMA store / TMA reduce-add, in 64-column chunks)
-// Tile 128 x BN x 64 per CTA (BN = 64 | 128 | 256).  TWO mode: the pair works on a 256 x 256 tile, each CTA on 128 of its rows; each
-// CTA loads its own A and HALF of B, and multicasts that half into both CTAs' rings, so B is read from L2 once per pair.  A ring stage
-// is refilled only when the consumers of both CTAs have released it.  Operands may be K-major or MN-major (wgrad / dgrad / P.V use the MN-major form so no
+// Tile 128 x BN x 64 per CTA (BN = 64 | 128 | 256).  Operands may be K-major or MN-major (wgrad / dgrad / P.V use the MN-major form so no
 // transposes are ever materialised).  Up to 9 (A,B) pairs accumulate into one tile (TDNN taps, split-bf16 fp32-class mode), plus a
 // batched reduction loop (kz) for per-utterance wgrad, plus split-K.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 #include "../../include/pika_b200.h"
@@ -39,8 +36,7 @@ struct GemmParams {
     int b_off[PK_GEMM_MAX_PAIRS];
     int n_pairs, kz_count, num_k_blocks;
     int k_splits, iters_per_split;      // split-K over the flattened (pair, kz, k-block) iteration space
-    int split_major;                    // unit order: 1 = all tiles of split 0, then split 1, ... (CTAs that run together share a k-window)
-    int M, N, tiles_m, tiles_n, zb0, zb1;   // tiles_m counts 256-row tiles in TWO mode
+    int M, N, tiles_m, tiles_n, zb0, zb1;   // tiles_m / tiles_n: BM-row / BN-column tiles of one C matrix
     int a_sel2, a_sel3, b_sel2, b_sel3;
     int c_is_f32, c_accumulate;
     float alpha;
@@ -59,7 +55,7 @@ struct GemmParams {
 
 // EPI_WARPS: warps 1-3 TMA-store a whole BM x BN bf16 C tile from shared memory (bf16 C, EPI_PLAIN / EPI_LSE).
 // Otherwise the consumers stage 64-column chunks through two small buffers each.  The C tile costs BN = 256 its fourth ring stage.
-template <int BN, bool TWO, bool EPI_WARPS> struct GemmCfg {
+template <int BN, bool EPI_WARPS> struct GemmCfg {
     static constexpr int B_STAGE_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
     static constexpr int STAGES = BN == 256 ? (EPI_WARPS ? 3 : 4) : (BN == 128 ? 6 : 8);
@@ -69,8 +65,6 @@ template <int BN, bool TWO, bool EPI_WARPS> struct GemmCfg {
     static constexpr int BAR_OFF = BIAS_OFF + (EPI_WARPS ? BN * 4 : 0);
     static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;             // + barriers + alignment slack
     static constexpr int THREADS = 128 + CONSUMERS * 128;
-    static constexpr int RELEASES = CONSUMERS * (TWO ? 2 : 1);         // arrivals that free a ring stage
-    static_assert(!TWO || BN == 256, "the CTA-pair kernel works on 256 x 256 tiles");
     static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
@@ -79,13 +73,14 @@ PK_DEVICE int pick_sel(int sel, int zb0, int zb1, int kz) {
 }
 
 struct UnitCoord { int mb, nb, zb0, zb1, split; };
-// work unit -> (output tile, K split)
-PK_DEVICE UnitCoord decode_unit(const GemmParams& p, int unit, int out_tiles) {
+// work unit -> (output tile, K split).  Units run split-major: all tiles of split 0, then split 1, ..., so CTAs that run together
+// share a k-window.
+PK_DEVICE UnitCoord decode_unit(const GemmParams& p, int unit) {
     UnitCoord u;
-    int tile;
-    if (p.split_major) { u.split = unit / out_tiles; tile = unit - u.split * out_tiles; }
-    else { tile = unit / p.k_splits; u.split = unit - tile * p.k_splits; }
     const int tiles_per_z = p.tiles_m * p.tiles_n;
+    const int out_tiles = tiles_per_z * p.zb0 * p.zb1;
+    u.split = unit / out_tiles;
+    const int tile = unit - u.split * out_tiles;
     const int z = tile / tiles_per_z;
     const int r = tile - z * tiles_per_z;
     u.mb = r / p.tiles_n; u.nb = r - u.mb * p.tiles_n;
@@ -106,11 +101,11 @@ enum { EPI_PLAIN = 0, EPI_LSE = 1, EPI_FULL = 2 };
 // so the tensor-pipe idle time it causes is small.
 template <bool CF32, int EPI> constexpr bool epi_warps() { return !CF32 && EPI != EPI_FULL; }
 
-template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI, bool TWO>
-__global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
+template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI>
+__global__ void __launch_bounds__(GemmCfg<BN, epi_warps<CF32, EPI>()>::THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
     constexpr bool EW = epi_warps<CF32, EPI>();
     static_assert(EPI != EPI_LSE || (EW && BN == 256), "the row log-sum-exp epilogue works on bf16 256-wide tiles");
-    using Cfg = GemmCfg<BN, TWO, EW>;
+    using Cfg = GemmCfg<BN, EW>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
@@ -123,9 +118,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t rank = TWO ? cluster_ctarank() : 0u;                 // position in the CTA pair
-    const int worker = TWO ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;  // persistent worker (CTA or CTA pair)
-    const int n_workers = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+    const int worker = (int)blockIdx.x, n_workers = (int)gridDim.x;    // persistent CTAs stride over the work units
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < p.n_pairs; ++i) {
@@ -135,7 +128,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         tma_prefetch_desc(&p.c);
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full_bar[s], 1);              // the producer's expect_tx arrive
-            mbar_init(&empty_bar[s], Cfg::RELEASES); // one arrive per consumer warpgroup (of both CTAs in TWO mode)
+            mbar_init(&empty_bar[s], CONSUMERS);     // one arrive per consumer warpgroup
         }
         if (EW) {
             mbar_init(c_full, CONSUMERS * 4);
@@ -143,7 +136,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         }
         mbar_fence_init();
     }
-    if (TWO) cluster_sync_all(); else __syncthreads();
+    __syncthreads();
 
     const int out_tiles = p.tiles_m * p.tiles_n * p.zb0 * p.zb1;
     const int num_units = out_tiles * p.k_splits;                       // work units = tiles x K-splits
@@ -159,8 +152,8 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         uint32_t phase = 0;
         const int kzb = p.kz_count * p.num_k_blocks;
         for (int unit = worker; unit < num_units; unit += n_workers) {
-            const UnitCoord u = decode_unit(p, unit, out_tiles);
-            const int m0 = TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM, n0 = u.nb * BN;
+            const UnitCoord u = decode_unit(p, unit);
+            const int m0 = u.mb * BM, n0 = u.nb * BN;
             const int i0 = u.split * p.iters_per_split, i1 = min(k_iters_total, i0 + p.iters_per_split);
             // position in the flattened (pair, kz, k-block) space: decoded once per unit, then advanced by counters
             int pr = i0 / kzb;
@@ -184,18 +177,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
                 } else {
                     tma_load_4d_hint_p(sa, ma, &full_bar[stage], k0, m0 + a_off, a2, a3, p.pol_a, lead);
                 }
-                if (TWO) {           // this CTA's half of B (128 rows), written into both CTAs of the pair
-                    if (B_MN) {
-#pragma unroll
-                        for (int c = 0; c < BN / 128; ++c) {
-                            const int cc = (int)rank * (BN / 128) + c;
-                            tma_load_4d_mc_hint_p(sb + cc * (64 * BK * 2), mbp, &full_bar[stage], n0 + cc * 64, k0 + b_off, b2, b3, 3, p.pol_b, lead);
-                        }
-                    } else {
-                        tma_load_4d_mc_hint_p(sb + (int)rank * (BN / 2) * 128, mbp, &full_bar[stage], k0, n0 + (int)rank * (BN / 2) + b_off, b2, b3, 3,
-                                              p.pol_b, lead);
-                    }
-                } else if (B_MN) {
+                if (B_MN) {
 #pragma unroll
                     for (int c = 0; c < BN / 64; ++c)
                         tma_load_4d_hint_p(sb + c * (64 * BK * 2), mbp, &full_bar[stage], n0 + c * 64, k0 + b_off, b2, b3, p.pol_b, lead);
@@ -221,8 +203,8 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         const uint32_t store_pred = (threadIdx.x == 32) ? 1u : 0u;
         uint32_t cph = 0;
         for (int unit = worker; unit < num_units; unit += n_workers, cph ^= 1) {
-            const UnitCoord u = decode_unit(p, unit, out_tiles);
-            const int m0 = TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM, n0 = u.nb * BN;
+            const UnitCoord u = decode_unit(p, unit);
+            const int m0 = u.mb * BM, n0 = u.nb * BN;
             // the consumers read the previous tile's bias before they marked C full, which this warp waited for
             for (int c = et; c < BN; c += 96) sts_f32(sbias + c * 4, (p.bias != nullptr && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f);
             __syncwarp();
@@ -266,9 +248,8 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
     uint32_t phase = 0;
     uint32_t chunk_ctr = 0;
     uint32_t cph = 0;                                  // EW: parity of the C tile's barriers
-    // a stage is released to this CTA's producer and, in TWO mode, to the peer's (whose multicast writes into this CTA's ring)
     auto release = [&](int s) {
-        if (et == 0) { mbar_arrive(&empty_bar[s]); if (TWO) mbar_arrive_remote(&empty_bar[s], rank ^ 1u); }
+        if (et == 0) mbar_arrive(&empty_bar[s]);
     };
     // EPI_LSE: (max * log2e, sum 2^(x * log2e - max)) of each row's rounded values.  The max is taken in registers while the tile is
     // rounded; the sum of the tile the warp wrote last is read back from its own 16 rows of the C tile in LSE_SLICES slices, one
@@ -309,7 +290,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
         lse_pending = false;
     };
     for (int unit = worker; unit < num_units; unit += n_workers) {
-        const UnitCoord u = decode_unit(p, unit, out_tiles);
+        const UnitCoord u = decode_unit(p, unit);
         const int k_iters = min(k_iters_total, (u.split + 1) * p.iters_per_split) - u.split * p.iters_per_split;
         int prev = -1;
         for (int k = 0; k < k_iters; ++k) {
@@ -382,7 +363,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
                 x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, 2));
                 lse_m0 = x0 * L2E; lse_m1 = x1 * L2E;
                 lse_s0 = 0.f; lse_s1 = 0.f;
-                lse_row = (TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM) + wg * 64 + r0;
+                lse_row = u.mb * BM + wg * 64 + r0;
                 lse_nb = u.nb;
                 lse_nvalid = nvalid;
                 lse_pending = true;
@@ -392,7 +373,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
 
         // ---------------------------------------------- epilogue (EPI_FULL, f32 C)
         const int zb0 = u.zb0, zb1 = u.zb1;
-        const int m0 = (TWO ? u.mb * (2 * BM) + (int)rank * BM : u.mb * BM) + wg * 64;
+        const int m0 = u.mb * BM + wg * 64;
         const int n0 = u.nb * BN;
         if (m0 >= p.M) continue;                       // uniform across the warpgroup
         const int mrow[2] = {m0 + r0, m0 + r0 + 8};
@@ -471,8 +452,6 @@ __global__ void __launch_bounds__(GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>::THRE
     }
     if (!EW && store_pred) tma_store_wait<0>();
     }
-    // the peer may still arrive on this CTA's barriers: neither CTA of a pair leaves before both are done
-    if (TWO) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -548,105 +527,60 @@ int encode_tiled_bf16_3d(CUtensorMap* out, const void* ptr, const unsigned long 
     return 0;
 }
 
-template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI, bool TWO>
+template <bool A_MN, bool B_MN, int BN, bool CF32, int EPI>
 static int launch_gemm_e(const GemmParams& gp, int workers, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, TWO, epi_warps<CF32, EPI>()>;
-    auto kern = gemm_wgmma_kernel<A_MN, B_MN, BN, CF32, EPI, TWO>;
+    using Cfg = GemmCfg<BN, epi_warps<CF32, EPI>()>;
+    auto kern = gemm_wgmma_kernel<A_MN, B_MN, BN, CF32, EPI>;
     static bool configured = false;
     if (!configured) {
         PK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         configured = true;
     }
-    if (TWO) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(2 * workers);
-        cfg.blockDim = dim3(Cfg::THREADS);
-        cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        // a GPC whose SM count is odd cannot host a pair on every SM: launch no more persistent pairs than can be resident at once,
-        // or the extra ones would run as a second wave after the others finished all their tiles
-        static int max_pairs = -1;
-        if (max_pairs < 0) {
-            int n = 0;
-            PK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-            PK_CHECK_ARG(n > 0, "gemm: no 2-CTA cluster of the pair kernel fits on this device");
-            max_pairs = n;
-        }
-        if (workers > max_pairs) {
-            workers = max_pairs;
-            cfg.gridDim = dim3(2 * workers);
-        }
-        PK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, gp));
-    } else {
-        kern<<<workers, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(gp);
-        PK_CHECK_LAUNCH();
-    }
+    kern<<<workers, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(gp);
+    PK_CHECK_LAUNCH();
     count_launch();
     return 0;
 }
 
-template <bool A_MN, bool B_MN, int BN, bool CF32, bool TWO>
+template <bool A_MN, bool B_MN, int BN, bool CF32>
 static int launch_gemm(const GemmParams& gp, int workers, cudaStream_t stream) {
     if (gp.row_lse != nullptr) {
         // the row log-sum-exp epilogue exists for the joint projection's layout only: K-major operands, bf16 C, 256-wide tiles
-        if constexpr (!A_MN && !B_MN && BN == 256 && !CF32) return launch_gemm_e<false, false, 256, false, EPI_LSE, TWO>(gp, workers, stream);
+        if constexpr (!A_MN && !B_MN && BN == 256 && !CF32) return launch_gemm_e<false, false, 256, false, EPI_LSE>(gp, workers, stream);
         set_last_error("gemm: row_lse needs K-major operands, a bf16 C and block_n = 256");
         return -1;
     }
-    if (gp.drop_thresh != 0u || gp.aux_mode != PK_AUX_NONE) return launch_gemm_e<A_MN, B_MN, BN, CF32, EPI_FULL, TWO>(gp, workers, stream);
-    return launch_gemm_e<A_MN, B_MN, BN, CF32, EPI_PLAIN, TWO>(gp, workers, stream);
+    if (gp.drop_thresh != 0u || gp.aux_mode != PK_AUX_NONE) return launch_gemm_e<A_MN, B_MN, BN, CF32, EPI_FULL>(gp, workers, stream);
+    return launch_gemm_e<A_MN, B_MN, BN, CF32, EPI_PLAIN>(gp, workers, stream);
 }
 
-template <int BN, bool TWO>
+template <int BN>
 static int dispatch_major(const GemmParams& gp, int a_mn, int b_mn, int workers, cudaStream_t stream) {
     if (gp.c_is_f32) {
-        if (!a_mn && !b_mn) return launch_gemm<false, false, BN, true, TWO>(gp, workers, stream);
-        if (!a_mn && b_mn) return launch_gemm<false, true, BN, true, TWO>(gp, workers, stream);
-        if (a_mn && !b_mn) return launch_gemm<true, false, BN, true, TWO>(gp, workers, stream);
-        return launch_gemm<true, true, BN, true, TWO>(gp, workers, stream);
+        if (!a_mn && !b_mn) return launch_gemm<false, false, BN, true>(gp, workers, stream);
+        if (!a_mn && b_mn) return launch_gemm<false, true, BN, true>(gp, workers, stream);
+        if (a_mn && !b_mn) return launch_gemm<true, false, BN, true>(gp, workers, stream);
+        return launch_gemm<true, true, BN, true>(gp, workers, stream);
     }
-    if (!a_mn && !b_mn) return launch_gemm<false, false, BN, false, TWO>(gp, workers, stream);
-    if (!a_mn && b_mn) return launch_gemm<false, true, BN, false, TWO>(gp, workers, stream);
-    if (a_mn && !b_mn) return launch_gemm<true, false, BN, false, TWO>(gp, workers, stream);
-    return launch_gemm<true, true, BN, false, TWO>(gp, workers, stream);
+    if (!a_mn && !b_mn) return launch_gemm<false, false, BN, false>(gp, workers, stream);
+    if (!a_mn && b_mn) return launch_gemm<false, true, BN, false>(gp, workers, stream);
+    if (a_mn && !b_mn) return launch_gemm<true, false, BN, false>(gp, workers, stream);
+    return launch_gemm<true, true, BN, false>(gp, workers, stream);
 }
 
-static int env_int(const char* name, int dflt) {
-    const char* e = getenv(name);
-    return e ? atoi(e) : dflt;
-}
 static uint64_t policy_of(int code) { return code == 1 ? kL2EvictFirst : (code == 2 ? kL2EvictLast : kL2EvictNormal); }
 
-// Kernel flavour for a problem: tile width and whether the CTA-pair kernel runs it.  One place, shared by the launch and by
-// pk_gemm_row_lse_parts (the caller sizes the partials buffer from it).
-struct GemmPlan { int bn; bool two; };
-static GemmPlan plan_gemm(long long M, long long N, int block_n, int two_sm_req) {
-    GemmPlan pl;
-    pl.bn = block_n ? block_n : (N <= 64 ? 64 : (N <= 128 ? 128 : 256));
-    // PK_GEMM_2SM=1 lets the automatic choice pick the pair kernel.  Off by default: on an H100 80GB HBM3 (700 W limit), with the
-    // epilogue on its own warps, it took 31.2 ms on the joint's fc2 forward with row LSE against 28.0 ms on single CTAs, 27.5 against
-    // 20.6 ms on the fc2 dgrad and 34.8 against 20.9 ms on the fc2 wgrad (scripts/gemm_lab.py fc2, one run each)
-    static int use_2sm = -1;
-    if (use_2sm < 0) use_2sm = env_int("PK_GEMM_2SM", 0);
-    static int min_tiles = -1;               // smallest number of 256 x 256 tiles handed to the pair kernel
-    if (min_tiles < 0) min_tiles = env_int("PK_GEMM_2SM_MIN_TILES", 1);
-    const long long tiles2 = ((M + 255) / 256) * ((N + 255) / 256);
-    const int want = two_sm_req < 0 ? 0 : (two_sm_req > 0 ? 1 : (use_2sm && tiles2 >= min_tiles));
-    pl.two = want && pl.bn == 256 && M > 128;
-    return pl;
-}
+// Tile width for an [M, N] output.  One place, shared by the launch and by pk_gemm_row_lse_parts (the caller sizes the partials
+// buffer from it).
+static int plan_block_n(long long N, int block_n) { return block_n ? block_n : (N <= 64 ? 64 : (N <= 128 ? 128 : 256)); }
 
 }  // namespace pk
 
-// every row's columns of an N tile belong to one CTA on both flavours: one partial per N tile
-extern "C" int pk_gemm_row_lse_parts(long long M, long long N, int block_n, int two_sm) {
-    const pk::GemmPlan pl = pk::plan_gemm(M, N, block_n ? block_n : 256, two_sm);
-    return (int)((N + pl.bn - 1) / pl.bn);
+// every row's columns of an N tile belong to one CTA: one partial per N tile
+extern "C" int pk_gemm_row_lse_parts(long long M, long long N, int block_n) {
+    (void)M;
+    const int bn = pk::plan_block_n(N, block_n ? block_n : 256);
+    return (int)((N + bn - 1) / bn);
 }
 
 extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
@@ -662,9 +596,7 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
     PK_CHECK_ARG(M > 0 && N > 0, "empty C");
     PK_CHECK_ARG(d->aux == nullptr || d->aux_mode == PK_AUX_NONE || (N % 8 == 0), "aux epilogue needs N % 8 == 0");
     PK_CHECK_ARG(d->block_n == 0 || d->block_n == 64 || d->block_n == 128 || d->block_n == 256, "block_n must be 64, 128 or 256");
-    const GemmPlan plan = plan_gemm(M, N, d->row_lse ? (d->block_n ? d->block_n : 256) : d->block_n, d->two_sm);
-    const int bn = plan.bn;
-    const bool two_sm = plan.two;       // CTA-pair kernel: 256 x 256 per pair (needs M > 128 so that the second CTA has rows)
+    const int bn = plan_block_n(N, d->row_lse ? (d->block_n ? d->block_n : 256) : d->block_n);
 
     {   // the tensor-map encoder is a driver-API call: make sure this host thread (e.g. an autograd worker) has the primary context bound
         static thread_local bool ctx_ready = false;
@@ -679,7 +611,7 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
         PK_CHECK_ARG(ka == K && kb == K, "all pairs must share the reduction extent K");
         int rc = make_map(&gp.a[i], d->a[i], 0, 64, d->a_mn_major ? 64 : BM, "A");
         if (rc) return rc;
-        rc = make_map(&gp.b[i], d->b[i], 0, 64, d->b_mn_major ? 64 : (two_sm ? bn / 2 : bn), "B");   // a CTA of a pair loads half of B
+        rc = make_map(&gp.b[i], d->b[i], 0, 64, d->b_mn_major ? 64 : bn, "B");
         if (rc) return rc;
         gp.a_off[i] = d->a_row_off[i];
         gp.b_off[i] = d->b_row_off[i];
@@ -693,7 +625,7 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
     gp.num_k_blocks = (int)((K + BK - 1) / BK);
     gp.M = (int)M;
     gp.N = (int)N;
-    gp.tiles_m = (int)(two_sm ? (M + 2 * BM - 1) / (2 * BM) : (M + BM - 1) / BM);
+    gp.tiles_m = (int)((M + BM - 1) / BM);
     gp.tiles_n = (int)((N + bn - 1) / bn);
     gp.zb0 = (int)d->c.dim[2];
     gp.zb1 = (int)d->c.dim[3];
@@ -721,54 +653,34 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
                  "row_lse needs a 2-D bf16 C with N % 8 == 0, block_n = 256, no dropout / aux");
     {   // L2 eviction priorities by stream size: an operand that fits in L2 many times over (a weight matrix) is kept with evict_last,
         // a multi-GB streamed operand (the wgrad's activations) is not; a C stream much larger than L2 leaves first.
-        // PK_GEMM_L2_HINTS=0 -> all normal.
-        static int hints = -1;
-        if (hints < 0) hints = env_int("PK_GEMM_L2_HINTS", 1);
         const long long K_ = (long long)gp.num_k_blocks * BK * gp.kz_count;
         const long long a_bytes = M * K_ * 2 * gp.n_pairs, b_bytes = N * K_ * 2 * gp.n_pairs;
         const long long c_bytes = M * N * (gp.c_is_f32 ? 4 : 2) * gp.zb0 * gp.zb1;
         const long long small = 32ll << 20, big = 256ll << 20;
-        gp.pol_a = policy_of(hints && a_bytes <= small && gp.zb0 * gp.zb1 == 1 ? 2 : 0);
-        gp.pol_b = policy_of(hints && b_bytes <= small && gp.zb0 * gp.zb1 == 1 ? 2 : 0);
-        gp.pol_c = policy_of(hints && c_bytes >= big ? 1 : 0);
+        gp.pol_a = policy_of(a_bytes <= small && gp.zb0 * gp.zb1 == 1 ? 2 : 0);
+        gp.pol_b = policy_of(b_bytes <= small && gp.zb0 * gp.zb1 == 1 ? 2 : 0);
+        gp.pol_c = policy_of(c_bytes >= big ? 1 : 0);
     }
 
     const long long out_tiles = (long long)gp.tiles_m * gp.tiles_n * gp.zb0 * gp.zb1;
-    const int workers_max = two_sm ? num_sms() / 2 : num_sms();
+    const int workers_max = num_sms();
     // split-K: under-filled grids with a long reduction (wgrad, the LSTM's recurrent dgrad) are cut along the
     // flattened (pair, kz, k-block) axis; partial tiles are combined with TMA reduce-add into a zeroed f32 C.
     const int k_iters_total = gp.n_pairs * gp.kz_count * gp.num_k_blocks;
     int splits = 1;
     const bool plain_epi = d->bias == nullptr && d->act == PK_ACT_NONE && d->drop_p == 0.f && gp.aux_mode == PK_AUX_NONE;
     if (d->k_splits > 0) splits = d->k_splits;
-    else if (gp.c_is_f32 && plain_epi && gp.zb0 == 1 && gp.zb1 == 1 && k_iters_total >= 16) {
-        // PK_GEMM_SPLIT_MODE: 1 (default) = the split count (>= 8 k-blocks each, <= PK_GEMM_SPLIT_MAX = 16) that wastes the least of the last
-        // wave, preferring fewer splits on ties | 0 = fill about two waves
-        static int mode = -1, smax = -1;
-        if (mode < 0) { mode = env_int("PK_GEMM_SPLIT_MODE", 1); smax = env_int("PK_GEMM_SPLIT_MAX", 16); }
+    else if (gp.c_is_f32 && plain_epi && gp.zb0 == 1 && gp.zb1 == 1 && k_iters_total >= 16 && out_tiles < 6 * workers_max) {
+        // the split count (>= 8 k-blocks each, <= 16) that wastes the least of the last wave, preferring fewer splits on ties
         const int w = workers_max;
-        if (mode == 0) {
-            if (out_tiles < 2 * w) {
-                splits = (int)((2 * w + out_tiles / 2) / out_tiles);
-                if (splits > k_iters_total / 8) splits = k_iters_total / 8;
-                if (splits > 64) splits = 64;
-            }
-        } else if (out_tiles < 6 * w) {
-            double best = 0.0;
-            for (int sp = 1; sp <= smax && sp <= k_iters_total / 8; ++sp) {
-                const long long units = out_tiles * sp;
-                const double eff = (double)units / (double)(((units + w - 1) / w) * w);
-                if (eff > best + 0.02) { best = eff; splits = sp; }
-            }
+        double best = 0.0;
+        for (int sp = 1; sp <= 16 && sp <= k_iters_total / 8; ++sp) {
+            const long long units = out_tiles * sp;
+            const double eff = (double)units / (double)(((units + w - 1) / w) * w);
+            if (eff > best + 0.02) { best = eff; splits = sp; }
         }
-        if (splits < 1) splits = 1;
     }
     PK_CHECK_ARG(splits == 1 || (gp.c_is_f32 && plain_epi && gp.zb0 == 1 && gp.zb1 == 1), "split-K needs a plain f32 2-D C");
-    {
-        static int sm = -1;
-        if (sm < 0) sm = env_int("PK_GEMM_SPLIT_MAJOR", 1);
-        gp.split_major = sm;
-    }
     gp.iters_per_split = (k_iters_total + splits - 1) / splits;
     gp.k_splits = (k_iters_total + gp.iters_per_split - 1) / gp.iters_per_split;
     if (gp.k_splits > 1) {
@@ -780,8 +692,7 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
     PK_CHECK_ARG(num_tiles < (1ll << 31), "too many tiles");
     int grid = workers_max;
     if (num_tiles < grid) grid = (int)num_tiles;
-    if (two_sm) return dispatch_major<256, true>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
-    if (bn == 64) return dispatch_major<64, false>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
-    if (bn == 128) return dispatch_major<128, false>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
-    return dispatch_major<256, false>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
+    if (bn == 64) return dispatch_major<64>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
+    if (bn == 128) return dispatch_major<128>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
+    return dispatch_major<256>(gp, d->a_mn_major, d->b_mn_major, grid, stream);
 }

@@ -55,44 +55,21 @@ PK_DEVICE void bulk_g2s_mc(void* smem_dst, const void* gsrc, uint32_t bytes, uin
 }
 PK_DEVICE void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
-// mode 0: membar.gl + relaxed atomic + volatile polling + membar.gl (round 1).  mode 1 (default): release reduction, acquire polling loads
-// (this CTA's writes of the step are ordered before its arrival by bar.sync + cumulativity; no separate membar.gl on either side).
-// mode 3: hierarchical (measured SLOWER than mode 1: 6.49 vs 5.81 us per forward step, two cluster barriers cost more than the contention
-// they remove) -- the hardware cluster barrier gathers the cn CTAs of a cluster, ONE
-// thread per cluster does the mode-1 handshake on the global counter (128 -> 16 serialised atomics on one line), a second cluster
-// barrier releases the peers.  Causality chains through the cluster-scope and gpu-scope release/acquire pairs.  PK_LSTM_BARRIER selects.
+// Release reduction on the counter, acquire polling loads: this CTA's writes of the step are ordered before its arrival by bar.sync +
+// cumulativity, so no separate membar.gl is needed on either side.  (A hierarchical form -- a hardware cluster barrier, one thread per
+// cluster doing this handshake on the counter, a second cluster barrier to release the peers -- measured slower: 6.49 against 5.81 us
+// per forward step; the two cluster barriers cost more than the contention they remove.)
 // ``nct`` = CTAs that meet at this barrier: the CTAs of one direction (a bidirectional launch keeps one counter per direction, so
 // the two recurrences never wait on each other).
-PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, int mode, uint32_t cn, uint32_t cr, unsigned int nct) {
-    if (mode == 3 && cn > 1) {
-        cluster_sync_all();
-        if (cr == 0 && threadIdx.x == 0) {
-            const unsigned int target = (nct / cn) * step_index;
-            asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-            unsigned int seen;
-            do {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-            } while (seen < target);
-        }
-        cluster_sync_all();
-        return;
-    }
+PK_DEVICE void grid_barrier(unsigned int* counter, unsigned int step_index, unsigned int nct) {
     const unsigned int target = nct * step_index;
     __syncthreads();
     if (threadIdx.x == 0) {
-        if (mode == 0) {
-            __threadfence();
-            atomicAdd(counter, 1u);
-            while (*reinterpret_cast<volatile unsigned int*>(counter) < target) {
-            }
-            __threadfence();
-        } else {
-            asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-            unsigned int seen;
-            do {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-            } while (seen < target);
-        }
+        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
+        unsigned int seen;
+        do {
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
+        } while (seen < target);
     }
     __syncthreads();
 }
@@ -141,7 +118,7 @@ template <typename T>
 __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float* __restrict__ gx, const __nv_bfloat16* __restrict__ w_hh,
                                                                      T* __restrict__ out, int ldo, __nv_bfloat16* hx, float* __restrict__ gates_save,
                                                                      float* __restrict__ cs, const int* __restrict__ lens, int B, int Bt, int U,
-                                                                     int H, int reverse, unsigned int* counter, int bar_mode) {
+                                                                     int H, int reverse, unsigned int* counter) {
     // B = sequences of this launch (<= 32); Bt = sequences of the whole batch: gates_save / cs are time-major [U, Bt, .] and the
     // caller passes them already offset to this launch's first sequence (batches larger than 32 run as independent launches)
     extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -247,7 +224,7 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_fwd_kernel(const float
             hx[(long long)(s & 1) * LS_MB * H + (long long)cb * H + j0 + cj] = __float2bfloat16_rn(0.f);
             if (cb < B) out[((long long)cb * U + s) * ldo + j0 + cj] = from_f32<T>(0.f);      // s >= L_b: a padded position
         }
-        if (s + 1 < S) grid_barrier(counter, (unsigned int)(s + 1), bar_mode, cn, cr, dir.nct);
+        if (s + 1 < S) grid_barrier(counter, (unsigned int)(s + 1), dir.nct);
     }
     if (cb < B)
         for (int t = S; t < U; ++t) out[((long long)cb * U + t) * ldo + j0 + cj] = from_f32<T>(0.f);     // past this launch's longest sequence
@@ -262,7 +239,7 @@ template <typename T>
 __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __restrict__ dout, int ldo, const float* __restrict__ gates_save,
                                                                      const float* __restrict__ cs, const __nv_bfloat16* __restrict__ w_hh,
                                                                      __nv_bfloat16* dG, const __nv_bfloat16* zrow, const int* __restrict__ lens,
-                                                                     int B, int Bt, int U, int H, int reverse, unsigned int* counter, int bar_mode) {
+                                                                     int B, int Bt, int U, int H, int reverse, unsigned int* counter) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
     const int G4 = 4 * H;
     const int PW = G4 + LS_PAD;                                                  // Wt_s pitch
@@ -395,17 +372,13 @@ __global__ void __launch_bounds__(LS_THREADS, 1) lstm_seq_bwd_kernel(const T* __
             __nv_bfloat16* d = dG + ((long long)s * Bt + cb) * G4 + j0 + cj;     // s >= L_b: a padded position
             d[0] = d[H] = d[2 * H] = d[3 * H] = __float2bfloat16_rn(0.f);
         }
-        if (s > 0) grid_barrier(counter, (unsigned int)(S - s), bar_mode, cn, cr, dir.nct);
+        if (s > 0) grid_barrier(counter, (unsigned int)(S - s), dir.nct);
     }
 }
 }  // namespace pk
 
 using namespace pk;
 
-static int lstm_bar_mode() {
-    static const int m = getenv("PK_LSTM_BARRIER") ? atoi(getenv("PK_LSTM_BARRIER")) : 1;
-    return m;
-}
 // cooperative launch with thread-block clusters of ``cs`` CTAs; cs is the largest of 8/4/2 for which the whole grid is co-resident
 static int lstm_launch(const void* fn, int grid, int smem, void** args, cudaStream_t st, int* cluster_cache) {
     cudaLaunchConfig_t cfg = {};
@@ -413,9 +386,8 @@ static int lstm_launch(const void* fn, int grid, int smem, void** args, cudaStre
     cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeCooperative; attr[0].val.cooperative = 1;
     if (*cluster_cache == 0) {
-        static const int want = getenv("PK_LSTM_CLUSTER") ? atoi(getenv("PK_LSTM_CLUSTER")) : 8;
         int pick = 1;
-        for (int cs = want; cs >= 2; cs >>= 1) {
+        for (int cs = 8; cs >= 2; cs >>= 1) {
             if (grid % cs) continue;
             attr[1].id = cudaLaunchAttributeClusterDimension; attr[1].val.clusterDim.x = cs; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
             cfg.attrs = attr; cfg.numAttrs = 2;
@@ -457,7 +429,6 @@ extern "C" int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* 
     const void* fn = out_dtype == PK_BF16 ? (const void*)lstm_seq_fwd_kernel<__nv_bfloat16> : (const void*)lstm_seq_fwd_kernel<float>;
     PK_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const size_t es = out_dtype == PK_BF16 ? 2 : 4;
-    int bar_mode = lstm_bar_mode();
     const int grid = n_dir * H / LS_HJ;
     static int cluster_f[2][2][64] = {};
     for (int b0 = 0; b0 < B; b0 += LS_MB) {                    // sequences are independent: 32 per cooperative launch
@@ -469,7 +440,7 @@ extern "C" int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* 
         const int* lens_c = lens ? lens + b0 : nullptr;
         PK_CHECK_CUDA(cudaMemsetAsync(counter, 0, 256, st));
         void* args[] = {(void*)&gx_c, (void*)&w, (void*)&out_c, (void*)&ldo, (void*)&hx, (void*)&gs_c, (void*)&cs_c, (void*)&lens_c, (void*)&nb,
-                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter, (void*)&bar_mode};
+                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter};
         rc = lstm_launch(fn, grid, smem, args, st, lstm_cluster_slot(cluster_f, out_dtype == PK_BF16 ? 0 : 1, n_dir, H));
         if (rc) return rc;
         count_launch();
@@ -490,7 +461,6 @@ extern "C" int pk_lstm_seq_bwd_ex(const void* dout, int dtype, int ldo, const fl
     const void* fn = dtype == PK_BF16 ? (const void*)lstm_seq_bwd_kernel<__nv_bfloat16> : (const void*)lstm_seq_bwd_kernel<float>;
     PK_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const size_t es = dtype == PK_BF16 ? 2 : 4;
-    int bar_mode = lstm_bar_mode();
     const int grid = n_dir * H / LS_HJ;
     static int cluster_b[2][2][64] = {};
     for (int b0 = 0; b0 < B; b0 += LS_MB) {
@@ -502,18 +472,10 @@ extern "C" int pk_lstm_seq_bwd_ex(const void* dout, int dtype, int ldo, const fl
         const int* lens_c = lens ? lens + b0 : nullptr;
         PK_CHECK_CUDA(cudaMemsetAsync(counter, 0, 256, st));
         void* args[] = {(void*)&dout_c, (void*)&ldo, (void*)&gs_c, (void*)&cs_c, (void*)&w, (void*)&dg, (void*)&zrow, (void*)&lens_c, (void*)&nb,
-                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter, (void*)&bar_mode};
+                        (void*)&Bt, (void*)&U, (void*)&H, (void*)&reverse, (void*)&counter};
         rc = lstm_launch(fn, grid, smem, args, st, lstm_cluster_slot(cluster_b, dtype == PK_BF16 ? 0 : 1, n_dir, H));
         if (rc) return rc;
         count_launch();
     }
     return 0;
-}
-extern "C" int pk_lstm_seq_fwd(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, float* gates_save, float* cs, int B,
-                               int U, int H, void* ws, void* stream) {
-    return pk_lstm_seq_fwd_ex(gx, w_hh_bf16, out, out_dtype, H, gates_save, cs, nullptr, B, U, H, 1, 0, ws, stream);
-}
-extern "C" int pk_lstm_seq_bwd(const void* dout, int dtype, const float* gates_save, const float* cs, const void* w_hh_bf16, void* dG_bf16,
-                               int B, int U, int H, void* ws, void* stream) {
-    return pk_lstm_seq_bwd_ex(dout, dtype, H, gates_save, cs, w_hh_bf16, dG_bf16, nullptr, B, U, H, 1, 0, ws, stream);
 }

@@ -492,21 +492,19 @@ extern "C" long long pk_rnnt_loss_workspace_bytes(int B, int T, int U1) {
     const long long nodes = (long long)B * T * U1;
     return (2 * skew + 3 * nodes) * 4 + 2 * skew * 8 + 256;
 }
-// gradient-kernel grid: shared by the launch and by the column-sum workspace query
-static void rnnt_grad_grid(long long rows, int* ru_out, int* ctas_per_sm_out, long long* rpc_out, int* ggrid_out, int* variant_out) {
-    static int variant = -1;                         // tuning hook (PK_RNNT_GRAD_VARIANT=0..3), default chosen by measurement
-    if (variant < 0) { const char* e = getenv("PK_RNNT_GRAD_VARIANT"); variant = e ? atoi(e) : 1; }
-    const int ru = (variant == 0) ? 1 : (variant == 3 ? 4 : 2);
-    const int ctas_per_sm = (variant == 2) ? 2 : 3;
-    const int gcta = pk::num_sms() * ctas_per_sm * 4;
+// gradient-kernel grid: 3 CTAs per SM x 4 waves, rows per CTA a multiple of the 2 rows each thread keeps in flight.  Shared by the
+// launch and by the column-sum workspace query.
+static void rnnt_grad_grid(long long rows, long long* rpc_out, int* ggrid_out) {
+    const int ru = 2;
+    const int gcta = pk::num_sms() * 3 * 4;
     long long rpc = (rows + gcta - 1) / gcta;
     rpc = (rpc + ru - 1) / ru * ru;
     if (rpc > 2048) rpc = 2048;                      // 16 bytes of shared memory per row
-    *ru_out = ru; *ctas_per_sm_out = ctas_per_sm; *rpc_out = rpc; *ggrid_out = (int)((rows + rpc - 1) / rpc); *variant_out = variant;
+    *rpc_out = rpc; *ggrid_out = (int)((rows + rpc - 1) / rpc);
 }
 extern "C" long long pk_rnnt_loss_colsum_workspace_bytes(int B, int T, int U1, int ldv) {
-    int ru, cps, ggrid, variant; long long rpc;
-    rnnt_grad_grid((long long)B * T * U1, &ru, &cps, &rpc, &ggrid, &variant);
+    int ggrid; long long rpc;
+    rnnt_grad_grid((long long)B * T * U1, &rpc, &ggrid);
     return (long long)ggrid * ldv * 4;
 }
 
@@ -568,9 +566,8 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
     PK_CHECK_LAUNCH(); count_launch();
     if (dlogits != nullptr) {
         PK_CHECK_ARG(ldv <= 8192, "V too large for the gradient kernel (V <= 8192)");
-        int ru, ctas_per_sm, ggrid, variant; long long rpc;
-        rnnt_grad_grid(rows, &ru, &ctas_per_sm, &rpc, &ggrid, &variant);
-        (void)ru; (void)ctas_per_sm;
+        int ggrid; long long rpc;
+        rnnt_grad_grid(rows, &rpc, &ggrid);
         float* cs_part = nullptr;                        // [ggrid][ldv] per-CTA partial column sums, after the lattice workspace
         if (dlogits_colsum) {
             const long long base_bytes = pk_rnnt_loss_workspace_bytes(B, T, U1);
@@ -582,14 +579,8 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
 #define PK_GRAD_LAUNCH(TT, RU, MB)                                                                                         \
         rnnt_grad_kernel<TT, RU, MB><<<ggrid, GRAD_THREADS, gsmem, stream>>>(reinterpret_cast<const TT*>(logits), labels, label_lens, d, lse, \
                                                                             gb, gl, reinterpret_cast<TT*>(dlogits), cs_part, rpc)
-        if (dtype == PK_BF16) {
-            if (variant == 0) PK_GRAD_LAUNCH(__nv_bfloat16, 1, 3);
-            else if (variant == 2) PK_GRAD_LAUNCH(__nv_bfloat16, 2, 2);
-            else if (variant == 3) PK_GRAD_LAUNCH(__nv_bfloat16, 4, 2);
-            else PK_GRAD_LAUNCH(__nv_bfloat16, 2, 3);
-        } else {
-            PK_GRAD_LAUNCH(float, 2, 2);
-        }
+        if (dtype == PK_BF16) PK_GRAD_LAUNCH(__nv_bfloat16, 2, 3);
+        else PK_GRAD_LAUNCH(float, 2, 2);
 #undef PK_GRAD_LAUNCH
         PK_CHECK_LAUNCH(); count_launch();
         if (dlogits_colsum) {

@@ -15,7 +15,6 @@ trainer/model/rnnt_tdnn_transformer.py:73-89, trainer/model/modules/{transformer
 multi_headed_attn.py:110-241, position_ffn.py:27-39}.
 """
 import math
-import os
 import weakref
 
 import torch
@@ -142,43 +141,6 @@ def stage_conv1d_weight(weight, ld):
     return parts
 
 
-# opt-in: isolated dgrads can be faster with a K-major B, but in the full step the extra transposes cancel the gain
-_DGRAD_KMAJOR = os.environ.get("PK_DGRAD_KMAJOR", "0") != "0"
-
-
-def transposed_parts(parts):
-    """Transposed bf16 copies [K, N] of staged weight parts [N, K] so a dgrad reads its B operand K-major
-    (PK_DGRAD_KMAJOR=1).  The copy hangs off the staged tensor, so it
-    lives exactly as long as that staging does."""
-    out = []
-    for p in parts:
-        t = getattr(p, "_pk_transposed", None)
-        if t is None:
-            t = torch.empty(p.shape[1], p.shape[0], dtype=torch.bfloat16, device=p.device)
-            K.transpose_bf16(p, t)
-            p._pk_transposed = t
-        out.append(t)
-    return out
-
-
-def dgrad_b(parts, rows=None, cols=None):
-    """B operand of dx = dy @ W for staged W parts [N, K] (optionally the sub-block rows x cols):
-    returns (b_parts, b_mn)."""
-    if _DGRAD_KMAJOR and all(p.shape[0] % 8 == 0 for p in parts):
-        t = transposed_parts(parts)                      # [K, N]
-        if cols is not None:
-            t = [p[cols[0]:cols[1]] for p in t]
-        if rows is not None:
-            t = [p[:, rows[0]:rows[1]] for p in t]
-        return t, False
-    sub = parts
-    if rows is not None:
-        sub = [p[rows[0]:rows[1]] for p in sub]
-    if cols is not None:
-        sub = [p[:, cols[0]:cols[1]] for p in sub]
-    return sub, True
-
-
 def _cat_bias(params):
     """Concatenated f32 bias for a row-concatenated weight (cached like the weights)."""
     if len(params) == 1:
@@ -276,11 +238,11 @@ class LinearFn(torch.autograd.Function):
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
-            wb, wmn = dgrad_b(ctx.w_parts)
+            # dx = dy @ W reads the staged W [N, K] as an MN-major B operand
             if ctx.mask_input_scale > 0:
-                gemm_parts([d_parts], [wb], dx, b_mn=wmn, aux=x, aux_mode=K.AUX_MASK_NZ, aux_scale=ctx.mask_input_scale)
+                gemm_parts([d_parts], [ctx.w_parts], dx, b_mn=True, aux=x, aux_mode=K.AUX_MASK_NZ, aux_scale=ctx.mask_input_scale)
             else:
-                gemm_parts([d_parts], [wb], dx, b_mn=wmn)
+                gemm_parts([d_parts], [ctx.w_parts], dx, b_mn=True)
             if dx.shape[1] != x.shape[1]:
                 dx = dx[:, :x.shape[1]]
         # dW_i = dpre[:, rows_i]^T x ; db_i = colsum(dpre)[rows_i]
@@ -345,15 +307,12 @@ class TdnnFn(torch.autograd.Function):
             dpre = torch.empty_like(y)
             K.mask_nz(dy.contiguous(), y, dpre, 1.0)
         d_parts = stage_act(dpre)
-        b_taps, wmn = [], True
-        for k in range(3):
-            bt, wmn = dgrad_b(ctx.w_parts, cols=(k * C, (k + 1) * C))
-            b_taps.append(bt)
+        b_taps = [[p[:, k * C:(k + 1) * C] for p in ctx.w_parts] for k in range(3)]
         dx = None
         if ctx.needs_input_grad[0]:
             if stride == 1:
                 dx = torch.empty_like(x)
-                gemm_parts([d_parts] * 3, b_taps, dx, b_mn=wmn, a_sel=(K.SEL_ZB0, K.SEL_ZERO),
+                gemm_parts([d_parts] * 3, b_taps, dx, b_mn=True, a_sel=(K.SEL_ZB0, K.SEL_ZERO),
                            b_sel=(K.SEL_ZERO, K.SEL_ZERO), a_row_off=[0, -dil, -2 * dil])
             else:
                 # rows tau = k*dil + t*stride of the three taps are disjoint when the residues differ
@@ -361,7 +320,7 @@ class TdnnFn(torch.autograd.Function):
                 dx = torch.zeros_like(x)
                 span = (t_out - 1) * stride + 1
                 for k in range(3):
-                    gemm_parts([d_parts], [b_taps[k]], dx[:, k * dil: k * dil + span: stride, :], b_mn=wmn,
+                    gemm_parts([d_parts], [b_taps[k]], dx[:, k * dil: k * dil + span: stride, :], b_mn=True,
                                a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO))
         gw = grad_of(ctx.weight).view(N, 3 * C)
         span = (t_out - 1) * stride + 1
@@ -411,11 +370,8 @@ class CausalConvFn(torch.autograd.Function):
             dx = _new((B, T, ld), dtype=torch.float32 if len(d_parts) > 1 else None, like=y)
             for k0 in range(0, Kw, per):
                 ks = list(range(k0, min(Kw, k0 + per)))
-                b_taps, wmn = [], True
-                for k in ks:
-                    bt, wmn = dgrad_b(ctx.w_parts, cols=(k * ld, (k + 1) * ld))
-                    b_taps.append(bt)
-                gemm_parts([d_parts] * len(ks), b_taps, dx, b_mn=wmn, a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO),
+                b_taps = [[p[:, k * ld:(k + 1) * ld] for p in ctx.w_parts] for k in ks]
+                gemm_parts([d_parts] * len(ks), b_taps, dx, b_mn=True, a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO),
                            a_row_off=[Kw - 1 - k for k in ks], accumulate=k0 > 0)
         gw = torch.empty(N, Kw * ld, dtype=torch.float32, device=y.device)
         gemm_parts([d_parts], [ctx.a_parts], gw, a_mn=True, b_mn=True, a_sel=(K.SEL_KZ, K.SEL_ZERO), b_sel=(K.SEL_KZ, K.SEL_ZERO),
@@ -472,8 +428,7 @@ class LayerNormFn(torch.autograd.Function):
         return dx, None, None, None
 
 
-_FUSED_ATTN = os.environ.get("PK_FUSED_ATTN", "1") != "0"
-_FOLD_MASKS = os.environ.get("PK_FOLD_MASKS", "1") != "0"
+_FUSED_ATTN = True          # tests/test_layers_gpu.py and scripts/attn_bench.py set False to run the materialised path on every shape
 
 
 class AttentionFn(torch.autograd.Function):
@@ -707,12 +662,8 @@ class LstmLayerFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             # dx = sum_d dG_d W_ih_d: one GEMM over the directions' (A, B) pairs
             dx = torch.empty_like(x)
-            taps, wbs, wmn = [], [], True
-            for d in range(n_dir):
-                wb, wmn = dgrad_b(ctx.wih_parts[d])
-                taps.append([p[d] for p in dg_all])
-                wbs.append(wb)
-            gemm_parts(taps, wbs, dx.permute(1, 0, 2), b_mn=wmn, a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO))
+            taps = [[p[d] for p in dg_all] for d in range(n_dir)]
+            gemm_parts(taps, ctx.wih_parts, dx.permute(1, 0, 2), b_mn=True, a_sel=(K.SEL_ZB0, K.SEL_ZERO), b_sel=(K.SEL_ZERO, K.SEL_ZERO))
         return (dx, None) + (None,) * (4 * n_dir)
 
 
@@ -749,9 +700,9 @@ def _ldv(V):
     return (V + 7) // 8 * 8
 
 
-# on by default: the fc2 GEMM epilogue does more work, and the 13.9 GB first pass of the loss goes away;
-# PK_FUSED_LSE=0 restores the stand-alone first pass
-_FUSED_LSE = os.environ.get("PK_FUSED_LSE", "1") != "0"
+# the fc2 GEMM epilogue does more work, and the 13.9 GB first pass of the loss goes away.  tests/test_layers_gpu.py sets False
+# to compare against the stand-alone first pass
+_FUSED_LSE = True
 
 
 # measurement hook (bench.py): when set to a dict, single launches of the step are bracketed by CUDA events on the launching stream,
@@ -814,8 +765,7 @@ def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None)
     dl_parts = [p.view(R, ldv) for p in stage_act(dlogits)]
     dl_v = [p[:, :V] for p in dl_parts]
     dh = _new((R, H), like=dlogits)
-    w2b, w2mn = dgrad_b(st["w2"])
-    gemm_parts([dl_v], [w2b], dh, b_mn=w2mn)
+    gemm_parts([dl_v], [st["w2"]], dh, b_mn=True)
     gemm_parts([dl_v], [st["h_parts"]], grad_of(fc2.weight), a_mn=True, b_mn=True)
     if db2 is None:
         db2 = torch.empty(ldv, dtype=torch.float32, device=dlogits.device)
@@ -837,13 +787,11 @@ def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None)
     d_enc = d_pred = None
     if need_enc:
         d_enc = _new((B * T, H), like=dlogits)
-        wb, wmn = dgrad_b(st["wx"], cols=(0, H))
-        gemm_parts([dex_parts], [wb], d_enc, b_mn=wmn)
+        gemm_parts([dex_parts], [[p[:, :H] for p in st["wx"]]], d_enc, b_mn=True)
         d_enc = d_enc.view(B, T, H)
     if need_pred:
         d_pred = _new((B * U1, H), like=dlogits)
-        wb, wmn = dgrad_b(st["wx"], cols=(H, 2 * H))
-        gemm_parts([dpy_parts], [wb], d_pred, b_mn=wmn)
+        gemm_parts([dpy_parts], [[p[:, H:] for p in st["wx"]]], d_pred, b_mn=True)
         d_pred = d_pred.view(B, U1, H)
     return d_enc, d_pred
 
@@ -973,7 +921,7 @@ def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None):
     ctxv = AttentionFn.apply(qkv.view(B, T, -1), att.head_count, p, _next_seed() if p > 0 else 0, causal, key_pad)
     h1 = linear(ctxv.view(B * T, -1), att.final_linear.weight, att.final_linear.bias, drop_p=p, residual=x2)
     ln2 = LayerNormFn.apply(h1, ff.layer_norm, ff.layer_norm.weight, ff.layer_norm.bias)
-    fold = _FOLD_MASKS and ln2.dtype == torch.bfloat16
+    fold = ln2.dtype == torch.bfloat16
     inter = linear(ln2, ff.w_1.weight, ff.w_1.bias, act=True, drop_p=p, premasked=fold)
     # w_2's dgrad epilogue applies w_1's ReLU(+dropout) mask: inter != 0 <=> active and kept
     return linear(inter, ff.w_2.weight, ff.w_2.bias, drop_p=p, residual=h1,
@@ -990,14 +938,14 @@ def encoder_forward_act(enc, x, x_len=None, t_out=None):
     C = enc.tdnn_nhid
     if T < 43:
         raise ValueError("encoder input has %d frames; the TDNN stack needs at least 43 (receptive field 21+1+21)" % T)
-    fold = _FOLD_MASKS            # ReLU masks ride in the BatchNorm backward (pk_bn_bwd relu_mask) instead of separate passes
-    h = linear(_to_act(x).view(B * T, D), enc.fc_in.weight, enc.fc_in.bias, act=True, premasked=fold)
-    h = BatchNormFn.apply(h, enc.bn_in, training, enc.bn_in.weight, enc.bn_in.bias, fold)
+    # ReLU masks ride in the BatchNorm backward (pk_bn_bwd relu_mask) instead of separate passes
+    h = linear(_to_act(x).view(B * T, D), enc.fc_in.weight, enc.fc_in.bias, act=True, premasked=True)
+    h = BatchNormFn.apply(h, enc.bn_in, training, enc.bn_in.weight, enc.bn_in.bias, True)
     for l, (conv, bn) in enumerate(zip(enc.hidden_conv, enc.hidden_bn)):
         dil, stride = enc.TDNN_DIL_STRIDE[l]
-        h3 = TdnnFn.apply(h.view(B, T, C), conv.weight, conv.bias, dil, stride, fold)
+        h3 = TdnnFn.apply(h.view(B, T, C), conv.weight, conv.bias, dil, stride, True)
         T = h3.shape[1]
-        h = BatchNormFn.apply(h3.view(B * T, C), bn, training, bn.weight, bn.bias, fold)
+        h = BatchNormFn.apply(h3.view(B * T, C), bn, training, bn.weight, bn.bias, True)
         if (l + 1) % 3 == 0:
             h = transformer_layer(enc.transformer[l // 3], h, B, T, training)
     h = BatchNormFn.apply(h, enc.bn_final, training, enc.bn_final.weight, enc.bn_final.bias)

@@ -43,7 +43,7 @@ def _fill_view(v, t):
 
 def gemm(a, b, c, a_mn=False, b_mn=False, a_sel=(SEL_ZB0, SEL_ZB1), b_sel=(SEL_ZB0, SEL_ZB1), kz_count=1,
          a_row_off=None, b_row_off=None, alpha=1.0, bias=None, act=ACT_NONE, drop_p=0.0, drop_seed=0,
-         aux=None, aux_mode=AUX_NONE, aux_scale=1.0, accumulate=False, block_n=0, k_splits=0, two_sm=0, row_lse=None):
+         aux=None, aux_mode=AUX_NONE, aux_scale=1.0, accumulate=False, block_n=0, k_splits=0, row_lse=None):
     """C = epilogue(alpha * sum_p A_p @ B_p^T) on the wgmma tensor cores (include/pika_b200.h).
 
     a, b: a bf16 view or a list of views (pairs).  Views are torch tensors of <= 4 dims laid out
@@ -88,19 +88,18 @@ def gemm(a, b, c, a_mn=False, b_mn=False, a_sel=(SEL_ZB0, SEL_ZB1), b_sel=(SEL_Z
         d.aux_scale = aux_scale
     d.block_n = block_n
     d.k_splits = k_splits
-    d.two_sm = two_sm
     if row_lse is not None:
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and c.dim() == 2
-        assert tuple(row_lse.shape) == (row_lse_parts(c.shape[-2], c.shape[-1], block_n, two_sm), c.shape[-2], 2)
+        assert tuple(row_lse.shape) == (row_lse_parts(c.shape[-2], c.shape[-1], block_n), c.shape[-2], 2)
         d.row_lse = row_lse.data_ptr()
     check(lib.pk_gemm_bf16(ctypes.byref(d), _stream()), "pk_gemm_bf16")
     return c
 
 
-def row_lse_parts(M, N, block_n=0, two_sm=0):
-    """number of per-row (max, sum-exp) partials the GEMM writes into ``row_lse`` for an [M, N] output: one per N tile on
-    both kernel flavours (every row's columns are owned by one CTA)"""
-    return int(lib.pk_gemm_row_lse_parts(M, N, block_n, two_sm))
+def row_lse_parts(M, N, block_n=0):
+    """number of per-row (max, sum-exp) partials the GEMM writes into ``row_lse`` for an [M, N] output: one per N tile
+    (every row's columns are owned by one CTA)"""
+    return int(lib.pk_gemm_row_lse_parts(M, N, block_n))
 
 
 def rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=None, grad_scale=None, dlogits=None, want_grad=True, colsum=None,
@@ -148,15 +147,6 @@ def cast_split(src, hi, lo=None, cols_pad=None, scale=1.0):
     assert hi.shape[-1] == cols_pad and hi.stride(-1) == 1 and src.stride(-1) == 1
     check(lib.pk_cast_split(_P(src), _I(_dt(src)), _L(src.stride(0)), _P(hi), _P(lo), _L(hi.stride(0)), _L(rows),
                             _I(cols), _I(cols_pad), _F(scale), _stream()), "pk_cast_split")
-
-
-def transpose_bf16(src, dst):
-    """dst [cols, rows] = src [rows, cols]^T (bf16, row strides free)"""
-    rows, cols = src.shape
-    assert src.dtype == torch.bfloat16 and dst.dtype == torch.bfloat16 and dst.shape == (cols, rows)
-    assert src.stride(1) == 1 and dst.stride(1) == 1
-    check(lib.pk_transpose_bf16(_P(src), _L(src.stride(0)), _P(dst), _L(dst.stride(0)), _I(rows), _I(cols), _stream()),
-          "pk_transpose_bf16")
 
 
 def attention_lse_stride(T):
@@ -332,21 +322,6 @@ def _lstm_scratch(H, device):
         lib.pk_lstm_seq_workspace_bytes.restype = ctypes.c_longlong
         _lstm_ws[key] = torch.zeros(int(lib.pk_lstm_seq_workspace_bytes(H)), dtype=torch.uint8, device=device)
     return _lstm_ws[key]
-
-
-def lstm_seq_fwd(gx, w_hh, out, gates_save, cs):
-    B, U, G4 = gx.shape
-    H = G4 // 4
-    assert gx.is_contiguous() and out.is_contiguous() and w_hh.dtype == torch.bfloat16 and w_hh.is_contiguous()
-    check(lib.pk_lstm_seq_fwd(_P(gx), _P(w_hh), _P(out), _I(_dt(out)), _P(gates_save), _P(cs), _I(B), _I(U), _I(H),
-                              _P(_lstm_scratch(H, gx.device)), _stream()), "pk_lstm_seq_fwd")
-
-
-def lstm_seq_bwd(dout, gates_save, cs, w_hh, dG):
-    B, U, H = dout.shape
-    assert dout.is_contiguous() and dG.dtype == torch.bfloat16 and dG.is_contiguous()
-    check(lib.pk_lstm_seq_bwd(_P(dout), _I(_dt(dout)), _P(gates_save), _P(cs), _P(w_hh), _P(dG), _I(B), _I(U), _I(H),
-                              _P(_lstm_scratch(H, dout.device)), _stream()), "pk_lstm_seq_bwd")
 
 
 def _lens_arg(lens, B):

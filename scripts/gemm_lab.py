@@ -1,8 +1,7 @@
 """GEMM lab: the step's dominant shapes timed stand-alone with CUDA events (inputs >> L2, 3 warm-ups), one line per shape.
-Kernel-selection knobs are read from the environment by the library (PK_GEMM_2SM, PK_GEMM_2SM_MIN_TILES, PK_GEMM_SPLIT_MODE,
-PK_GEMM_SPLIT_MAX, PK_GEMM_SPLIT_MAJOR, PK_GEMM_L2_HINTS), so one process = one configuration:
+The first line names the build (pk_version), so that runs of two builds can be told apart:
 
-    PK_GEMM_2SM=1 python scripts/gemm_lab.py fc2        # the CTA-pair (2-CTA cluster) kernel on the three joint GEMMs
+    python scripts/gemm_lab.py fc2        # the three joint GEMMs
     python scripts/gemm_lab.py all
 
 Each result is also spot-checked against torch on a few rows so that a fast-but-wrong variant cannot slip through.
@@ -82,8 +81,7 @@ def run(name, M, N, Kd, a_mn, b_mn, cdt, lse=False, bias=False, **kw):
 
 R = 32 * 240 * 151
 which = sys.argv[1] if len(sys.argv) > 1 else "all"
-env = {k: v for k, v in os.environ.items() if k.startswith("PK_")}
-print(json.dumps(dict(config=env)), flush=True)
+print(json.dumps(dict(config=dict(pk_version=int(K.lib.pk_version())))), flush=True)
 bf, f32 = torch.bfloat16, torch.float32
 if which in ("fc2", "all", "fwd"):
     run("fc2_fwd_plain", R, 6000, 1024, False, False, bf, bias=True)

@@ -182,21 +182,20 @@ def test_gemm_split_bf16_fp32_class():
     assert rel(c, ref) < 3e-5
 
 
-@pytest.mark.parametrize("two_sm", [-1, 1])
 @pytest.mark.parametrize("mnk", [(300, 6000, 256), (128, 256, 64), (1000, 520, 192), (2049, 6000, 128)])
-def test_gemm_row_lse_partials(mnk, two_sm):
+def test_gemm_row_lse_partials(mnk):
     """pk_gemm_desc.row_lse: per-row, per-column-group (max*log2e, sum 2^(x*log2e-max)) of the ROUNDED bf16 outputs: one group per
-    256-wide N tile on both the single-CTA and the CTA-pair kernel (a CTA of a pair owns whole rows of the 256 x 256 tile)."""
+    256-wide N tile."""
     import math
     M, N, Kd = mnk
     a, b = rnd(M, Kd, seed=11, scale=0.5), rnd(N, Kd, seed=12, scale=0.5)
     bias = torch.randn(N, device="cuda")
     c = torch.full((M, N), float("nan"), device="cuda", dtype=torch.bfloat16)
-    nt = K().row_lse_parts(M, N, 256, two_sm)
+    nt = K().row_lse_parts(M, N, 256)
     gw = 256 * ((N + 255) // 256) // nt                 # columns per group
     assert nt == (N + 255) // 256
     parts = torch.full((nt, M, 2), float("nan"), device="cuda")
-    K().gemm(a, b, c, bias=bias, block_n=256, row_lse=parts, two_sm=two_sm)
+    K().gemm(a, b, c, bias=bias, block_n=256, row_lse=parts)
     ref = a.float() @ b.float().t() + bias
     assert rel(c, ref) < 4e-3
     m = parts[:, :, 0].max(0).values
@@ -239,38 +238,42 @@ def test_gemm_split_k(mnk, a_mn, b_mn, ks):
 @pytest.mark.parametrize("cdt", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, False), (True, True)])
 @pytest.mark.parametrize("mnk", [(304, 520, 136), (2048, 1024, 1024), (136, 256, 64), (1000, 264, 200)])
-def test_gemm_cta_pair_kernel(mnk, a_mn, b_mn, cdt):
-    """the CTA-pair flavour (a 2-CTA cluster on a 256 x 256 tile, B shared through TMA multicast) on every operand layout, incl.
-    ragged M / N (the second CTA of the last pair may own no rows at all)"""
+def test_gemm_bn256_every_layout_ragged(mnk, a_mn, b_mn, cdt):
+    """256-wide tiles with bias on every operand layout and both C types, incl. ragged M / N (a last row tile with few valid rows,
+    a last N tile with few valid columns)"""
     M, N, Kd = mnk
     a = rnd(Kd, M, seed=21) if a_mn else rnd(M, Kd, seed=21)
     b = rnd(Kd, N, seed=22) if b_mn else rnd(N, Kd, seed=22)
     c = torch.full((M, N), float("nan"), device="cuda", dtype=cdt)
     bias = torch.randn(N, device="cuda")
-    K().gemm(a, b, c, a_mn=a_mn, b_mn=b_mn, bias=bias, block_n=256, two_sm=1)
+    K().gemm(a, b, c, a_mn=a_mn, b_mn=b_mn, bias=bias, block_n=256)
     af = a.float().t() if a_mn else a.float()
     bf = b.float().t() if b_mn else b.float()
     assert rel(c, af @ bf.t() + bias) < (2e-5 if cdt == torch.float32 else 4e-3)
 
 
-def test_gemm_cta_pair_split_k_taps_and_full_epilogue():
-    """CTA-pair kernel: split-K with reduce-add, three accumulated taps with row offsets, dropout + residual epilogue"""
+def test_gemm_bn256_split_k_taps_and_full_epilogue():
+    """256-wide tiles: split-K with reduce-add, three accumulated taps with row offsets, ReLU + dropout + residual epilogue"""
     M, N, Kd = 6000, 1024, 4000
     a, b = rnd(Kd, M, seed=31, scale=0.3), rnd(Kd, N, seed=32, scale=0.3)
     c = torch.full((M, N), float("nan"), device="cuda")
-    K().gemm(a, b, c, a_mn=True, b_mn=True, two_sm=1, block_n=256, k_splits=3)
+    K().gemm(a, b, c, a_mn=True, b_mn=True, block_n=256, k_splits=3)
     assert rel(c, a.float().t() @ b.float()) < 2e-5
     # taps: y[t] = sum_k x[t + k] W_k^T
     T, C, Nn = 700, 128, 512
     x = rnd(T + 2, C, seed=33)
     w = [rnd(Nn, C, seed=40 + k) for k in range(3)]
     y = torch.empty(T, Nn, device="cuda")
-    K().gemm([x[k:k + T] for k in range(3)], w, y, two_sm=1, block_n=256)
+    K().gemm([x[k:k + T] for k in range(3)], w, y, block_n=256)
     ref = sum(x[k:k + T].float() @ w[k].float().t() for k in range(3))
     assert rel(y, ref) < 2e-5
     res = rnd(T, Nn, seed=50)
-    y1 = torch.empty(T, Nn, device="cuda", dtype=torch.bfloat16)
-    y2 = torch.empty(T, Nn, device="cuda", dtype=torch.bfloat16)
-    for out, two in ((y1, 1), (y2, -1)):
-        K().gemm(x[:T], w[0], out, two_sm=two, block_n=256, drop_p=0.2, drop_seed=99, aux=res, aux_mode=K().AUX_ADD, act=K().ACT_RELU)
-    assert torch.equal(y1, y2)          # same counter-based mask, same arithmetic per element on both flavours
+    y = torch.empty(T, Nn, device="cuda", dtype=torch.bfloat16)
+    K().gemm(x[:T], w[0], y, block_n=256, drop_p=0.2, drop_seed=99, aux=res, aux_mode=K().AUX_ADD, act=K().ACT_RELU)
+    # the same counter-based mask without the residual: a dropped element is exactly 0 there (and where the ReLU gives 0, dropped
+    # or kept make no difference)
+    m = torch.empty_like(y)
+    K().gemm(x[:T], w[0], m, block_n=256, drop_p=0.2, drop_seed=99, act=K().ACT_RELU)
+    kept = m != 0
+    ref = torch.where(kept, torch.relu(x[:T].float() @ w[0].float().t()) / 0.8, 0.0) + res.float()
+    assert rel(y, ref) < 4e-3

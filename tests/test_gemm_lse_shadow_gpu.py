@@ -22,10 +22,9 @@ def shape(case, n_sm):
     return 256 * n_sm + 77, 2 * 256 + 128  # ~6 tiles per worker; the last N tile's second 128-column half is empty
 
 
-@pytest.mark.parametrize("two_sm", [0, 1])
 @pytest.mark.parametrize("Kd", [64, 200])
 @pytest.mark.parametrize("case", ["one_tile_per_worker", "six_tiles_per_worker"])
-def test_gemm_row_lse_partials(two_sm, Kd, case):
+def test_gemm_row_lse_partials(Kd, case):
     from pika_b200 import kernels as K
     n_sm = torch.cuda.get_device_properties(0).multi_processor_count
     M, N = shape(case, n_sm)
@@ -36,8 +35,8 @@ def test_gemm_row_lse_partials(two_sm, Kd, case):
     b[:, -1] = 1
     bias = torch.randn(N, device="cuda") * 3
     c = torch.full((M, N), float("nan"), device="cuda", dtype=torch.bfloat16)
-    parts = torch.full((K.row_lse_parts(M, N, 256, two_sm), M, 2), float("nan"), device="cuda")
-    K.gemm(a, b, c, alpha=0.5, bias=bias, block_n=256, two_sm=two_sm, row_lse=parts)
+    parts = torch.full((K.row_lse_parts(M, N, 256), M, 2), float("nan"), device="cuda")
+    K.gemm(a, b, c, alpha=0.5, bias=bias, block_n=256, row_lse=parts)
     ref = 0.5 * (a.float() @ b.float().t()) + bias
     assert ((c.float() - ref).norm() / ref.norm()).item() < 4e-3
     assert parts.shape[0] == (N + 255) // 256
