@@ -177,6 +177,25 @@ int pk_softmax_masked_fwd(const float* S, long long ld_s, void* P, void* Pd, int
                           int q_len, int heads, int causal, const uint8_t* key_pad, float drop_p, uint32_t seed, void* stream);
 int pk_softmax_bwd(const float* dPd, long long ld_d, const void* P, long long ld_p, void* dS, int dtype, long long rows,
                    int n, float drop_p, uint32_t seed, void* stream);
+/* Relative-position self-attention (Shaw et al.; trainer/model/modules/multi_headed_attn.py:9-41,186-229), max_rel = m > 0:
+ *   scores_ij = alpha q_i.k_j + alpha q_i.R[b(i,j)],  out_i = sum_j Pd_ij v_j + sum_j Pd_ij R[b(i,j)],  b(i,j) = clamp(j-i, -m, m) + m
+ * with R the [2m+1, dh] table (key and value relations alike).  The GEMMs around these kernels form QR = alpha Q R^T and
+ * G = dO R^T; the kernels gather them along the band and reduce P / dS back onto the 2m+1 buckets.
+ * Rows of S / P / dPd / dS are (sequence, head, query i) as for pk_softmax_masked_fwd, with q_len = n (self-attention).  Rows of
+ * QR, Pb, G, dSb ([sequences * n * heads, ld_r] f32) are token-major: (sequence, query i, head).
+ *   fwd: P = softmax(mask(S + QR[b])), Pd = dropout(P) as pk_softmax_masked_fwd (causal and key_pad optional here);
+ *        Pb[., r] = sum over keys j with b(i,j) = r of Pd (as stored).
+ *   bwd: dS = softmax_bwd(dPd + G[b]) as pk_softmax_bwd;  dSb[., r] = sum over keys j with b(i,j) = r of dS (as stored).
+ * Every entry of Pb / dSb is written (0 for buckets no key reaches and for the padding [2m+1, ld_r)).
+ * Limits: n <= ld_p <= 2048 (the row lives in one warp's registers), ld_s / ld_d >= ld_p, pitches multiples of 8;
+ *         1 <= m <= 1024, ld_r >= 2m+1 and a multiple of 8. */
+#define PK_RELPOS_MAX 1024
+int pk_softmax_masked_relpos_fwd(const float* S, long long ld_s, const float* QR, long long ld_r, void* P, void* Pd, int dtype,
+                                 long long ld_p, long long rows, int n, int q_len, int heads, int causal, const uint8_t* key_pad,
+                                 int max_rel, float* Pb, float drop_p, uint32_t seed, void* stream);
+int pk_softmax_relpos_bwd(const float* dPd, long long ld_d, const float* G, long long ld_r, const void* P, long long ld_p, void* dS,
+                          int dtype, long long rows, int n, int q_len, int heads, int max_rel, float* dSb, float drop_p,
+                          uint32_t seed, void* stream);
 /* nn.Dropout with the counter-based RNG shared with the GEMM epilogue; mask_nz: dx = dy * (y != 0) * scale */
 int pk_dropout(const void* x, void* y, int dtype, long long n, float p, uint32_t seed, void* stream);
 int pk_mask_nz(const void* dy, const void* y, void* dx, int dtype, long long n, float scale, void* stream);

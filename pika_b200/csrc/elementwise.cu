@@ -553,6 +553,165 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(const float* __restric
     }
 }
 
+// ------------------------------------------------------------------------------- relative positions (Shaw et al.)
+// Query i and key j of one sequence share the table row bucket(i, j) = clamp(j - i, -mr, mr) + mr
+// (trainer/model/modules/multi_headed_attn.py:9-24).  Along a row the buckets form a band: bucket r in (0, 2mr) is the single key
+// j = i - mr + r, bucket 0 collects every j <= i - mr and bucket 2mr every j >= i + mr.  So the gather of the table terms is one
+// scalar load per key, and the per-bucket reduction is a shifted copy of the row plus two warp sums -- no atomics, no [T, T, d]
+// tensor.  The bucket rows (QR, Pb, G, dSb) are token-major: row (sequence, query, head), the layout of the [B, T, heads*dh]
+// activations, so the GEMMs that produce and consume them see plain 2-D matrices.
+PK_DEVICE int relpos_bucket(int dist, int mr) { return min(max(dist, -mr), mr) + mr; }
+
+// out[r] = sum of v over keys j < n with bucket(i, j) = r, for r < ld_r (0 for buckets no key reaches and for the padding r > 2mr).
+// v holds the row in the softmax kernels' register layout.  Every entry of out is written by exactly one lane.
+template <int SM_CH>
+PK_DEVICE void relpos_bucket_sums(const float (&v)[SM_CH][8], float* __restrict__ out, int ld_r, int i, int mr, int n, int lane) {
+    float lo = 0.f, hi = 0.f;
+#pragma unroll
+    for (int k = 0; k < SM_CH; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const int c = lane * 8 + k * 256 + e;
+            if (c < n) {
+                const int dist = c - i;
+                if (dist <= -mr) lo += v[k][e];
+                else if (dist >= mr) hi += v[k][e];
+                else out[dist + mr] = v[k][e];
+            }
+        }
+    lo = warp_sum(lo);
+    hi = warp_sum(hi);
+    for (int r = lane; r < ld_r; r += 32) {
+        const int j = i - mr + r;
+        if (r == 0) out[0] = lo;
+        else if (r == 2 * mr) out[r] = hi;
+        else if (r > 2 * mr || j < 0 || j >= n) out[r] = 0.f;
+    }
+}
+
+// pk_softmax_masked_fwd with the key relations: S[r, j] + QR[rr, bucket(i, j)] is masked and normalised, and the bucket sums of
+// the dropped-out probabilities Pd (as stored, i.e. rounded to T) go to Pb[rr, :].  rr = (sequence * q_len + i) * heads + head.
+template <typename T, int SM_CH>
+__global__ void __launch_bounds__(256) softmax_relpos_fwd_kernel(const float* __restrict__ S, long long ld_s, const float* __restrict__ QR,
+                                                                 long long ld_r, T* __restrict__ P, T* __restrict__ Pd, long long ld_p,
+                                                                 long long rows, int n, uint32_t drop_thresh, float drop_scale, uint32_t seed,
+                                                                 int q_len, int heads, int causal, const uint8_t* __restrict__ key_pad,
+                                                                 int mr, float* __restrict__ Pb) {
+    const int lane = threadIdx.x & 31;
+    const long long warp = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long r = warp; r < rows; r += nw) {
+        const long long seq = r / ((long long)heads * q_len);
+        const int i = (int)(r % q_len), h = (int)((r / q_len) % heads);
+        const long long rr = (seq * q_len + i) * heads + h;
+        const float* sr = S + r * ld_s;
+        const float* qr = QR + rr * ld_r;
+        const int lim = causal ? min(n, i + 1) : n;
+        const uint8_t* kp = key_pad ? key_pad + seq * n : nullptr;
+        float v[SM_CH][8];
+        float mx = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < SM_CH; ++k) {
+            const int c0 = lane * 8 + k * 256;
+            if (c0 < (int)ld_p) ld8f(sr + c0, v[k]);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int c = c0 + e;
+                if (c >= lim || (kp && kp[c])) v[k][e] = -INFINITY;
+                else v[k][e] += qr[relpos_bucket(c - i, mr)];
+                mx = fmaxf(mx, v[k][e]);
+            }
+        }
+        mx = warp_max(mx);
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < SM_CH; ++k)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) { v[k][e] = __expf(v[k][e] - mx); s += v[k][e]; }
+        const float inv = 1.f / warp_sum(s);
+#pragma unroll
+        for (int k = 0; k < SM_CH; ++k) {
+            const int c0 = lane * 8 + k * 256;
+            if (c0 < (int)ld_p) {
+                float o[8];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) { o[e] = to_f32<T>(from_f32<T>(v[k][e] * inv)); v[k][e] = o[e]; }
+                if (drop_thresh) {
+                    const uint32_t salt = drop_row_salt((uint64_t)r, seed);
+#pragma unroll
+                    for (int e2 = 0; e2 < 4; ++e2) {
+                        const uint32_t km = drop_pair(salt, (uint32_t)((c0 >> 1) + e2), drop_thresh);
+                        v[k][2 * e2] = (km & 1u) ? o[2 * e2] * drop_scale : 0.f;
+                        v[k][2 * e2 + 1] = (km & 2u) ? o[2 * e2 + 1] * drop_scale : 0.f;
+                    }
+                }
+                V8<T>::store(P + r * ld_p + c0, o);
+                if (Pd != P) V8<T>::store(Pd + r * ld_p + c0, v[k]);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) v[k][e] = to_f32<T>(from_f32<T>(v[k][e]));
+            }
+        }
+        relpos_bucket_sums<SM_CH>(v, Pb + rr * ld_r, (int)ld_r, i, mr, n, lane);
+    }
+}
+// pk_softmax_bwd with the value relations: dPd[r, j] + G[rr, bucket(i, j)] (G = dO R^T) is the gradient of Pd; the bucket sums of
+// dS (as stored) go to dSb[rr, :].
+template <typename T, int SM_CH>
+__global__ void __launch_bounds__(256) softmax_relpos_bwd_kernel(const float* __restrict__ dPd, long long ld_d, const float* __restrict__ G,
+                                                                 long long ld_r, const T* __restrict__ P, long long ld_p, T* __restrict__ dS,
+                                                                 long long rows, int n, uint32_t drop_thresh, float drop_scale, uint32_t seed,
+                                                                 int q_len, int heads, int mr, float* __restrict__ dSb) {
+    const int lane = threadIdx.x & 31;
+    const long long warp = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long r = warp; r < rows; r += nw) {
+        const long long seq = r / ((long long)heads * q_len);
+        const int i = (int)(r % q_len), h = (int)((r / q_len) % heads);
+        const long long rr = (seq * q_len + i) * heads + h;
+        const float* g = G + rr * ld_r;
+        float d[SM_CH][8], pv[SM_CH][8];
+        float dot = 0.f;
+#pragma unroll
+        for (int k = 0; k < SM_CH; ++k) {
+            const int c0 = lane * 8 + k * 256;
+            if (c0 < (int)ld_p) {
+                ld8f(dPd + r * ld_d + c0, d[k]);
+                V8<T>::load(P + r * ld_p + c0, pv[k]);
+#pragma unroll
+                for (int e = 0; e < 8; ++e)
+                    if (c0 + e < n) d[k][e] += g[relpos_bucket(c0 + e - i, mr)];
+                if (drop_thresh) {
+                    const uint32_t salt = drop_row_salt((uint64_t)r, seed);
+#pragma unroll
+                    for (int e2 = 0; e2 < 4; ++e2) {
+                        const uint32_t km = drop_pair(salt, (uint32_t)((c0 >> 1) + e2), drop_thresh);
+                        d[k][2 * e2] = (km & 1u) ? d[k][2 * e2] * drop_scale : 0.f;
+                        d[k][2 * e2 + 1] = (km & 2u) ? d[k][2 * e2 + 1] * drop_scale : 0.f;
+                    }
+                }
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    if (c0 + e >= n) { d[k][e] = 0.f; pv[k][e] = 0.f; }
+                    dot += d[k][e] * pv[k][e];
+                }
+            }
+        }
+        dot = warp_sum(dot);
+#pragma unroll
+        for (int k = 0; k < SM_CH; ++k) {
+            const int c0 = lane * 8 + k * 256;
+            if (c0 < (int)ld_p) {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) d[k][e] = pv[k][e] * (d[k][e] - dot);
+                V8<T>::store(dS + r * ld_p + c0, d[k]);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) d[k][e] = to_f32<T>(from_f32<T>(d[k][e]));
+            }
+        }
+        relpos_bucket_sums<SM_CH>(d, dSb + rr * ld_r, (int)ld_r, i, mr, n, lane);
+    }
+}
+
 // =============================================================================== misc elementwise
 // y = dropout(x) with the GEMM epilogue's index convention (flat index of a contiguous tensor); 8 elements per thread
 // (scalar tail for n % 8), 16-byte accesses.
@@ -1147,6 +1306,36 @@ extern "C" int pk_softmax_bwd(const float* dPd, long long ld_d, const void* P, l
     else { PK_DISPATCH_T(dtype, (softmax_bwd_kernel<T, 8><<<grid, 256, 0, STREAM(stream)>>>(dPd, ld_d, (const T*)P, ld_p, (T*)dS, rows, n, th, sc, seed))); }
     DONE();
 }
+#define PK_RELPOS_CHECKS(ld_x, ld_p)                                                                                                  \
+    PK_CHECK_ARG(rows > 0 && n > 0 && ld_p >= n && ld_x >= ld_p && ld_p <= 2048 && ld_p % 8 == 0 && ld_x % 8 == 0,                     \
+                 "relative-position softmax rows: n <= ld_p <= 2048, pitches multiples of 8");                                         \
+    PK_CHECK_ARG(q_len == n && heads > 0 && rows % ((long long)heads * q_len) == 0,                                                     \
+                 "relative-position softmax: self-attention rows = sequences * heads * n");                                             \
+    PK_CHECK_ARG(max_rel >= 1 && max_rel <= PK_RELPOS_MAX && ld_r >= 2 * max_rel + 1 && ld_r % 8 == 0,                               \
+                 "relative positions: 1 <= max_rel <= 1024, ld_r >= 2*max_rel + 1 and a multiple of 8")
+extern "C" int pk_softmax_masked_relpos_fwd(const float* S, long long ld_s, const float* QR, long long ld_r, void* P, void* Pd, int dtype,
+                                            long long ld_p, long long rows, int n, int q_len, int heads, int causal, const uint8_t* key_pad,
+                                            int max_rel, float* Pb, float drop_p, uint32_t seed, void* stream) {
+    PK_RELPOS_CHECKS(ld_s, ld_p);
+    const int grid = grid_for(rows, 8);
+    const uint32_t th = drop_thresh16_of(drop_p);
+    const float sc = drop_scale16_of(th);
+    if (ld_p <= 1024) { PK_DISPATCH_T(dtype, (softmax_relpos_fwd_kernel<T, 4><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, QR, ld_r, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, q_len, heads, causal, key_pad, max_rel, Pb))); }
+    else { PK_DISPATCH_T(dtype, (softmax_relpos_fwd_kernel<T, 8><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, QR, ld_r, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, q_len, heads, causal, key_pad, max_rel, Pb))); }
+    DONE();
+}
+extern "C" int pk_softmax_relpos_bwd(const float* dPd, long long ld_d, const float* G, long long ld_r, const void* P, long long ld_p, void* dS,
+                                     int dtype, long long rows, int n, int q_len, int heads, int max_rel, float* dSb, float drop_p,
+                                     uint32_t seed, void* stream) {
+    PK_RELPOS_CHECKS(ld_d, ld_p);
+    const int grid = grid_for(rows, 8);
+    const uint32_t th = drop_thresh16_of(drop_p);
+    const float sc = drop_scale16_of(th);
+    if (ld_p <= 1024) { PK_DISPATCH_T(dtype, (softmax_relpos_bwd_kernel<T, 4><<<grid, 256, 0, STREAM(stream)>>>(dPd, ld_d, G, ld_r, (const T*)P, ld_p, (T*)dS, rows, n, th, sc, seed, q_len, heads, max_rel, dSb))); }
+    else { PK_DISPATCH_T(dtype, (softmax_relpos_bwd_kernel<T, 8><<<grid, 256, 0, STREAM(stream)>>>(dPd, ld_d, G, ld_r, (const T*)P, ld_p, (T*)dS, rows, n, th, sc, seed, q_len, heads, max_rel, dSb))); }
+    DONE();
+}
+#undef PK_RELPOS_CHECKS
 
 extern "C" int pk_dropout(const void* x, void* y, int dtype, long long n, float p, uint32_t seed, void* stream) {
     const int grid = grid_for(n, 256 * 8);

@@ -436,15 +436,21 @@ class AttentionFn(torch.autograd.Function):
     softmax((Q/sqrt(d)) K^T [masked]) -> dropout -> V   (trainer/model/modules/multi_headed_attn.py:199-223).
     Unmasked (the encoder): the fused wgmma kernels.  ``causal`` / ``key_pad`` (uint8 [B,T], 1 = padding key; the transformer
     prediction net, trainer/model/rnnt_conv_transformer_lm.py:66-70): batched GEMMs + the masked softmax kernel (short label
-    sequences; the mask only enters the forward softmax -- a dropped key has probability 0, so its dS is 0 as well)."""
+    sequences; the mask only enters the forward softmax -- a dropped key has probability 0, so its dS is 0 as well).
+    ``rel``: the relative-position table R [2m+1, dh] (``self_attn.relative_positions_embeddings.weight``, multi_headed_attn.py:9-41,
+    186-229), shared by the key and the value relations; it always takes the materialised path.  The band kernels
+    (pk_softmax_masked_relpos_fwd / pk_softmax_relpos_bwd) add QR = (alpha Q) R^T to the scores and reduce Pd / dS onto the 2m+1
+    buckets (Pb / dSb, token-major rows); the rest is GEMMs: out += Pb R, G = dO R^T, dQ += alpha dSb R, dR = dSb^T (alpha Q) + Pb^T dO.
+    dR is written into ``grad_of(rel)`` (the engine's gradient contract), so no gradient is returned for it."""
 
     @staticmethod
-    def forward(ctx, qkv, heads, drop_p, seed, causal=False, key_pad=None):
+    def forward(ctx, qkv, heads, drop_p, seed, causal=False, key_pad=None, rel=None):
         B, T, D3 = qkv.shape
         D = D3 // 3
         dh = D // heads
         masked = causal or key_pad is not None
-        ctx.fused = _FUSED_ATTN and qkv.dtype == torch.bfloat16 and dh == 64 and not masked
+        ctx.rel = rel
+        ctx.fused = _FUSED_ATTN and qkv.dtype == torch.bfloat16 and dh == 64 and not masked and rel is None
         if ctx.fused:
             # scores / probabilities never leave the SM (pika_b200/csrc/attention_tc.cu)
             qkv = qkv.contiguous()
@@ -467,14 +473,32 @@ class AttentionFn(torch.autograd.Function):
         gemm_parts([q], [k], S[:, :, :, :T], alpha=alpha)
         P = _new((B, heads, T, Tp), like=qkv)
         Pd = _new((B, heads, T, Tp), like=qkv) if drop_p > 0 else P
-        if masked:
+        rel_out = {}
+        if rel is not None:
+            nb = rel.shape[0]                                   # 2m + 1 buckets
+            r_parts = stage_weight(rel)
+            # alpha Q, token-major [B*T*heads, dh]: the A operand of QR and the B operand of dR
+            qc = [torch.empty(B * T, D, dtype=torch.bfloat16, device=qkv.device) for _ in parts]
+            K.cast_split(qkv.view(B * T, D3)[:, :D], qc[0], qc[1] if len(qc) > 1 else None, scale=alpha)
+            qc = [p.view(B * T * heads, dh) for p in qc]
+            QR = torch.empty(B * T * heads, (nb + 7) // 8 * 8, dtype=torch.float32, device=qkv.device)
+            gemm_parts([qc], [r_parts], QR[:, :nb])
+            Pb = torch.empty_like(QR)
+            K.softmax_masked_relpos_fwd(S, QR, P, Pd, Pb, T, heads, causal, key_pad, nb // 2, drop_p, seed)
+            del QR
+            pb_parts = [p[:, :nb] for p in stage_act(Pb)]
+            Y = torch.empty(B * T * heads, dh, dtype=torch.float32, device=qkv.device)        # Pb R, added in the PV epilogue
+            gemm_parts([pb_parts], [r_parts], Y, b_mn=True)
+            rel_out = dict(aux=Y.view(B, T, heads, dh).permute(0, 2, 1, 3), aux_mode=K.AUX_ADD)
+            ctx.r_parts, ctx.qc, ctx.pb_parts = r_parts, qc, pb_parts
+        elif masked:
             K.softmax_masked_fwd(S, P, Pd, T, T, heads, causal, key_pad, drop_p, seed)
         else:
             K.softmax_fwd(S, P, Pd, T, drop_p, seed)
         del S
         out = _new((B, T, D), like=qkv)
         pd_parts = stage_act(Pd)
-        gemm_parts([[p[:, :, :, :T] for p in pd_parts]], [v], out.view(B, T, heads, dh).permute(0, 2, 1, 3), b_mn=True)
+        gemm_parts([[p[:, :, :, :T] for p in pd_parts]], [v], out.view(B, T, heads, dh).permute(0, 2, 1, 3), b_mn=True, **rel_out)
         ctx.save_for_backward(qkv, P)
         ctx.pd_parts, ctx.parts = pd_parts, parts
         ctx.meta = (B, T, D, heads, dh, Tp, drop_p, seed, alpha)
@@ -487,7 +511,7 @@ class AttentionFn(torch.autograd.Function):
             B, T, D, heads, dh, _, drop_p, seed, alpha = ctx.meta
             dqkv = torch.empty_like(qkv)
             K.attention_bwd(qkv, out, dout.contiguous(), lse, dqkv, heads, alpha, drop_p, seed)
-            return dqkv, None, None, None, None, None
+            return dqkv, None, None, None, None, None, None
         qkv, P = ctx.saved_tensors
         B, T, D, heads, dh, Tp, drop_p, seed, alpha = ctx.meta
         dout = dout.contiguous()
@@ -505,13 +529,29 @@ class AttentionFn(torch.autograd.Function):
         dPd = torch.empty(B, heads, T, Tp, dtype=torch.float32, device=qkv.device)
         gemm_parts([do], [v], dPd[:, :, :, :T])
         dS = torch.empty_like(P)
-        K.softmax_bwd(dPd, P, dS, T, drop_p, seed)
+        rel, rel_dq = ctx.rel, {}
+        if rel is not None:
+            nb = rel.shape[0]
+            do2 = [p.view(B * T * heads, dh) for p in do_parts]
+            G = torch.empty(B * T * heads, (nb + 7) // 8 * 8, dtype=torch.float32, device=qkv.device)
+            gemm_parts([do2], [ctx.r_parts], G[:, :nb])
+            dSb = torch.empty_like(G)
+            K.softmax_relpos_bwd(dPd, G, P, dS, dSb, T, heads, nb // 2, drop_p, seed)
+            del G
+            dsb_parts = [p[:, :nb] for p in stage_act(dSb)]
+            Z = torch.empty(B * T * heads, dh, dtype=torch.float32, device=qkv.device)        # alpha dSb R, added in the dQ epilogue
+            gemm_parts([dsb_parts], [ctx.r_parts], Z, b_mn=True, alpha=alpha)
+            rel_dq = dict(aux=Z.view(B, T, heads, dh).permute(0, 2, 1, 3), aux_mode=K.AUX_ADD)
+            # dR = dSb^T (alpha Q) + Pb^T dO, reduced over every (sequence, query, head) row
+            gemm_parts([dsb_parts, ctx.pb_parts], [ctx.qc, do2], grad_of(rel), a_mn=True, b_mn=True)
+        else:
+            K.softmax_bwd(dPd, P, dS, T, drop_p, seed)
         del dPd
         ds_parts = [p[:, :, :, :T] for p in stage_act(dS)]
         # dQ = alpha * dS K ; dK = alpha * dS^T Q
-        gemm_parts([ds_parts], [k], head_view(dqkv, 0), b_mn=True, alpha=alpha)
+        gemm_parts([ds_parts], [k], head_view(dqkv, 0), b_mn=True, alpha=alpha, **rel_dq)
         gemm_parts([ds_parts], [q], head_view(dqkv, 1), a_mn=True, b_mn=True, alpha=alpha)
-        return dqkv, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None
 
 
 class EmbeddingFn(torch.autograd.Function):
@@ -912,13 +952,15 @@ def _to_act(x):
 
 
 def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None):
-    """x2 [B*T, D] -> [B*T, D]   (pre-LN attention block + position-wise FFN); ``causal`` / ``key_pad``: see AttentionFn."""
+    """x2 [B*T, D] -> [B*T, D]   (pre-LN attention block + position-wise FFN); ``causal`` / ``key_pad`` and the layer's relative-position
+    table (when it has one): see AttentionFn."""
     att, ff = layer.self_attn, layer.feed_forward
     p = _drop(layer.dropout_p, training)
     ln = LayerNormFn.apply(x2, layer.layer_norm, layer.layer_norm.weight, layer.layer_norm.bias)
     qkv = linear(ln, [att.linear_query.weight, att.linear_keys.weight, att.linear_values.weight],
                  [att.linear_query.bias, att.linear_keys.bias, att.linear_values.bias])
-    ctxv = AttentionFn.apply(qkv.view(B, T, -1), att.head_count, p, _next_seed() if p > 0 else 0, causal, key_pad)
+    rel = att.relative_positions_embeddings.weight if getattr(att, "max_relative_positions", 0) > 0 else None
+    ctxv = AttentionFn.apply(qkv.view(B, T, -1), att.head_count, p, _next_seed() if p > 0 else 0, causal, key_pad, rel)
     h1 = linear(ctxv.view(B * T, -1), att.final_linear.weight, att.final_linear.bias, drop_p=p, residual=x2)
     ln2 = LayerNormFn.apply(h1, ff.layer_norm, ff.layer_norm.weight, ff.layer_norm.bias)
     fold = ln2.dtype == torch.bfloat16
@@ -1025,9 +1067,7 @@ def prednet_forward_act(model, y):
 def conv_transformer_lm_forward_act(dec, src):
     """Transformer prediction net (trainer/model/rnnt_conv_transformer_lm.py:59-80): src [B,L] int64 (SOS already prepended) ->
     [B,L,output_dim].  Embedding -> num_layers x (causal Conv1d(k=5) + ReLU -> pre-LN transformer layer under the causal +
-    padding-key mask) -> LayerNorm -> linear_out."""
-    if getattr(dec, "max_relative_positions", 0) > 0:
-        raise NotImplementedError("pika_b200: relative position embeddings (max_relative_positions > 0) are not on the hot path")
+    padding-key mask, with relative-position attention when ``max_relative_positions`` > 0) -> LayerNorm -> linear_out."""
     B, L = src.shape
     emb = dec.embeddings
     ld = (emb.weight.shape[1] + 7) // 8 * 8

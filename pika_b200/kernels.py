@@ -243,6 +243,27 @@ def softmax_bwd(dPd, P, dS, n, drop_p, seed):
                              _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_softmax_bwd")
 
 
+def softmax_masked_relpos_fwd(S, QR, P, Pd, Pb, n, heads, causal, key_pad, max_rel, drop_p, seed):
+    """pk_softmax_masked_fwd with the relative-position key terms QR [sequences*n*heads, ld_r] added along the band; writes the bucket
+    sums Pb (same shape) of Pd.  Rows of S are (sequence, head, query), rows of QR / Pb (sequence, query, head)."""
+    rows = S.numel() // S.shape[-1]
+    if key_pad is not None:
+        assert key_pad.dtype == torch.uint8 and key_pad.is_contiguous() and key_pad.shape[-1] == n
+    assert QR.dtype == torch.float32 and Pb.dtype == torch.float32 and QR.stride(-1) == 1 and Pb.stride() == QR.stride()
+    check(lib.pk_softmax_masked_relpos_fwd(_P(S), _L(S.shape[-1]), _P(QR), _L(QR.stride(0)), _P(P), _P(Pd), _I(_dt(P)), _L(P.shape[-1]),
+                                           _L(rows), _I(n), _I(n), _I(heads), _I(int(bool(causal))), _P(key_pad), _I(max_rel), _P(Pb),
+                                           _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_softmax_masked_relpos_fwd")
+
+
+def softmax_relpos_bwd(dPd, G, P, dS, dSb, n, heads, max_rel, drop_p, seed):
+    """pk_softmax_bwd with the relative-position value terms G = dO R^T added along the band; writes the bucket sums dSb of dS"""
+    rows = P.numel() // P.shape[-1]
+    assert G.dtype == torch.float32 and dSb.dtype == torch.float32 and G.stride(-1) == 1 and dSb.stride() == G.stride()
+    check(lib.pk_softmax_relpos_bwd(_P(dPd), _L(dPd.shape[-1]), _P(G), _L(G.stride(0)), _P(P), _L(P.shape[-1]), _P(dS), _I(_dt(P)),
+                                    _L(rows), _I(n), _I(n), _I(heads), _I(max_rel), _P(dSb), _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()),
+          "pk_softmax_relpos_bwd")
+
+
 def dropout(x, y, p, seed):
     check(lib.pk_dropout(_P(x), _P(y), _I(_dt(x)), _L(x.numel()), _F(p), _U(seed & 0xFFFFFFFF), _stream()), "pk_dropout")
 

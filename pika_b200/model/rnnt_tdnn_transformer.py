@@ -11,9 +11,11 @@ import torch.nn as nn
 
 
 class _AttnParams(nn.Module):
-    """trainer/model/modules/multi_headed_attn.py:85-108 (parameter layout only)."""
+    """trainer/model/modules/multi_headed_attn.py:85-108 (parameter layout only).  ``max_relative_positions`` m > 0 adds the
+    relative-position table ``relative_positions_embeddings`` = nn.Embedding(2m+1, dim_per_head), created right after
+    ``final_linear`` as in the reference (:103-108)."""
 
-    def __init__(self, head_count, model_dim, dropout):
+    def __init__(self, head_count, model_dim, dropout, max_relative_positions=0):
         super().__init__()
         assert model_dim % head_count == 0
         self.dim_per_head = model_dim // head_count
@@ -24,6 +26,9 @@ class _AttnParams(nn.Module):
         self.linear_query = nn.Linear(model_dim, model_dim)
         self.dropout_p = dropout
         self.final_linear = nn.Linear(model_dim, model_dim)
+        self.max_relative_positions = max_relative_positions
+        if max_relative_positions > 0:
+            self.relative_positions_embeddings = nn.Embedding(2 * max_relative_positions + 1, self.dim_per_head)
 
 
 class _FfnParams(nn.Module):
@@ -40,9 +45,9 @@ class _FfnParams(nn.Module):
 class _TransformerLayerParams(nn.Module):
     """trainer/model/modules/transformer.py:74-83 (parameter layout only)."""
 
-    def __init__(self, d_model, heads, d_ff, dropout):
+    def __init__(self, d_model, heads, d_ff, dropout, max_relative_positions=0):
         super().__init__()
-        self.self_attn = _AttnParams(heads, d_model, dropout)
+        self.self_attn = _AttnParams(heads, d_model, dropout, max_relative_positions)
         self.feed_forward = _FfnParams(d_model, d_ff, dropout)
         self.layer_norm = nn.LayerNorm(d_model, eps=1e-6)
         self.dropout_p = dropout

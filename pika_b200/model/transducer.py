@@ -35,7 +35,8 @@ class Net(nn.Module):
                                    num_layers=opt.dec_layers, bidirectional=False, batch_first=True)
         else:                                          # trainer/model/transducer.py:62-68
             self.decoder = decoder_transformer(embeddings=self.embed, output_dim=self.hid_dim, d_model=512,
-                                               num_layers=opt.dec_layers, heads=8, d_ff=2048, dropout=opt.dropout)
+                                               num_layers=opt.dec_layers, heads=8, d_ff=2048, dropout=opt.dropout,
+                                               max_relative_positions=getattr(opt, "max_relative_positions", 0))
         self.fc1 = nn.Linear(2 * self.hid_dim, self.hid_dim)
         self.fc_gate = nn.Linear(2 * self.hid_dim, self.hid_dim)
         self.fc2 = nn.Linear(self.hid_dim, output_dim)

@@ -91,6 +91,9 @@ def build_parser():
     parser.add_argument('--layers', type=int, default=-1)
     parser.add_argument('--enc_layers', type=int, default=2)
     parser.add_argument('--dec_layers', type=int, default=2)
+    parser.add_argument('--max_relative_positions', type=int, default=0,
+                        help='relative-position self-attention in the transformer prediction net (--decoder_type transformer): clip '
+                             'distances to +-N, one table of 2N+1 rows per layer; 0 = off, the reference recipe')
     parser.add_argument('--rnn_size', type=int, default=512)
     parser.add_argument('--rnn_type', type=str, default='LSTM', choices=['LSTM'])
     parser.add_argument('--embd_dim', type=int, default=300)
