@@ -139,9 +139,14 @@ int pk_cast_split(const void* src, int src_dtype, long long ld_src, void* hi, vo
  *   trainer/model/modules/multi_headed_attn.py:199-223 (scale, softmax, dropout, context) and its autograd backward,
  * without materialising the [B, heads, T, T] score / probability tensors.
  *   q, k, v: element (b, t, h, d) at ptr[(b*T + t)*ld_qkv + h*64 + d]  (three column blocks of a fused [B,T,3D] projection)
- *   out / dout [B, T, heads*64] with row strides ld_out / ld_dout;  lse [B*heads*T] f32 saved for the backward
- *   dq, dk, dv: same addressing with row stride ld_dqkv;  dsum_ws: B*heads*T floats of scratch
- * Dropout masks are the same counter-based masks as pk_softmax_fwd/bwd for equal (drop_p, seed). */
+ *   out / dout [B, T, heads*64] with row strides ld_out / ld_dout;  lse [B*heads][pk_attention_lse_stride(T)] f32: the natural-log
+ *   row log-sum-exp of the scaled scores, entry t of (b, h) at lse[(b*heads + h)*pk_attention_lse_stride(T) + t], saved for the backward
+ *   dq, dk, dv: same addressing with row stride ld_dqkv;  dsum_ws: [B*heads][pk_attention_lse_stride(T)] f32 scratch
+ *   The padding t in [T, pk_attention_lse_stride(T)) of lse and dsum_ws is written by the kernels themselves (lse by the forward,
+ *   dsum_ws by the backward), so neither buffer needs initialising; the backward takes lse as the forward wrote it.
+ * Dropout masks are the same counter-based masks as pk_softmax_fwd/bwd for equal (drop_p, seed): row (b*heads + h)*T + t. */
+/* row pitch of lse / dsum_ws: T rounded up to a multiple of 64 */
+int pk_attention_lse_stride(int T);
 int pk_attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
                      int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream);
 int pk_attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,

@@ -297,7 +297,9 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
             const float l = quad_sum(l_run[hh]);
             inv[hh] = p.drop_scale / l;
             const int srow = srow0 + r0 + 8 * hh;
-            if ((lane & 3) == 0 && srow < T) p.lse[(size_t)bh * p.Tpad + srow] = (m_run[hh] + log2f(l)) * TA_LN2;
+            // rows in [T, Tpad) (zero queries: lse = ln(T)) are written too, so that the dK/dV mode, which streams whole 64-query
+            // tiles of lse, never reads a value the caller left there (a NaN would reach dK / dV through 0 * NaN)
+            if ((lane & 3) == 0 && srow < p.Tpad) p.lse[(size_t)bh * p.Tpad + srow] = (m_run[hh] + log2f(l)) * TA_LN2;
         }
 #pragma unroll
         for (int c = 0; c < 32; ++c) acc0[c] *= inv[(c >> 1) & 1];
@@ -326,6 +328,10 @@ __global__ void __launch_bounds__(256) attention_rowdot_tc_kernel(const __nv_bfl
         const float s = warp_sum(bf16lo(ov) * bf16lo(dv) + bf16hi(ov) * bf16hi(dv));
         if (lane == 0) dsum[((long long)b * heads + h) * Tpad + tt] = s;
     }
+    // D of the padding rows [T, Tpad) is 0, for the same reason as the forward's lse padding
+    const long long npad = (long long)B * heads * (Tpad - T);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npad; i += (long long)gridDim.x * blockDim.x)
+        dsum[(i / (Tpad - T)) * Tpad + T + i % (Tpad - T)] = 0.f;
 }
 
 static int attn_maps(AttnTcParams& p, const void* q, const void* k, const void* v, long long ld_qkv, const void* dout, long long ld_dout) {
@@ -384,7 +390,8 @@ extern "C" int pk_attention_fwd(const void* q, const void* k, const void* v, lon
     return launch_attn<0>(p, STREAM(stream));
 }
 
-/* dq/dk/dv share the row stride ld_dqkv (the fused [B,T,3D] gradient buffer); lse and dsum_ws: [B*heads][pk_attention_lse_stride(T)] */
+/* dq/dk/dv share the row stride ld_dqkv (the fused [B,T,3D] gradient buffer); lse and dsum_ws: [B*heads][pk_attention_lse_stride(T)],
+   whose padding t in [T, stride) the kernels write themselves (lse in the forward, dsum_ws here): neither needs initialising */
 extern "C" int pk_attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
                                 const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
                                 long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream) {

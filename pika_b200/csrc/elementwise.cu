@@ -1298,10 +1298,10 @@ extern "C" int pk_softmax_masked_fwd(const float* S, long long ld_s, void* P, vo
 }
 extern "C" int pk_softmax_bwd(const float* dPd, long long ld_d, const void* P, long long ld_p, void* dS, int dtype, long long rows,
                               int n, float drop_p, uint32_t seed, void* stream) {
+    PK_CHECK_ARG(rows > 0 && n > 0 && ld_p >= n && ld_d >= ld_p && ld_p <= 2048 && ld_p % 8 == 0 && ld_d % 8 == 0, "softmax rows: ld % 8 == 0, <= 2048 wide");
     const int grid = grid_for(rows, 8);
     const uint32_t th = drop_thresh16_of(drop_p);     // 16-bit pair mask (common.cuh drop_pair)
     const float sc = drop_scale16_of(th);
-    PK_CHECK_ARG(ld_p <= 2048 && ld_p % 8 == 0 && ld_d % 8 == 0, "softmax rows: ld % 8 == 0, <= 2048 wide");
     if (ld_p <= 1024) { PK_DISPATCH_T(dtype, (softmax_bwd_kernel<T, 4><<<grid, 256, 0, STREAM(stream)>>>(dPd, ld_d, (const T*)P, ld_p, (T*)dS, rows, n, th, sc, seed))); }
     else { PK_DISPATCH_T(dtype, (softmax_bwd_kernel<T, 8><<<grid, 256, 0, STREAM(stream)>>>(dPd, ld_d, (const T*)P, ld_p, (T*)dS, rows, n, th, sc, seed))); }
     DONE();

@@ -170,7 +170,7 @@ def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0):
     B, T, D3 = qkv.shape
     D = D3 // 3
     assert dout.is_contiguous() and dqkv.is_contiguous() and dqkv.shape == qkv.shape and dout.dtype == torch.bfloat16
-    ws = torch.zeros(B * heads * attention_lse_stride(T), dtype=torch.float32, device=qkv.device)     # pad entries must be finite (0)
+    ws = torch.zeros(B * heads * attention_lse_stride(T), dtype=torch.float32, device=qkv.device)     # D scratch (the kernel writes its padding too)
     base, gb, es = qkv.data_ptr(), dqkv.data_ptr(), 2
     vp = ctypes.c_void_p
     check(lib.pk_attention_bwd(vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(dout), _L(D), _P(lse), _P(ws),

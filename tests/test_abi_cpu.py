@@ -40,6 +40,18 @@ def test_workspace_queries_are_pure_host_functions():
     assert _lib.lib.pk_rnnt_loss_workspace_bytes(32, 240, 151) > 32 * 240 * 151 * 12
     _lib.lib.pk_frontend_workspace_bytes.restype = ctypes.c_longlong
     assert _lib.lib.pk_frontend_workspace_bytes(32, 160240, 1000, 80, 240) > 32 * 160240 * 12
+    # row pitch of the fused attention's lse / D vectors: T rounded up to 64
+    assert [_lib.lib.pk_attention_lse_stride(T) for T in (1, 63, 64, 65, 1000, 2048)] == [64, 64, 64, 128, 1024, 2048]
+
+
+def test_softmax_bwd_rejects_bad_shapes_before_touching_the_device():
+    """pk_softmax_bwd validates what its forward validates: n <= ld_p, ld_d >= ld_p, rows > 0"""
+    import ctypes as C
+    from pika_b200 import _lib
+    L, I, F, U, NULL = C.c_longlong, C.c_int, C.c_float, C.c_uint32, C.c_void_p(0)
+    for ld_d, ld_p, rows, n in ((64, 64, 16, 72), (56, 64, 16, 64), (64, 64, 0, 64), (64, 64, 16, 0)):
+        rc = _lib.lib.pk_softmax_bwd(NULL, L(ld_d), NULL, L(ld_p), NULL, I(0), L(rows), I(n), F(0.0), U(0), NULL)
+        assert rc < 0 and b"softmax rows" in _lib.lib.pk_last_error()
 
 
 def test_no_product_module_imports_the_oracle():
