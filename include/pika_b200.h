@@ -316,6 +316,34 @@ int pk_beam_advance_lm(const float* logits, int ldv, const float* row_lse, float
                        const int* step_ctx, int blk, int n_best, int beam_prune, const pk_lm_fst* fst, double lm_scale, double nonblk_reward,
                        int* set_state, double* set_cost, int* set_n, float* lm_scores, int max_states, int* err_flag, void* stream);
 
+/* Incremental step of the convolutional-transformer prediction net in the beam loop (pika_b200/csrc/beam_xf.cu): each row computes
+ * only its newest position p against a KV cache, decoder/transducer_decoder.py:117-120,151-171 without re-running the history.
+ * pool [n_entries][layers][3][D] (activation dtype): per layer the K row, the V row and (l >= 1) the layer's input, of one position;
+ * entry 0 = the shared SOS position, entry 1 + s*rows + row = the position `row` computes at beam step s.  slot [2][rows][S1] int32:
+ * position -> entry, ping-pong by step parity like hyp_tok [2][rows][S1] / hyp_len [2][rows].
+ * A row computes in step s = step_ctx[0] when next_ys[s][row] > blk, at p = hyp_len[s&1][row]; other rows are masked at the writes.
+ * init = 1: row 0 computes position 0 (token blk) into entry 0, and pk_beam_xf_select hands its output to every row. */
+typedef struct {
+    const int* next_ys;       /* [S+1][rows] */
+    const int* step_ctx;      /* [2] */
+    const int* hyp_tok;       /* [2][rows][S1] */
+    const int* hyp_len;       /* [2][rows] */
+    int* slot;                /* [2][rows][S1] */
+    void* pool;               /* [n_entries][layers][3][D] */
+    long long n_entries;
+    int blk, rows, S1, layers, D, dtype, init;
+} pk_beam_xf_state;
+/* taps [rows][5*ldc]: the causal Conv1d(k=5) im2col row of position p (x(p-4) .. x(p), zero before position 0).  Layer 0: embedding rows
+ * (f32 table [*, E]) of the tokens; layer >= 1: x_cur [rows][D] at p (also stored into the row's pool entry), the pool before it. */
+int pk_beam_xf_taps(const pk_beam_xf_state* st, int layer, const float* embed, int E, const void* x_cur, void* taps, int ldc, void* stream);
+/* qkv [rows][3D] (q | k | v) -> out [rows][D]: stores K / V of position p, attends over positions 0..p (fp32 online softmax, scale 1/8);
+ * head size 64 only.  max_rel > 0: relative positions, rel f32 [2*max_rel+1][64] shared by keys and values. */
+int pk_beam_xf_attn(const pk_beam_xf_state* st, int layer, const void* qkv, int heads, const float* rel, int max_rel, void* out, void* stream);
+/* h[row] = x[row] [rows][H] on the rows that computed a position */
+int pk_beam_xf_select(const pk_beam_xf_state* st, const void* x, void* h, int H, void* stream);
+/* after pk_beam_advance[_lm] of step s: slot[s&1^1][row] = slot[s&1][src] up to src's length (src = prev_ks[s][row], or row if it finished) */
+int pk_beam_xf_slots(const pk_beam_xf_state* st, const int* prev_ks, int K, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Persistent LSTM layer (pika_b200/csrc/lstm_seq.cu): the whole recurrence of one nn.LSTM layer in one
  * cooperative launch per 32 sequences (trainer/model/transducer.py:56-61,95), zero initial state.

@@ -3,7 +3,8 @@
 Same constructor and ``decode_batch(x, x_len, max_len) -> (ret, enc_out)`` contract
 (``ret = {"predictions": B x n_best lists of 0-d int64 tensors (full alignment incl. blanks, trailing EOS
 stripped), "scores": B x n_best 0-d f32 tensors}``).  All per-step work runs on the GPU for the whole batch:
-encoder-frame gather, masked LSTM step, factored joint, log-softmax, and one ``pk_beam_advance`` launch that
+encoder-frame gather, masked LSTM step (or the transformer prediction net's incremental KV-cached step, _XfBuffers),
+factored joint, log-softmax, and one ``pk_beam_advance`` launch that
 performs every utterance's score add / EOS + duplicate kill / top-k / finish rule / hypothesis update
 (decoder/beam_transducer.py:82-187), optionally with on-the-fly FST shallow fusion (:135-159,167-176).
 
@@ -26,7 +27,7 @@ import torch
 from .. import engine
 from .. import kernels as K
 from .. import _lib
-from .._lib import check, lib
+from .._lib import PikaError, check, lib
 
 _USE_GRAPH = os.environ.get("PK_DECODE_GRAPH", "1") != "0"      # 0: issue every launch of the beam loop from the host (debugging)
 _POLL = 4                                                        # graph replays (= 8 beam steps) between looks at the done counter
@@ -40,7 +41,7 @@ class _Workspace:
         self.B, self.Tcap, self.Scap, self.adt, self.dev = B, Tcap, Scap, adt, dev
         H = m.fc1.weight.shape[0]
         V = m.fc2.weight.shape[0]
-        L = m.decoder.num_layers if dec.xf is False else 0         # transformer prediction net: no recurrent state (see _xf_states)
+        L = m.decoder.num_layers if dec.xf is False else 0         # transformer prediction net: its state is the KV cache (_XfBuffers)
         E = m.embed.weight.shape[1]
         self.H, self.V, self.L, self.E = H, V, L, E
         # layer 0 reads the embedding row zero-padded to the hidden width, so that x W_ih^T + h W_hh^T of a layer is ONE GEMM launch with two
@@ -92,6 +93,7 @@ class _Workspace:
             self.lm = dict(fst=fst_struct, keep=keep, set_state=i32(2, B, Kb, MS),
                            set_cost=torch.zeros(2, B, Kb, MS, dtype=torch.float64, device=dev), set_n=i32(2, B, Kb),
                            lm_scores=f32(B, Kb), err=i32(1))
+        self.xf = _XfBuffers(self, dec, wbuf) if dec.xf else None
         self.graph = None
         self.kernels_per_replay = 0
         self.sig = None                     # what the captured graph baked in besides the workspace addresses
@@ -99,22 +101,19 @@ class _Workspace:
     def stage(self, dec):
         """live parameters -> the fixed staging buffers"""
         m, lstm = dec.model, dec.model.decoder
-
-        def put(bufs, param, cols_pad=None, rows=None):
-            mat = param.detach().reshape(param.shape[0], -1)
-            dst = bufs if rows is None else [b[rows[0]:rows[1]] for b in bufs]
-            K.cast_split(mat, dst[0], dst[1] if len(dst) > 1 else None, cols_pad=cols_pad or mat.shape[1])
         H = self.H
         for l in range(self.L):                          # (no LSTM layers with the transformer prediction net)
-            put(self.w_ih[l], getattr(lstm, "weight_ih_l%d" % l), cols_pad=self.ldx if l == 0 else None)
-            put(self.w_hh[l], getattr(lstm, "weight_hh_l%d" % l))
+            _put(self.w_ih[l], getattr(lstm, "weight_ih_l%d" % l), cols_pad=self.ldx if l == 0 else None)
+            _put(self.w_hh[l], getattr(lstm, "weight_hh_l%d" % l))
             K.add(getattr(lstm, "bias_ih_l%d" % l).detach(), getattr(lstm, "bias_hh_l%d" % l).detach(), self.bsum[l])
-        put(self.wx, m.fc1.weight, rows=(0, H))
-        put(self.wx, m.fc_gate.weight, rows=(H, 2 * H))
-        put(self.w2, m.fc2.weight)
+        _put(self.wx, m.fc1.weight, rows=(0, H))
+        _put(self.wx, m.fc_gate.weight, rows=(H, 2 * H))
+        _put(self.w2, m.fc2.weight)
         self.bx[:H].copy_(m.fc1.bias.detach())
         self.bx[H:].copy_(m.fc_gate.bias.detach())
         self.b2.copy_(m.fc2.bias.detach())
+        if self.xf is not None:
+            self.xf.stage(dec)
 
     def reset(self, dec, enc, x_len, ml_list):
         B, blk = self.B, dec.blk
@@ -132,6 +131,105 @@ class _Workspace:
         if self.lm is not None:
             for k in ("set_state", "set_cost", "set_n", "lm_scores", "err"):
                 self.lm[k].zero_()
+        if self.xf is not None:
+            self.xf.slot.zero_()                # position 0 of every row is the shared SOS entry 0
+
+
+class _XfBuffers:
+    """Device state of the transformer prediction net's incremental beam step (pika_b200/csrc/beam_xf.cu), at fixed addresses.
+
+    pool [1 + Scap * rows, layers, 3, d_model] (activation dtype): one entry per computed position, written once and never moved --
+    per layer its K row, its V row and (layer >= 1) the layer's input, which the next positions' causal conv taps read.  Entry 0 is
+    the SOS position shared by every row, entry 1 + s * rows + row the position that `row` computed at beam step s.  That is
+    (1 + Scap * rows) * layers * 3 * d_model elements: 3.0 GB in bf16 at batch 64 x beam 16, 2 layers, d_model 512, Scap = T' + 102 = 477.
+    slot [2, B, beam, Scap + 1] int32 maps a row's positions to entries, ping-ponged by step parity like hyp_tok and reordered by the
+    back-pointers after every advance (pk_beam_xf_slots), so the rows of one utterance share their common prefix's entries."""
+
+    def __init__(self, ws, dec, wbuf):
+        pn, dev, adt = dec.model.decoder, ws.dev, ws.adt
+        rows, H, S = ws.rows, ws.H, ws.Scap
+        self.layers, self.D, self.heads = len(pn.transformer), pn.linear_out.weight.shape[1], pn.transformer[0].self_attn.head_count
+        D, dff = self.D, pn.transformer[0].feed_forward.w_1.weight.shape[0]
+        act = lambda *s: torch.zeros(*s, dtype=adt, device=dev)                         # noqa: E731
+        f32 = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)               # noqa: E731
+        self.n_entries = 1 + S * rows
+        self.pool = torch.empty(self.n_entries, self.layers, 3, D, dtype=adt, device=dev)
+        self.slot = torch.zeros(2, ws.B, dec.beam_size, S + 1, dtype=torch.int32, device=dev)
+        self.ld_tap = [ws.ldx] + [D] * (self.layers - 1)                                # layer 0 reads the (padded) embedding rows
+        self.taps = [act(rows, 5 * ld) for ld in self.ld_tap]
+        self.cv, self.ln, self.ctx, self.h1, self.xl = (act(rows, D) for _ in range(5))
+        self.qkv, self.ff, self.xo = act(rows, 3 * D), act(rows, dff), act(rows, H)
+        self.mean, self.rstd = f32(rows), f32(rows)
+        # staged weights, re-filled from the live parameters at every decode_batch (stage)
+        n = self.layers
+        self.conv_w = [wbuf(D, 5 * ld) for ld in self.ld_tap]                           # tap-major: tap k at columns [k*ld, k*ld + C)
+        self.qkv_w, self.fo_w = [wbuf(3 * D, D) for _ in range(n)], [wbuf(D, D) for _ in range(n)]
+        self.w1, self.w2 = [wbuf(dff, D) for _ in range(n)], [wbuf(D, dff) for _ in range(n)]
+        self.conv_b, self.qkv_b, self.fo_b = [f32(D) for _ in range(n)], [f32(3 * D) for _ in range(n)], [f32(D) for _ in range(n)]
+        self.b1, self.b2 = [f32(dff) for _ in range(n)], [f32(D) for _ in range(n)]
+        self.ln1 = [(f32(D), f32(D)) for _ in range(n)]
+        self.ln2 = [(f32(D), f32(D)) for _ in range(n)]
+        self.lnf = (f32(D), f32(D))
+        self.out_w, self.out_b = wbuf(H, D), f32(H)
+        self.rel = [f32(*l.self_attn.relative_positions_embeddings.weight.shape) if getattr(l.self_attn, "max_relative_positions", 0) > 0
+                    else None for l in pn.transformer]
+        self.eps = [(l.layer_norm.eps, l.feed_forward.layer_norm.eps) for l in pn.transformer] + [pn.layer_norm.eps]
+        P = lambda t: t.data_ptr()                                                      # noqa: E731
+        self.st, self.st_init = (K.BeamXfState(P(ws.next_ys), P(ws.step_ctx), P(ws.hyp_tok), P(ws.hyp_len), P(self.slot), P(self.pool),
+                                               self.n_entries, dec.blk, rows, S + 1, self.layers, D, K._dt(self.pool), init)
+                                 for init in (0, 1))
+
+    def stage(self, dec):
+        pn = dec.model.decoder
+        for l, (conv, layer) in enumerate(zip(pn.conv, pn.transformer)):
+            att, ff = layer.self_attn, layer.feed_forward
+            N, C, Kw = conv.weight.shape
+            taps = torch.zeros(N, Kw, self.ld_tap[l], dtype=torch.float32, device=conv.weight.device)
+            taps[:, :, :C] = conv.weight.detach().permute(0, 2, 1)
+            _put(self.conv_w[l], taps.view(N, -1))
+            self.conv_b[l].copy_(conv.bias.detach())
+            for r, lin in enumerate((att.linear_query, att.linear_keys, att.linear_values)):
+                _put(self.qkv_w[l], lin.weight, rows=(r * self.D, (r + 1) * self.D))
+                self.qkv_b[l][r * self.D:(r + 1) * self.D].copy_(lin.bias.detach())
+            for w, b, lin in ((self.fo_w, self.fo_b, att.final_linear), (self.w1, self.b1, ff.w_1), (self.w2, self.b2, ff.w_2)):
+                _put(w[l], lin.weight)
+                b[l].copy_(lin.bias.detach())
+            for dst, ln in ((self.ln1[l], layer.layer_norm), (self.ln2[l], ff.layer_norm)):
+                dst[0].copy_(ln.weight.detach())
+                dst[1].copy_(ln.bias.detach())
+            if self.rel[l] is not None:
+                self.rel[l].copy_(att.relative_positions_embeddings.weight.detach())
+        self.lnf[0].copy_(pn.layer_norm.weight.detach())
+        self.lnf[1].copy_(pn.layer_norm.bias.detach())
+        _put(self.out_w, pn.linear_out.weight)
+        self.out_b.copy_(pn.linear_out.bias.detach())
+
+    def step(self, dec, h, init=False):
+        """the prediction net's output at every computing row's new position -> h [rows, H] (other rows keep theirs); ``init``: the SOS
+        position into entry 0 and its output into every row, ``decoder([blk])[:, -1]`` (decoder/transducer_decoder.py:117-120)"""
+        st = self.st_init if init else self.st
+        emb = dec.model.embed.weight.detach()
+        A = engine.stage_act
+        for l in range(self.layers):
+            K.beam_xf_taps(st, l, emb, self.xl if l > 0 else None, self.taps[l])
+            engine.gemm_parts([A(self.taps[l])], [self.conv_w[l]], self.cv, bias=self.conv_b[l], act=K.ACT_RELU)
+            K.layernorm_fwd(self.cv, self.ln, self.ln1[l][0], self.ln1[l][1], self.eps[l][0], self.mean, self.rstd)
+            engine.gemm_parts([A(self.ln)], [self.qkv_w[l]], self.qkv, bias=self.qkv_b[l])
+            K.beam_xf_attn(st, l, self.qkv, self.heads, self.rel[l], self.ctx)
+            engine.gemm_parts([A(self.ctx)], [self.fo_w[l]], self.h1, bias=self.fo_b[l], aux=self.cv, aux_mode=K.AUX_ADD)
+            K.layernorm_fwd(self.h1, self.ln, self.ln2[l][0], self.ln2[l][1], self.eps[l][1], self.mean, self.rstd)
+            engine.gemm_parts([A(self.ln)], [self.w1[l]], self.ff, bias=self.b1[l], act=K.ACT_RELU)
+            engine.gemm_parts([A(self.ff)], [self.w2[l]], self.xl, bias=self.b2[l], aux=self.h1, aux_mode=K.AUX_ADD)
+        K.layernorm_fwd(self.xl, self.ln, self.lnf[0], self.lnf[1], self.eps[-1], self.mean, self.rstd)
+        engine.gemm_parts([A(self.ln)], [self.out_w], self.xo, bias=self.out_b)
+        K.beam_xf_select(st, self.xo, h)
+
+
+def _put(bufs, param, cols_pad=None, rows=None):
+    """live parameter -> its fixed staging buffers ([hi] or [hi, lo] bf16), optionally into a row range of them"""
+    mat = param.detach().reshape(param.shape[0], -1)
+    dst = bufs if rows is None else [b[rows[0]:rows[1]] for b in bufs]
+    K.cast_split(mat, dst[0], dst[1] if len(dst) > 1 else None, cols_pad=cols_pad or mat.shape[1])
 
 
 class TransducerDecoder():
@@ -151,8 +249,12 @@ class TransducerDecoder():
         if args is not None and getattr(args, "bilas_rescorer", None) is not None:
             self.bilas_rescorer = args.bilas_rescorer
         self.xf = model.decoder_type != "rnn"            # convolutional-transformer prediction net (decoder/transducer_decoder.py:117-120,151-171)
-        if self.xf and lm_scorer is not None:
-            raise NotImplementedError("pika_b200: FST fusion is wired to the LSTM prediction net only")
+        if self.xf:
+            heads = {l.self_attn.head_count for l in model.decoder.transformer}
+            d_model = model.decoder.linear_out.weight.shape[1]
+            if any(d_model != 64 * h for h in heads):
+                raise PikaError("pika_b200: the transformer prediction net's beam step needs a head size of 64 (d_model %d, heads %s)"
+                                % (d_model, sorted(heads)))
         self._ws = None
         self.last_replays = self.kernels_per_replay = 0
 
@@ -165,29 +267,10 @@ class TransducerDecoder():
             ws = self._ws = _Workspace(self, B, max(Tenc, ws.Tcap if same else 0), max(S, ws.Scap if same else 0), adt, dev)
         return ws
 
-    def _xf_states(self, ws, par):
-        """prediction-net output for every beam row from its current partial hypothesis (transformer branch,
-        decoder/transducer_decoder.py:117-120,151-171).  The reference re-runs the whole history through the network for the rows that
-        just emitted a label and keeps / reorders the stored output row otherwise; the network is causal and masks padding keys, so a
-        row's output at its last position depends on its own history only -- recomputing every row from the hypothesis buffers
-        (which ``pk_beam_advance`` already reorders) gives the same values and needs no state reorder."""
-        m, rows = self.model, ws.rows
-        hl = ws.hyp_len[par].reshape(rows)
-        lmax = int(hl.max().item())
-        pad = m.embed.padding_idx
-        src = torch.full((rows, lmax + 1), pad, dtype=torch.long, device=ws.dev)
-        src[:, 0] = self.blk
-        if lmax > 0:
-            tok = ws.hyp_tok[par].reshape(rows, -1)[:, :lmax].long()
-            keep = torch.arange(lmax, device=ws.dev)[None, :] < hl[:, None]
-            src[:, 1:] = torch.where(keep, tok, torch.full_like(tok, pad))
-        out = engine.conv_transformer_lm_forward_act(m.decoder, src)                       # [rows, lmax + 1, H]
-        return out[torch.arange(rows, device=ws.dev), hl.long()].contiguous()
-
-    def _beam_step(self, ws, h, c, t_idx, h_out, c_out, t_out, par=None):
+    def _beam_step(self, ws, h, c, t_idx, h_out, c_out, t_out):
         """one iteration of `while not all(b.done() ...)` (decoder/transducer_decoder.py:123-186) for the whole batch;
-        graph-capturable with the LSTM prediction net: no host reads, no step-dependent arguments (the kernels read the step from
-        ``step_ctx``).  ``par`` (transformer prediction net only): parity of the step, selects the live hypothesis buffers."""
+        graph-capturable: no host reads, no step-dependent arguments (the kernels read the step from ``step_ctx``).  With the
+        transformer prediction net h[0] holds dec_states and the incremental step (_XfBuffers.step) replaces the LSTM cells."""
         m, Kb, blk = self.model, self.beam_size, self.blk
         P, st = K._P, K._stream
         H, V, L, rows = ws.H, ws.V, ws.L, ws.rows
@@ -203,7 +286,9 @@ class TransducerDecoder():
                 engine.gemm_parts([engine.stage_act(h[l])], [ws.w_hh[l]], ws.gates, accumulate=True, k_splits=1)
             check(lib.pk_beam_lstm_cell(P(ws.gates), P(ws.next_ys), P(ws.step_ctx), blk, P(h[l]), dt, P(c[l]), rows, H, st()), "pk_beam_lstm_cell")
             xin = h[l]
-        dec_hid = self._xf_states(ws, par) if self.xf else h[L - 1]
+        if self.xf:
+            ws.xf.step(self, h[0])
+        dec_hid = h[0] if self.xf else h[L - 1]
         engine.gemm_parts([engine.stage_act(ws.enc_hid), engine.stage_act(dec_hid)],
                           [[p[:, :H] for p in ws.wx], [p[:, H:] for p in ws.wx]], ws.pre, bias=ws.bx)
         check(lib.pk_beam_gate(P(ws.pre), P(ws.hj), K._dt(ws.hj), rows, H, st()), "pk_beam_gate")
@@ -221,8 +306,10 @@ class TransducerDecoder():
             check(lib.pk_beam_advance_lm(*common, ctypes.byref(lm["fst"]), ctypes.c_double(self.lm_scorer_scale),
                                          ctypes.c_double(float(getattr(self.args, "nonblk_reward", 0.0))), P(lm["set_state"]), P(lm["set_cost"]),
                                          P(lm["set_n"]), P(lm["lm_scores"]), self.lm_max_states, P(lm["err"]), st()), "pk_beam_advance_lm")
-        check(lib.pk_beam_reorder(P(ws.prev_ks), P(ws.step_ctx), P(h), P(c), P(t_idx), P(h_out), P(c_out), P(t_out), dt, Kb, H, L, rows, st()),
-              "pk_beam_reorder")
+        if self.xf:
+            K.beam_xf_slots(ws.xf.st, ws.prev_ks, Kb)
+        check(lib.pk_beam_reorder(P(ws.prev_ks), P(ws.step_ctx), P(h), P(c), P(t_idx), P(h_out), P(c_out), P(t_out), dt, Kb, H, h.shape[0], rows,
+                                  st()), "pk_beam_reorder")
         check(lib.pk_beam_step_end(P(ws.step_ctx), P(ws.not_done), ws.Scap - 1, st()), "pk_beam_step_end")
 
     def _period(self, ws):
@@ -236,6 +323,13 @@ class TransducerDecoder():
         m, blk = self.model, self.blk
         dev = x.device if enc_out is None else enc_out.device
         assert dev.type == "cuda", "pika_b200 decodes on the GPU (there is no CPU fallback)"
+        if self.xf:
+            # a hypothesis of up to max_len + 1 labels plus SOS; the prediction net's causal mask buffer is max_size (5000) positions long
+            n = max(int(v) if v else 10000 for v in max_len) + 2
+            max_size = m.decoder.mask.shape[-1]
+            if n > max_size:
+                raise PikaError("pika_b200: max_len allows histories of %d positions; the transformer prediction net's max_size is %d"
+                                % (n, max_size))
         if enc_out is None:
             enc = engine.model_encoder_forward_act(m, x, x_len).contiguous()     # [B, T', H] (packed over x_len: LSTM encoder)
         else:
@@ -248,15 +342,16 @@ class TransducerDecoder():
         ws.reset(self, enc, x_len, ml_list)
 
         if self.xf:
-            return self._decode_loop_xf(ws, enc, B)
-        # initial decoder state = LSTM(embed(blk)) from zeros (decoder/transducer_decoder.py:116)
-        ws.x_emb.zero_()
-        ws.x_emb[:, :ws.E] = m.embed.weight.detach()[blk].to(ws.adt)
-        xin = ws.x_emb
-        for l in range(ws.L):
-            engine.gemm_parts([engine.stage_act(xin)], [ws.w_ih[l]], ws.gates, bias=ws.bsum[l])
-            K.lstm_cell_fwd(ws.gates, None, None, ws.c[l], ws.h[l], None, ws.rows, H)
-            xin = ws.h[l]
+            ws.xf.step(self, ws.h[0], init=True)                              # decoder([blk])[:, -1] (decoder/transducer_decoder.py:117-120)
+        else:
+            # initial decoder state = LSTM(embed(blk)) from zeros (decoder/transducer_decoder.py:116)
+            ws.x_emb.zero_()
+            ws.x_emb[:, :ws.E] = m.embed.weight.detach()[blk].to(ws.adt)
+            xin = ws.x_emb
+            for l in range(ws.L):
+                engine.gemm_parts([engine.stage_act(xin)], [ws.w_ih[l]], ws.gates, bias=ws.bsum[l])
+                K.lstm_cell_fwd(ws.gates, None, None, ws.c[l], ws.h[l], None, ws.rows, H)
+                xin = ws.h[l]
 
         max_steps = ws.Scap - 1
         sig = (m.embed.weight.data_ptr(), float(self.sm_scale), int(bool(self.beam_prune)), self.n_best, self.lm_scorer_scale,
@@ -288,18 +383,6 @@ class TransducerDecoder():
                 break
         if ws.lm is not None and int(ws.lm["err"].item()) != 0:
             raise RuntimeError("pika_b200: an FST state set outgrew lm_max_states=%d active states per beam" % self.lm_max_states)
-        return self._extract(ws, enc, B)
-
-    def _decode_loop_xf(self, ws, enc, B):
-        """beam loop with the transformer prediction net: issued step by step from the host (the history length, hence every shape
-        of the prediction net, changes with the step, so there is no fixed graph to replay)"""
-        bufs = ((ws.t_idx, ws.t_alt), (ws.t_alt, ws.t_idx))
-        for i in range(ws.Scap - 1):
-            t_in, t_out = bufs[i & 1]
-            self._beam_step(ws, ws.h, ws.c, t_in, ws.h, ws.c, t_out, par=i & 1)
-            if int(ws.not_done.item()) == 0:                                    # `while not all(b.done() for b in beam)`
-                break
-        self.last_replays = 0
         return self._extract(ws, enc, B)
 
     # ------------------------------------------------------------------------------------------------ LAS rescoring hooks

@@ -386,6 +386,36 @@ def scatter_add_rows(src, idx, dst):
     check(lib.pk_scatter_add_rows(_P(src), _P(idx), _P(dst), _I(_dt(src)), _L(rows), _I(C), _stream()), "pk_scatter_add_rows")
 
 
+class BeamXfState(ctypes.Structure):
+    """pk_beam_xf_state (include/pika_b200.h): the device buffers of the transformer prediction net's incremental beam step"""
+    _fields_ = [("next_ys", ctypes.c_void_p), ("step_ctx", ctypes.c_void_p), ("hyp_tok", ctypes.c_void_p), ("hyp_len", ctypes.c_void_p),
+                ("slot", ctypes.c_void_p), ("pool", ctypes.c_void_p), ("n_entries", ctypes.c_longlong), ("blk", ctypes.c_int),
+                ("rows", ctypes.c_int), ("S1", ctypes.c_int), ("layers", ctypes.c_int), ("D", ctypes.c_int), ("dtype", ctypes.c_int),
+                ("init", ctypes.c_int)]
+
+
+def beam_xf_taps(st, layer, embed, x_cur, taps):
+    """taps [rows, 5 * ldc]: the causal conv's im2col row of every row's new position (layer 0: embedding rows of ``embed`` f32)"""
+    assert embed.dtype == torch.float32 and embed.is_contiguous() and taps.is_contiguous()
+    check(lib.pk_beam_xf_taps(ctypes.byref(st), _I(layer), _P(embed), _I(embed.shape[1]), _P(x_cur), _P(taps), _I(taps.shape[1] // 5),
+                              _stream()), "pk_beam_xf_taps")
+
+
+def beam_xf_attn(st, layer, qkv, heads, rel, out):
+    """qkv [rows, 3D] -> out [rows, D]: single-query attention over each row's cached positions; rel: f32 [2m+1, 64] or None"""
+    assert qkv.is_contiguous() and out.is_contiguous() and (rel is None or (rel.dtype == torch.float32 and rel.is_contiguous()))
+    check(lib.pk_beam_xf_attn(ctypes.byref(st), _I(layer), _P(qkv), _I(heads), _P(rel), _I(0 if rel is None else rel.shape[0] // 2), _P(out),
+                              _stream()), "pk_beam_xf_attn")
+
+
+def beam_xf_select(st, x, h):
+    check(lib.pk_beam_xf_select(ctypes.byref(st), _P(x), _P(h), _I(h.shape[-1]), _stream()), "pk_beam_xf_select")
+
+
+def beam_xf_slots(st, prev_ks, K):
+    check(lib.pk_beam_xf_slots(ctypes.byref(st), _P(prev_ks), _I(K), _stream()), "pk_beam_xf_slots")
+
+
 def ce_grad(z, tok, coef, scale, dz, n):
     rows, ld = z.shape
     check(lib.pk_ce_grad(_P(z), _I(_dt(z)), _L(ld), _P(tok), _P(coef), _F(scale), _P(dz), _L(rows), _I(n), _stream()), "pk_ce_grad")
