@@ -144,14 +144,31 @@ int pk_cast_split(const void* src, int src_dtype, long long ld_src, void* hi, vo
  *   dq, dk, dv: same addressing with row stride ld_dqkv;  dsum_ws: [B*heads][pk_attention_lse_stride(T)] f32 scratch
  *   The padding t in [T, pk_attention_lse_stride(T)) of lse and dsum_ws is written by the kernels themselves (lse by the forward,
  *   dsum_ws by the backward), so neither buffer needs initialising; the backward takes lse as the forward wrote it.
- * Dropout masks are the same counter-based masks as pk_softmax_fwd/bwd for equal (drop_p, seed): row (b*heads + h)*T + t. */
+ * Dropout masks are the same counter-based masks as pk_softmax_fwd/bwd for equal (drop_p, seed): row (b*heads + h)*T + t.
+ * pk_attention_fwd / pk_attention_bwd draw the mask from seed in every kernel.  pk_attention_fwd_bits also writes every keep decision
+ * as one bit into keep_bits, and pk_attention_bwd_bits reads those bits instead of hashing (so it takes no seed) -- the cheaper pair
+ * for a forward whose backward follows.  keep_bits is caller-allocated, pk_attention_keep_bits_bytes(B, T, heads) bytes, 16-byte
+ * aligned, needs no initialising, and may be NULL only when drop_p == 0.  Layout, with n = 2 * ceil(T / 128) blocks of 64 along each axis:
+ *   words [B*heads][n query blocks][n key blocks][128] (uint32); in block (qb, kb) the decision for query qb*64 + r, key kb*64 + c
+ *   is bit ((r >> 3) & 1) * 16 + (c >> 3) * 2 + (c & 1) of word (r >> 4) * 32 + ((c & 7) >> 1) * 8 + (r & 7).
+ * That is the wgmma accumulator layout of the 64 x 64 score block: the thread that holds (r, c) in the forward and dQ kernels owns
+ * the whole word, and the dK/dV kernel, which holds the transposed block, finds its 32 decisions in four pairs of adjacent words.
+ * Blocks beyond the sequence (query or key >= T) are never read for a decision that reaches an output. */
 /* row pitch of lse / dsum_ws: T rounded up to a multiple of 64 */
 int pk_attention_lse_stride(int T);
+/* bytes of the keep-bit buffer: B * heads * (2 * ceil(T / 128))^2 * 512 */
+long long pk_attention_keep_bits_bytes(int B, int T, int heads);
 int pk_attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
                      int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream);
 int pk_attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
                      const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
                      long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream);
+int pk_attention_fwd_bits(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                          int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits, void* stream);
+int pk_attention_bwd_bits(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                          const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                          long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
+                          void* stream);
 /* nn.BatchNorm1d over rows [rows, C] (trainer/model/rnnt_tdnn_transformer.py:41,58-59,69,76-82,85):
  * train: batch statistics incl. padded frames, running stats updated (momentum 0.1); eval: running stats.
  * stats_ws: pk_colstats_ws_floats(C) + 2*C floats scratch.  mean/rstd [C] are saved for the backward. */

@@ -76,6 +76,7 @@ def _sig(name, argtypes, restype=ctypes.c_int):
 _sig("pk_gemm_bf16", [ctypes.POINTER(GemmDesc), _vp])
 _sig("pk_gemm_row_lse_parts", [_ll, _ll, _i])
 _sig("pk_rnnt_loss_workspace_bytes", [_i, _i, _i], ctypes.c_longlong)
+_sig("pk_attention_keep_bits_bytes", [_i, _i, _i], ctypes.c_longlong)
 _sig("pk_rnnt_loss_colsum_workspace_bytes", [_i, _i, _i, _i], ctypes.c_longlong)
 _sig("pk_rnnt_loss_fwd_bwd", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp])
 _sig("pk_rnnt_loss_fwd_bwd_lse", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _i, _vp])

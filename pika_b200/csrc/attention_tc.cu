@@ -16,7 +16,11 @@
 //                    registers (the accumulator layout of an m64 x 16 block is the A-operand layout of wgmma).
 //
 // Dropout: counter-based mask shared with the stand-alone softmax kernels -- one 32-bit hash per PAIR of adjacent keys
-// (index (row * ceil(T/2) + key/2) over the [B*heads*T, T] probability matrix), 16 bits per element.
+// (index (row * ceil(T/2) + key/2) over the [B*heads*T, T] probability matrix), 16 bits per element.  The kernels are compiled
+// per dropout case (template DROP): none, hashed from the seed in every mode (pk_attention_fwd / _bwd), or keep bits
+// (pk_attention_fwd_bits / _bwd_bits): the forward alone hashes and writes each decision as one bit (layout in
+// include/pika_b200.h), and the backward reads them -- MODE 1 one word per thread and tile straight from global memory, MODE 2 the
+// transposed 64 x 128 block through the loader's ring.
 #include <cstdlib>
 #include <cstring>
 
@@ -38,7 +42,10 @@ constexpr int TA_TILE_X = TA_BC * 128;            // 8 KB
 constexpr int TA_OFF_STAT = 0;                    // two stationary tiles
 constexpr int TA_OFF_RING = 2 * TA_TILE_S;        // NST x (X1, X2)
 constexpr int TA_OFF_VEC = TA_OFF_RING + TA_NST * 2 * TA_TILE_X;       // [NST][2][64] floats (MODE 2: lse, D of the streamed queries)
-constexpr int TA_OFF_BAR = TA_OFF_VEC + TA_NST * 2 * TA_BC * 4;
+enum : int { TA_DROP_NONE = 0, TA_DROP_HASH = 1, TA_DROP_BITS = 2 };
+constexpr int TA_KB_BLOCK = 512;                                        // keep bits of one 64 x 64 (query, key) block
+constexpr int TA_OFF_KB = TA_OFF_VEC + TA_NST * 2 * TA_BC * 4;          // [NST][2 blocks] keep bits (MODE 2, dropout)
+constexpr int TA_OFF_BAR = TA_OFF_KB + TA_NST * 2 * TA_KB_BLOCK;
 constexpr int TA_SMEM = TA_OFF_BAR + 256 + 1024;
 
 struct AttnTcParams {
@@ -47,7 +54,8 @@ struct AttnTcParams {
     __nv_bfloat16* dq; __nv_bfloat16* dk; __nv_bfloat16* dv; long long ld_dqkv;
     float* lse;                                   // [B*heads][Tpad] natural-log row log-sum-exp of the scaled scores
     float* dsum;                                  // [B*heads][Tpad] D_i = sum_d dO_id O_id
-    int B, T, heads, Tpad, Tp2;
+    uint32_t* keep_bits;                          // [B*heads][nkb][nkb][128] words (MODE 0 writes, MODES 1 / 2 read); dropout only
+    int B, T, heads, Tpad, Tp2, nkb;
     float alpha;
     uint32_t thresh16; float drop_scale; uint32_t seed;
 };
@@ -59,6 +67,8 @@ PK_DEVICE void frag_a(const float (&x)[32], int kk, uint32_t (&a)[4]) {
     a[2] = pack_bf16x2(x[8 * kk + 4], x[8 * kk + 5]);
     a[3] = pack_bf16x2(x[8 * kk + 6], x[8 * kk + 7]);
 }
+// first word of the keep bits of query block qb x key block kb (64 x 64 each) of (batch, head) bh
+PK_DEVICE size_t kb_block(const AttnTcParams& p, int bh, int qb, int kb) { return (((size_t)bh * p.nkb + qb) * p.nkb + kb) * (TA_KB_BLOCK / 4); }
 PK_DEVICE float quad_max(float v) { return fmaxf(v, fmaxf(__shfl_xor_sync(0xffffffffu, v, 1), __shfl_xor_sync(0xffffffffu, fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1)), 2))); }
 PK_DEVICE float quad_sum(float v) { v += __shfl_xor_sync(0xffffffffu, v, 1); return v + __shfl_xor_sync(0xffffffffu, v, 2); }
 
@@ -75,7 +85,9 @@ PK_DEVICE void store_tile(const float (&x)[32], __nv_bfloat16* base, long long l
     }
 }
 
-template <int MODE>
+// DROP: TA_DROP_NONE (p = 0: no mask code at all), TA_DROP_HASH (every mode hashes the mask from the seed) or TA_DROP_BITS (MODE 0
+// hashes it and writes the keep bits, MODES 1 / 2 read them)
+template <int MODE, int DROP>
 __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -114,18 +126,23 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
             tma_load_3d_p(smem + TA_OFF_STAT + half * TA_TILE_X, ma0, stat_full, h * 64, row_base + half * 64, b, lead);
             if (MODE != 0) tma_load_3d_p(smem + TA_OFF_STAT + TA_TILE_S + half * TA_TILE_X, ma1, stat_full, h * 64, row_base + half * 64, b, lead);
         }
+        constexpr bool kb_load = MODE == 2 && DROP == TA_DROP_BITS;
         int stage = 0;
         uint32_t phase = 0;
         for (int j = 0; j < n_tiles; ++j) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* x1 = smem + TA_OFF_RING + stage * 2 * TA_TILE_X;
-            mbar_arrive_expect_tx_p(&full_bar[stage], 2 * TA_TILE_X + (MODE == 2 ? 2 * TA_BC * 4 : 0), lead);
+            mbar_arrive_expect_tx_p(&full_bar[stage], 2 * TA_TILE_X + (MODE == 2 ? 2 * TA_BC * 4 : 0) + (kb_load ? 2 * TA_KB_BLOCK : 0), lead);
             tma_load_3d_p(x1, mx1, &full_bar[stage], h * 64, j * TA_BC, b, lead);
             tma_load_3d_p(x1 + TA_TILE_X, mx2, &full_bar[stage], h * 64, j * TA_BC, b, lead);
             if (MODE == 2) {
                 const size_t off = (size_t)bh * p.Tpad + (size_t)j * TA_BC;
                 bulk_load_p(vec + (stage * 2 + 0) * TA_BC, p.lse + off, TA_BC * 4, &full_bar[stage], lead);
                 bulk_load_p(vec + (stage * 2 + 1) * TA_BC, p.dsum + off, TA_BC * 4, &full_bar[stage], lead);
+                // streamed query block j x the CTA's two key blocks: adjacent in the layout, so one 1 KB copy
+                if (kb_load)
+                    bulk_load_p(smem + TA_OFF_KB + stage * 2 * TA_KB_BLOCK, p.keep_bits + kb_block(p, bh, j, 2 * blockIdx.x), 2 * TA_KB_BLOCK,
+                                &full_bar[stage], lead);
             }
             if (++stage == TA_NST) { stage = 0; phase ^= 1; }
         }
@@ -141,19 +158,21 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     const int srow0 = row_base + wg * 64;             // first stationary index of the warpgroup
     const uint64_t stat_row0 = (uint64_t)bh * (uint64_t)T;   // row offset into the dropout index space
     const float c2 = p.alpha * TA_LOG2E;
-    const bool use_drop = p.thresh16 != 0u;
+    constexpr bool use_drop = DROP != TA_DROP_NONE, KB = DROP == TA_DROP_BITS;
     const uint32_t sbase = smem_u32(smem);
     const uint64_t kdesc = make_smem_desc_sw128(0, 16, 1024);                  // K-major tile: rows of 128 B
     const uint64_t mdesc = make_smem_desc_sw128(0, 8192, 1024);                // MN-major tile: 8-row atoms along K
     auto kmaj = [&](uint32_t addr, int k4) { return kdesc + (uint64_t)((addr >> 4) & 0x3FFF) + (uint64_t)(k4 * 2); };
     auto mnmaj = [&](uint32_t addr, int k4) { return mdesc + (uint64_t)((addr >> 4) & 0x3FFF) + (uint64_t)(k4 * 128); };
     const uint32_t st0 = sbase + TA_OFF_STAT + wg * TA_TILE_X, st1 = st0 + TA_TILE_S;
-    uint32_t row_salt[2];                             // MODE 0/1: the probability rows are this thread's rows
+    // keep-bit word of this thread inside a 64 x 64 block (MODE 0 / 1: this thread's (query, key) pairs, see pika_b200.h)
+    const int kb_word = (et >> 5) * 32 + (lane & 3) * 8 + (lane >> 2);
+    uint32_t row_salt[2];                             // MODE 0 / 1: the probability rows are this thread's rows
     float lse2[2] = {0.f, 0.f}, dsum_r[2] = {0.f, 0.f};
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         const int srow = srow0 + r0 + 8 * hh;
-        row_salt[hh] = drop_row_salt(stat_row0 + (uint64_t)srow, p.seed);
+        if (MODE == 0 || (MODE == 1 && !KB)) row_salt[hh] = drop_row_salt(stat_row0 + (uint64_t)srow, p.seed);
         if (MODE == 1 && srow < T) {
             lse2[hh] = p.lse[(size_t)bh * p.Tpad + srow] * TA_LOG2E;
             dsum_r[hh] = p.dsum[(size_t)bh * p.Tpad + srow];
@@ -166,41 +185,35 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
     mbar_wait(stat_full, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int j = 0; j < n_tiles; ++j) {
-        const int col0 = j * TA_BC;
-        const int nvalid = min(TA_BC, T - col0);      // streamed indices of this tile inside the sequence
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t x1 = sbase + TA_OFF_RING + stage * 2 * TA_TILE_X, x2 = x1 + TA_TILE_X;
-        float s[32], dp[32];
-        wgmma_fence_acc(s);
-        wgmma_fence();
+    if (MODE == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int j = 0; j < n_tiles; ++j) {
+            const int col0 = j * TA_BC;
+            const int nvalid = min(TA_BC, T - col0);  // streamed indices of this tile inside the sequence
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t x1 = sbase + TA_OFF_RING + stage * 2 * TA_TILE_X, x2 = x1 + TA_TILE_X;
+            float s[32];
+            wgmma_fence_acc(s);
+            wgmma_fence();
 #pragma unroll
-        for (int k4 = 0; k4 < 4; ++k4) wgmma_ss_n64<0, 0>(s, kmaj(st0, k4), kmaj(x1, k4), k4 > 0 ? 1u : 0u);
-        if (MODE != 0) {
-            wgmma_fence_acc(dp);
+            for (int k4 = 0; k4 < 4; ++k4) wgmma_ss_n64<0, 0>(s, kmaj(st0, k4), kmaj(x1, k4), k4 > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(s);
+            if (nvalid < TA_BC) {                     // last tile only (uniform): keys beyond the sequence get probability 0
 #pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) wgmma_ss_n64<0, 0>(dp, kmaj(st1, k4), kmaj(x2, k4), k4 > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_acc(s);
-        if (MODE != 0) wgmma_fence_acc(dp);
-        if (nvalid < TA_BC) {                         // last tile only (uniform): streamed indices beyond the sequence get probability 0
-#pragma unroll
-            for (int c = 0; c < 32; ++c) if ((c >> 2) * 8 + cq + (c & 1) >= nvalid) s[c] = -INFINITY;
-        }
-        if (MODE == 0) {
+                for (int c = 0; c < 32; ++c) if ((c >> 2) * 8 + cq + (c & 1) >= nvalid) s[c] = -INFINITY;
+            }
+            uint32_t kbits = 0u;
+            float corr[2];
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 float mx = -INFINITY;
 #pragma unroll
                 for (int nb = 0; nb < 8; ++nb) mx = fmaxf(mx, fmaxf(s[nb * 4 + 2 * hh], s[nb * 4 + 2 * hh + 1]));
                 const float m_new = fmaxf(m_run[hh], quad_max(mx) * c2);   // finite: every tile holds a valid column
-                const float corr = ex2_approx(m_run[hh] - m_new);            // 0 on the first tile
-#pragma unroll
-                for (int nb = 0; nb < 8; ++nb) { acc0[nb * 4 + 2 * hh] *= corr; acc0[nb * 4 + 2 * hh + 1] *= corr; }
+                corr[hh] = ex2_approx(m_run[hh] - m_new);                    // 0 on the first tile
                 float sum = 0.f;
 #pragma unroll
                 for (int nb = 0; nb < 8; ++nb) {
@@ -212,81 +225,130 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
                         const uint32_t km = drop_pair(row_salt[hh], (uint32_t)((col0 + nb * 8 + cq) >> 1), p.thresh16);
                         if (!(km & 1u)) pr[0] = 0.f;
                         if (!(km & 2u)) pr[1] = 0.f;
+                        kbits |= km << (hh * 16 + nb * 2);
                     }
                 }
-                l_run[hh] = l_run[hh] * corr + sum;   // this thread's columns only; the quad is summed at the end
+                l_run[hh] = l_run[hh] * corr[hh] + sum;   // this thread's columns only; the quad is summed at the end
                 m_run[hh] = m_new;
             }
+            // streaming store: the backward reads the bits long after the rest of the step has cycled L2
+            if (KB) __stcs(p.keep_bits + kb_block(p, bh, 2 * blockIdx.x + wg, j) + kb_word, kbits);
+            // every A fragment is packed before the fence, so ptxas need not fence again between the register-fed wgmma
+            uint32_t a[4][4];
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) frag_a(s, kk, a[kk]);
+#pragma unroll
+            for (int c = 0; c < 32; ++c) acc0[c] *= corr[(c >> 1) & 1];
             wgmma_fence_acc(acc0);
             wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                uint32_t a[4];
-                frag_a(s, kk, a);
-                wgmma_rs_n64<1>(acc0, a, mnmaj(x2, kk), 1u);
-            }
-        } else {
-            float pd[32], ds[32];
-            const float* lse_t = vec + (stage * 2 + 0) * TA_BC;
-            const float* dsum_t = lse_t + TA_BC;
-            uint32_t qsalt[16];
-            if (MODE == 2 && use_drop) {
-                // the probability rows of this tile are the streamed queries (this thread's columns): one salt per query
+            for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<1>(acc0, a[kk], mnmaj(x2, kk), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc0);
+            if (et == 0) mbar_arrive(&empty_bar[stage]);
+            if (++stage == TA_NST) { stage = 0; phase ^= 1; }
+        }
+    } else {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int j = 0; j < n_tiles; ++j) {
+            const int col0 = j * TA_BC;
+            uint32_t kw = 0u;                             // MODE 1: keep bits of this tile, loaded under the wgmma below
+            if (MODE == 1 && KB && use_drop) kw = __ldg(p.keep_bits + kb_block(p, bh, 2 * blockIdx.x + wg, j) + kb_word);
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t x1 = sbase + TA_OFF_RING + stage * 2 * TA_TILE_X, x2 = x1 + TA_TILE_X;
+            float s[32], dp[32];
+            wgmma_fence_acc(s);
+            wgmma_fence();
 #pragma unroll
-                for (int c = 0; c < 16; ++c) qsalt[c] = drop_row_salt(stat_row0 + (uint64_t)(col0 + (c >> 1) * 8 + cq + (c & 1)), p.seed);
-            }
+            for (int k4 = 0; k4 < 4; ++k4) wgmma_ss_n64<0, 0>(s, kmaj(st0, k4), kmaj(x1, k4), k4 > 0 ? 1u : 0u);
+            wgmma_fence_acc(dp);
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
+            for (int k4 = 0; k4 < 4; ++k4) wgmma_ss_n64<0, 0>(dp, kmaj(st1, k4), kmaj(x2, k4), k4 > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(s);
+            wgmma_fence_acc(dp);
+            {
+                float pd[32], ds[32];
+                const float* lse_t = vec + (stage * 2 + 0) * TA_BC;
+                const float* dsum_t = lse_t + TA_BC;
+                // MODE 2: the probability rows of this tile are the streamed queries (this thread's columns), the keys are this thread's
+                // rows.  Query q = nb*8 + cq + e, key w*16 + lane/4 + 8hh of the warpgroup's block sit in word (nb/2)*32 + (lane/8)*8 +
+                // cq + e at bit (nb%2)*16 + 4w + 2hh + (lane/4)%2: four 8-byte loads give the tile's 32 bits
+                uint32_t kq[4][2], qsalt[16];
+                if (MODE == 2 && !KB && use_drop) {
+                    // without bits: one salt per streamed query (the probability rows of this tile)
 #pragma unroll
-                for (int nb = 0; nb < 8; ++nb) {
-                    uint32_t keep = 3u;
-                    if (use_drop) {
-                        if (MODE == 1) {
-                            keep = drop_pair(row_salt[hh], (uint32_t)((col0 + nb * 8 + cq) >> 1), p.thresh16);
-                        } else {
-                            // probability row = streamed query, key = this thread's row
-                            const uint32_t key = (uint32_t)(srow0 + r0 + 8 * hh);
-                            const uint32_t bit = (key & 1u) ? 2u : 1u;
-                            keep = ((drop_pair(qsalt[2 * nb], key >> 1, p.thresh16) & bit) ? 1u : 0u) |
-                                   ((drop_pair(qsalt[2 * nb + 1], key >> 1, p.thresh16) & bit) ? 2u : 0u);
+                    for (int c = 0; c < 16; ++c) qsalt[c] = drop_row_salt(stat_row0 + (uint64_t)(col0 + (c >> 1) * 8 + cq + (c & 1)), p.seed);
+                }
+                if (MODE == 2 && KB && use_drop) {
+                    const uint32_t kb_addr = sbase + TA_OFF_KB + (stage * 2 + wg) * TA_KB_BLOCK + ((lane >> 3) * 8 + cq) * 4;
+                    const int sh = (et >> 5) * 4 + ((lane >> 2) & 1);
+#pragma unroll
+                    for (int m = 0; m < 4; ++m) {
+                        const uint2 v = lds_u32x2(kb_addr + m * 128);
+                        kq[m][0] = v.x >> sh;
+                        kq[m][1] = v.y >> sh;
+                    }
+                }
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                    for (int nb = 0; nb < 8; ++nb) {
+                        uint32_t keep = 3u;
+                        if (use_drop) {
+                            if (MODE == 1) {
+                                keep = KB ? (kw >> (hh * 16 + nb * 2)) & 3u
+                                          : drop_pair(row_salt[hh], (uint32_t)((col0 + nb * 8 + cq) >> 1), p.thresh16);
+                            } else if (KB) {
+                                const int bit = (nb & 1) * 16 + 2 * hh;
+                                keep = ((kq[nb >> 1][0] >> bit) & 1u) | (((kq[nb >> 1][1] >> bit) & 1u) << 1);
+                            } else {
+                                // probability row = streamed query, key = this thread's row
+                                const uint32_t key = (uint32_t)(srow0 + r0 + 8 * hh);
+                                const uint32_t bit = (key & 1u) ? 2u : 1u;
+                                keep = ((drop_pair(qsalt[2 * nb], key >> 1, p.thresh16) & bit) ? 1u : 0u) |
+                                       ((drop_pair(qsalt[2 * nb + 1], key >> 1, p.thresh16) & bit) ? 2u : 0u);
+                            }
+                        }
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int c = nb * 4 + 2 * hh + e;
+                            const int cl = nb * 8 + cq + e;           // streamed index inside the tile
+                            const float l2 = (MODE == 1) ? lse2[hh] : lse_t[cl] * TA_LOG2E;
+                            const float dd = (MODE == 1) ? dsum_r[hh] : dsum_t[cl];
+                            const float pr = ex2_approx(fmaf(s[c], c2, -l2));
+                            const bool kp = (keep >> e) & 1u;
+                            const float dpe = kp ? dp[c] * p.drop_scale : 0.f;
+                            ds[c] = pr * (dpe - dd);
+                            if (MODE == 2) pd[c] = kp ? pr * p.drop_scale : 0.f;
                         }
                     }
+                }
+                uint32_t a[4][4], a2[4][4];                   // packed before the fence, as in the forward
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int c = nb * 4 + 2 * hh + e;
-                        const int cl = nb * 8 + cq + e;           // streamed index inside the tile
-                        const float l2 = (MODE == 1) ? lse2[hh] : lse_t[cl] * TA_LOG2E;
-                        const float dd = (MODE == 1) ? dsum_r[hh] : dsum_t[cl];
-                        const float pr = ex2_approx(fmaf(s[c], c2, -l2));
-                        const bool kp = (keep >> e) & 1u;
-                        const float dpe = kp ? dp[c] * p.drop_scale : 0.f;
-                        ds[c] = pr * (dpe - dd);
-                        if (MODE == 2) pd[c] = kp ? pr * p.drop_scale : 0.f;
-                    }
+                for (int kk = 0; kk < 4; ++kk) {
+                    frag_a(ds, kk, a[kk]);
+                    if (MODE == 2) frag_a(pd, kk, a2[kk]);
+                }
+                wgmma_fence_acc(acc0);
+                if (MODE == 2) wgmma_fence_acc(acc1);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    wgmma_rs_n64<1>(acc0, a[kk], mnmaj(x1, kk), 1u);                    // MODE 1: dQ += dS K;  MODE 2: dK += dS^T Q
+                    if (MODE == 2) wgmma_rs_n64<1>(acc1, a2[kk], mnmaj(x2, kk), 1u);    // dV += Pd^T dO
                 }
             }
+            wgmma_commit();
+            wgmma_wait<0>();
             wgmma_fence_acc(acc0);
             if (MODE == 2) wgmma_fence_acc(acc1);
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                uint32_t a[4];
-                frag_a(ds, kk, a);
-                if (MODE == 1) wgmma_rs_n64<1>(acc0, a, mnmaj(x1, kk), 1u);        // dQ += dS K
-                else wgmma_rs_n64<1>(acc0, a, mnmaj(x1, kk), 1u);                   // dK += dS^T Q
-                if (MODE == 2) {
-                    uint32_t a2[4];
-                    frag_a(pd, kk, a2);
-                    wgmma_rs_n64<1>(acc1, a2, mnmaj(x2, kk), 1u);                   // dV += Pd^T dO
-                }
-            }
+            if (et == 0) mbar_arrive(&empty_bar[stage]);
+            if (++stage == TA_NST) { stage = 0; phase ^= 1; }
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_acc(acc0);
-        if (MODE == 2) wgmma_fence_acc(acc1);
-        if (et == 0) mbar_arrive(&empty_bar[stage]);
-        if (++stage == TA_NST) { stage = 0; phase ^= 1; }
     }
 
     // ---- epilogue
@@ -349,8 +411,8 @@ static int attn_maps(AttnTcParams& p, const void* q, const void* k, const void* 
     return 0;
 }
 
-template <int MODE> static int launch_attn(const AttnTcParams& p, cudaStream_t st) {
-    auto kern = attention_tc_kernel<MODE>;
+template <int MODE, int DROP> static int launch_attn_drop(const AttnTcParams& p, cudaStream_t st) {
+    auto kern = attention_tc_kernel<MODE, DROP>;
     static bool configured = false;
     if (!configured) {
         PK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TA_SMEM));
@@ -361,12 +423,21 @@ template <int MODE> static int launch_attn(const AttnTcParams& p, cudaStream_t s
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }
+template <int MODE> static int launch_attn(const AttnTcParams& p, cudaStream_t st) {
+    if (p.thresh16 == 0u) return launch_attn_drop<MODE, TA_DROP_NONE>(p, st);
+    return p.keep_bits ? launch_attn_drop<MODE, TA_DROP_BITS>(p, st) : launch_attn_drop<MODE, TA_DROP_HASH>(p, st);
+}
 
 }  // namespace pk
 
 #define STREAM(s) reinterpret_cast<cudaStream_t>(s)
 
 extern "C" int pk_attention_lse_stride(int T) { return (T + 63) / 64 * 64; }
+static int attn_kb_blocks(int T) { return (T + 127) / 128 * 2; }
+extern "C" long long pk_attention_keep_bits_bytes(int B, int T, int heads) {
+    const long long n = attn_kb_blocks(T);
+    return (long long)B * heads * n * n * pk::TA_KB_BLOCK;
+}
 
 #define ATTN_CHECKS()                                                                                                      \
     PK_CHECK_ARG(B > 0 && T > 0 && heads > 0, "bad dims");                                                                 \
@@ -374,14 +445,18 @@ extern "C" int pk_attention_lse_stride(int T) { return (T + 63) / 64 * 64; }
     PK_CHECK_ARG(ld_qkv % 8 == 0 && ld_out % 8 == 0, "row strides must be multiples of 8 elements (16 bytes)");            \
     PK_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f, "drop_p out of range");                                                    \
     PK_CHECK_ARG((long long)B * heads < 65536, "B * heads must be < 65536")
+#define KEEP_BITS_CHECK()                                                                                                  \
+    PK_CHECK_ARG(drop_p == 0.f || (keep_bits != nullptr && ((uintptr_t)keep_bits & 15) == 0),                               \
+                 "keep_bits must be a 16-byte aligned buffer of pk_attention_keep_bits_bytes when drop_p > 0")
 
-extern "C" int pk_attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
-                                int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream) {
+static int attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                         int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits, void* stream) {
     using namespace pk;
     ATTN_CHECKS();
     static thread_local AttnTcParams p;
     memset(&p, 0, sizeof(p));
     p.B = B; p.T = T; p.heads = heads; p.Tpad = pk_attention_lse_stride(T); p.Tp2 = (T + 1) / 2;
+    p.keep_bits = drop_p > 0.f ? keep_bits : nullptr; p.nkb = attn_kb_blocks(T);
     int rc = attn_maps(p, q, k, v, ld_qkv, nullptr, 0);
     if (rc) return rc;
     p.out = (__nv_bfloat16*)out; p.ld_o = ld_out; p.lse = lse;
@@ -391,16 +466,19 @@ extern "C" int pk_attention_fwd(const void* q, const void* k, const void* v, lon
 }
 
 /* dq/dk/dv share the row stride ld_dqkv (the fused [B,T,3D] gradient buffer); lse and dsum_ws: [B*heads][pk_attention_lse_stride(T)],
-   whose padding t in [T, stride) the kernels write themselves (lse in the forward, dsum_ws here): neither needs initialising */
-extern "C" int pk_attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
-                                const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
-                                long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream) {
+   whose padding t in [T, stride) the kernels write themselves (lse in the forward, dsum_ws here): neither needs initialising.
+   keep_bits NULL: the kernels hash the mask from seed */
+static int attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                         const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                         long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed,
+                         const uint32_t* keep_bits, void* stream) {
     using namespace pk;
     ATTN_CHECKS();
     PK_CHECK_ARG(ld_dout % 8 == 0 && ld_dqkv % 8 == 0, "row strides must be multiples of 8 elements (16 bytes)");
     static thread_local AttnTcParams p;
     memset(&p, 0, sizeof(p));
     p.B = B; p.T = T; p.heads = heads; p.Tpad = pk_attention_lse_stride(T); p.Tp2 = (T + 1) / 2;
+    p.keep_bits = drop_p > 0.f ? const_cast<uint32_t*>(keep_bits) : nullptr; p.nkb = attn_kb_blocks(T);
     int rc = attn_maps(p, q, k, v, ld_qkv, dout, ld_dout);
     if (rc) return rc;
     p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv; p.ld_dqkv = ld_dqkv;
@@ -416,4 +494,29 @@ extern "C" int pk_attention_bwd(const void* q, const void* k, const void* v, lon
     rc = launch_attn<1>(p, STREAM(stream));
     if (rc) return rc;
     return launch_attn<2>(p, STREAM(stream));
+}
+
+extern "C" int pk_attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                                int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream) {
+    return attention_fwd(q, k, v, ld_qkv, out, ld_out, lse, B, T, heads, dh, alpha, drop_p, seed, nullptr, stream);
+}
+extern "C" int pk_attention_fwd_bits(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                                     int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits,
+                                     void* stream) {
+    KEEP_BITS_CHECK();
+    return attention_fwd(q, k, v, ld_qkv, out, ld_out, lse, B, T, heads, dh, alpha, drop_p, seed, keep_bits, stream);
+}
+extern "C" int pk_attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                                const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                                long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, void* stream) {
+    return attention_bwd(q, k, v, ld_qkv, out, ld_out, dout, ld_dout, lse, dsum_ws, dq, dk, dv, ld_dqkv, B, T, heads, dh, alpha, drop_p, seed,
+                         nullptr, stream);
+}
+extern "C" int pk_attention_bwd_bits(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                                     const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                                     long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
+                                     void* stream) {
+    KEEP_BITS_CHECK();
+    return attention_bwd(q, k, v, ld_qkv, out, ld_out, dout, ld_dout, lse, dsum_ws, dq, dk, dv, ld_dqkv, B, T, heads, dh, alpha, drop_p, 0u,
+                         keep_bits, stream);
 }

@@ -346,6 +346,11 @@ PK_DEVICE uint4 lds_u32x4(uint32_t addr) {
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
     return v;
 }
+PK_DEVICE uint2 lds_u32x2(uint32_t addr) {
+    uint2 v;
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr) : "memory");
+    return v;
+}
 PK_DEVICE float2 lds_f32x2(uint32_t addr) {
     float2 v;
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");

@@ -457,8 +457,9 @@ class AttentionFn(torch.autograd.Function):
             out = _new((B, T, D), like=qkv)
             lse = torch.zeros(B * heads * K.attention_lse_stride(T), dtype=torch.float32, device=qkv.device)   # pad entries finite
             alpha = 1.0 / math.sqrt(dh)
-            K.attention_fwd(qkv, out, lse, heads, alpha, drop_p, seed)
-            ctx.save_for_backward(qkv, out, lse)
+            keep_bits = K.attention_keep_bits(B, T, heads, drop_p, qkv.device)   # dropout decisions, for the backward
+            K.attention_fwd(qkv, out, lse, heads, alpha, drop_p, seed, keep_bits=keep_bits)
+            ctx.save_for_backward(qkv, out, lse, keep_bits)
             ctx.meta = (B, T, D, heads, dh, 0, drop_p, seed, alpha)
             return out
         Tp = (T + 7) // 8 * 8
@@ -507,10 +508,10 @@ class AttentionFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         if ctx.fused:
-            qkv, out, lse = ctx.saved_tensors
+            qkv, out, lse, keep_bits = ctx.saved_tensors
             B, T, D, heads, dh, _, drop_p, seed, alpha = ctx.meta
             dqkv = torch.empty_like(qkv)
-            K.attention_bwd(qkv, out, dout.contiguous(), lse, dqkv, heads, alpha, drop_p, seed)
+            K.attention_bwd(qkv, out, dout.contiguous(), lse, dqkv, heads, alpha, drop_p, seed, keep_bits=keep_bits)
             return dqkv, None, None, None, None, None, None
         qkv, P = ctx.saved_tensors
         B, T, D, heads, dh, Tp, drop_p, seed, alpha = ctx.meta

@@ -154,28 +154,45 @@ def attention_lse_stride(T):
     return int(lib.pk_attention_lse_stride(T))
 
 
-def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0):
-    """qkv [B,T,3D] bf16 (q | k | v column blocks) -> out [B,T,D], lse [B*heads*T] f32 (fused attention, head dim 64)"""
+def attention_keep_bits(B, T, heads, drop_p, device):
+    """the dropout keep-bit buffer attention_fwd fills and attention_bwd reads (None when drop_p == 0: nothing is dropped)"""
+    if drop_p <= 0:
+        return None
+    return torch.empty(int(lib.pk_attention_keep_bits_bytes(B, T, heads)) // 4, dtype=torch.int32, device=device)
+
+
+def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0, keep_bits=None):
+    """qkv [B,T,3D] bf16 (q | k | v column blocks) -> out [B,T,D], lse [B*heads*T] f32 (fused attention, head dim 64).
+    keep_bits (attention_keep_bits): also write the dropout decisions there, for attention_bwd to read."""
     B, T, D3 = qkv.shape
     D = D3 // 3
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and out.is_contiguous() and out.shape == (B, T, D)
     assert lse.dtype == torch.float32 and lse.numel() == B * heads * attention_lse_stride(T)
     base, es = qkv.data_ptr(), 2
     vp = ctypes.c_void_p
-    check(lib.pk_attention_fwd(vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(lse), _I(B), _I(T),
-                               _I(heads), _I(D // heads), _F(alpha), _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_attention_fwd")
+    args = (vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(lse), _I(B), _I(T), _I(heads), _I(D // heads),
+            _F(alpha), _F(drop_p), _U(seed & 0xFFFFFFFF))
+    if keep_bits is None:
+        check(lib.pk_attention_fwd(*args, _stream()), "pk_attention_fwd")
+        return
+    assert keep_bits.is_contiguous() and keep_bits.numel() * keep_bits.element_size() >= lib.pk_attention_keep_bits_bytes(B, T, heads)
+    check(lib.pk_attention_fwd_bits(*args, _P(keep_bits), _stream()), "pk_attention_fwd_bits")
 
 
-def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0):
+def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0, keep_bits=None):
+    """dqkv <- gradient of attention_fwd; with keep_bits (the forward's) the mask is read from them, otherwise drawn from seed"""
     B, T, D3 = qkv.shape
     D = D3 // 3
     assert dout.is_contiguous() and dqkv.is_contiguous() and dqkv.shape == qkv.shape and dout.dtype == torch.bfloat16
     ws = torch.zeros(B * heads * attention_lse_stride(T), dtype=torch.float32, device=qkv.device)     # D scratch (the kernel writes its padding too)
     base, gb, es = qkv.data_ptr(), dqkv.data_ptr(), 2
     vp = ctypes.c_void_p
-    check(lib.pk_attention_bwd(vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(dout), _L(D), _P(lse), _P(ws),
-                               vp(gb), vp(gb + D * es), vp(gb + 2 * D * es), _L(D3), _I(B), _I(T), _I(heads), _I(D // heads), _F(alpha),
-                               _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_attention_bwd")
+    args = (vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(dout), _L(D), _P(lse), _P(ws),
+            vp(gb), vp(gb + D * es), vp(gb + 2 * D * es), _L(D3), _I(B), _I(T), _I(heads), _I(D // heads), _F(alpha), _F(drop_p))
+    if keep_bits is None:
+        check(lib.pk_attention_bwd(*args, _U(seed & 0xFFFFFFFF), _stream()), "pk_attention_bwd")
+    else:
+        check(lib.pk_attention_bwd_bits(*args, _P(keep_bits), _stream()), "pk_attention_bwd_bits")
 
 
 _col_ws = {}

@@ -1,29 +1,105 @@
-"""fused vs materialised attention at the bench shape (B=32, heads=16, T=994): fwd+bwd ms"""
-import sys, os
+"""Fused encoder self-attention at the bench shape (B=32, heads=16, head dim 64): forward, dQ and dK/dV timed separately.
+
+    python scripts/attn_bench.py [--T 994] [--p 0,0.2] [--iters 20] [--dump DIR]
+
+Each line is one JSON object: forward and backward milliseconds from CUDA events around engine.AttentionFn (allocations
+included, as in the train step), then the per-kernel split of one more run of the same calls under torch.profiler.  The
+achieved rate counts 9 T^2 * 64 multiply-adds per (batch, head) (2 forward, 3 dQ, 4 dK/dV).  --dump writes O, lse and
+dQ|dK|dV of the seeded inputs to DIR (one .pt per p), so that two builds can be compared element by element."""
+import argparse
+import collections
+import inspect
+import json
+import os
+import re
+import sys
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch
-from pika_b200 import engine as E
-E.set_precision("bf16")
-B, T, heads = int(os.environ.get("B", 32)), int(os.environ.get("T", 994)), 16
-D = heads * 64
-g = torch.Generator(device="cuda").manual_seed(1)
-qkv0 = (torch.randn(B, T, 3 * D, generator=g, device="cuda") * 0.5).bfloat16()
-dy = torch.randn(B, T, D, generator=g, device="cuda").bfloat16()
-def run(fused, p):
-    E._FUSED_ATTN = fused
-    qkv = qkv0.clone().requires_grad_(True)
-    out = E.AttentionFn.apply(qkv, heads, p, 99)
-    out.backward(dy)
-    return out, qkv.grad
-for p in (0.0, 0.1):
-    for fused in (False, True):
-        for _ in range(2): run(fused, p)
+import torch  # noqa: E402
+
+from pika_b200 import engine as E  # noqa: E402
+from pika_b200 import kernels as K  # noqa: E402
+
+
+def inputs(B, T, heads):
+    D = heads * 64
+    g = torch.Generator(device="cuda").manual_seed(1)
+    qkv = (torch.randn(B, T, 3 * D, generator=g, device="cuda") * 0.5).bfloat16()
+    dy = torch.randn(B, T, D, generator=g, device="cuda").bfloat16()
+    return qkv, dy
+
+
+def outputs(qkv, dy, heads, p, seed):
+    """O, lse and dQ|dK|dV through kernels.attention_fwd / _bwd (whichever keep-bits interface this build has)"""
+    B, T, D3 = qkv.shape
+    out = torch.empty(B, T, D3 // 3, dtype=torch.bfloat16, device="cuda")
+    lse = torch.zeros(B * heads * K.attention_lse_stride(T), device="cuda")
+    alpha = 0.125
+    dqkv = torch.empty_like(qkv)
+    if "keep_bits" in inspect.signature(K.attention_bwd).parameters:
+        bits = K.attention_keep_bits(B, T, heads, p, qkv.device)
+        K.attention_fwd(qkv, out, lse, heads, alpha, p, seed, keep_bits=bits)
+        K.attention_bwd(qkv, out, dy, lse, dqkv, heads, alpha, p, seed, keep_bits=bits)
+    else:
+        K.attention_fwd(qkv, out, lse, heads, alpha, p, seed)
+        K.attention_bwd(qkv, out, dy, lse, dqkv, heads, alpha, p, seed)
+    torch.cuda.synchronize()
+    return dict(out=out, lse=lse, dqkv=dqkv)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--B", type=int, default=32)
+    ap.add_argument("--T", type=int, default=994)
+    ap.add_argument("--heads", type=int, default=16)
+    ap.add_argument("--p", default="0,0.2")
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--tag", default="")
+    ap.add_argument("--dump", default=None)
+    a = ap.parse_args()
+    E.set_precision("bf16")
+    B, T, heads = a.B, a.T, a.heads
+    qkv0, dy = inputs(B, T, heads)
+    tflop = 9 * 2 * B * heads * T * T * 64 / 1e12
+    seed = 99
+    for p in (float(x) for x in a.p.split(",")):
+        qkv = qkv0.clone().requires_grad_(True)
+
+        def fwd():
+            return E.AttentionFn.apply(qkv, heads, p, seed)
+
+        for _ in range(3):
+            fwd().backward(dy)
         torch.cuda.synchronize()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        for _ in range(5): run(fused, p)
-        e.record(); torch.cuda.synchronize()
-        print("drop %.1f fused=%d  %.3f ms fwd+bwd" % (p, fused, s.elapsed_time(e) / 5), flush=True)
-    a, b = run(True, p), run(False, p)
-    r = lambda x, y: ((x.float() - y.float()).norm() / y.float().norm()).item()
-    print("  rel out %.2e  rel grad %.2e" % (r(a[0], b[0]), r(a[1], b[1])), flush=True)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3 * a.iters)]
+        for i in range(a.iters):
+            ev[3 * i].record()
+            out = fwd()
+            ev[3 * i + 1].record()
+            out.backward(dy)
+            ev[3 * i + 2].record()
+        torch.cuda.synchronize()
+        f = sorted(ev[3 * i].elapsed_time(ev[3 * i + 1]) for i in range(a.iters))
+        b = sorted(ev[3 * i + 1].elapsed_time(ev[3 * i + 2]) for i in range(a.iters))
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                fwd().backward(dy)
+            torch.cuda.synchronize()
+        kern = collections.defaultdict(float)
+        for e in prof.events():
+            if e.device_type == torch.autograd.DeviceType.CUDA and "attention" in e.name:
+                name = re.sub(r"\(.*", "", e.name).replace("void ", "").replace("pk::", "")
+                kern[name] += e.device_time_total / 5 / 1000.0
+        fm, bm = f[len(f) // 2], b[len(b) // 2]
+        print(json.dumps(dict(tag=a.tag, B=B, T=T, heads=heads, p=p, fwd_ms=round(fm, 4), bwd_ms=round(bm, 4),
+                              total_ms=round(fm + bm, 4), tflops=round(tflop / (fm + bm) * 1e3, 1),
+                              kernels_ms={k: round(v, 4) for k, v in sorted(kern.items())})), flush=True)
+        if a.dump:
+            os.makedirs(a.dump, exist_ok=True)
+            torch.save({k: v.cpu() for k, v in outputs(qkv0, dy, heads, p, seed).items()},
+                       os.path.join(a.dump, "attn_T%d_p%g.pt" % (T, p)))
+
+
+if __name__ == "__main__":
+    main()
