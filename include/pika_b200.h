@@ -285,6 +285,37 @@ int pk_fbank(const float* wave, long long ld_wave, const int* n_frames, int B, i
              const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, float preemph, float* feats,
              float dither, unsigned int dither_seed, void* stream);
 
+/* Front end with on-the-fly noise and reverberation (loader/audio.py:426-513 AudioSegment.add_noise / convolve_and_normalize,
+ * loader/otf_utt_loader.py:224-228), per utterance: speed -> normalize(target_db) -> add_noise -> convolve_and_normalize -> int16
+ * -> fbank ...  Arguments up to `stream` are those of pk_frontend_fwd; then
+ *   noise        int16 bank of concatenated noise segments (device), or null for no noise
+ *   noise_idx    [B] int32 segment of each utterance; noise_off [B] int64 ABSOLUTE bank offset of the utterance's first noise
+ *                sample (segment start + drawn offset; new_len[b] samples are read); snr [B] f64 dB
+ *   noise_rms_db [n_noise] f64: rms_db of each whole segment (float32 samples, as AudioSegment.rms_db)
+ *   rir          int16 bank of concatenated RIRs (device), or null for no reverberation
+ *   rir_off      [n_rir] int64 start, rir_len [n_rir] int32 length (>= 1), rir_idx [B] int32 RIR of each utterance
+ *   rir_max_len  host-side bound >= every rir_len[rir_idx[b]], in [1, 65536] (pass 1 without RIRs); sets the FFT block length
+ * The convolution is fftconvolve(x, h, "same") in float64 (uniformly partitioned overlap-save); on the rate == 1.0 branch the
+ * result is rounded to float32, like the reference's float32 samples.  err_flag also reports a renormalisation gain above 300 dB.
+ * Workspace: pk_frontend_noise_rir_workspace_bytes (< 0 when rir_max_len is outside [1, 65536]; no device access). */
+long long pk_frontend_noise_rir_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D, int rir_max_len);
+int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                              const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
+                              int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
+                              const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
+                              int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                              long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
+                              const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,
+                              const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
+                              const int* rir_idx, int rir_max_len);
+
+/* scipy.signal.fftconvolve(x, h, "same") in float64 for ragged batches: x [B, ld_x] (lengths n_len), h [B, ld_h] (lengths
+ * m_len, 1 <= m_len <= m_max <= 65536) -> y [B, ld_y], n_len[b] samples each (y may alias x).  Workspace:
+ * pk_conv_same_f64_workspace_bytes (< 0 on bad dims). */
+long long pk_conv_same_f64_workspace_bytes(int B, int n_max, int m_max);
+int pk_conv_same_f64(const double* x, long long ld_x, const int* n_len, const double* h, long long ld_h, const int* m_len, int B,
+                     int n_max, int m_max, double* y, long long ld_y, void* workspace, long long workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Batched beam search (pika_b200/csrc/beam.cu): one launch per step for the whole batch.
  * Replaces decoder/beam_transducer.py:82-187 (BeamMergeTransducer.advance) and the gather / masked LSTM

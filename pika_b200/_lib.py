@@ -80,6 +80,9 @@ _sig("pk_attention_keep_bits_bytes", [_i, _i, _i], ctypes.c_longlong)
 _sig("pk_rnnt_loss_colsum_workspace_bytes", [_i, _i, _i, _i], ctypes.c_longlong)
 _sig("pk_rnnt_loss_fwd_bwd", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp])
 _sig("pk_rnnt_loss_fwd_bwd_lse", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _i, _vp])
+_sig("pk_frontend_noise_rir_workspace_bytes", [_i, _i, _i, _i, _i, _i], ctypes.c_longlong)
+_sig("pk_conv_same_f64_workspace_bytes", [_i, _i, _i], ctypes.c_longlong)
+_sig("pk_conv_same_f64", [_vp, _ll, _vp, _vp, _ll, _vp, _i, _i, _i, _vp, _ll, _vp, _ll, _vp])
 
 
 def check(rc, what=""):

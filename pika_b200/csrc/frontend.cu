@@ -67,6 +67,33 @@ __global__ void __launch_bounds__(AUG_THREADS) aug_resample_kernel(const short* 
     if (threadIdx.x == 0) partial[(long long)b * parts + blockIdx.x] = red[0];
 }
 
+// AudioSegment.normalize(target_db) gain from the per-CTA partial sums of squares (fixed summation order)
+PK_DEVICE double normalize_gain(const double* __restrict__ partial, int parts, int L, bool unit, double target_db, int* err_flag) {
+    double tot = 0.0;
+    for (int i = 0; i < parts; ++i) tot += partial[i];
+    double ms = (L > 0) ? tot / (double)L : 0.0;
+    if (unit) ms = (double)(float)ms;                                    // numpy float32 mean
+    ms = fmax(1e-20, ms);
+    const double rms_db = 10.0 * log10(ms);
+    double gain_db = target_db - rms_db;
+    if (gain_db > 300.0) { atomicExch(err_flag, 1); gain_db = 300.0; }  // reference raises ValueError
+    return pow(10.0, gain_db / 20.0);
+}
+
+// _convert_samples_from_float32(.., 'int16'): scale by 2^15, clip, C-cast truncation toward zero
+PK_DEVICE int quantise(double s, double gain, bool unit) {
+    if (unit) {
+        float v = __fmul_rn((float)s, (float)gain);
+        v = __fmul_rn(v, 32768.0f);
+        v = fminf(fmaxf(v, -32768.0f), 32767.0f);
+        return (int)v;
+    }
+    double v = __dmul_rn(s, gain);
+    v = __dmul_rn(v, 32768.0);
+    v = fmin(fmax(v, -32768.0), 32767.0);
+    return (int)v;
+}
+
 // pass B: gain from the mean square, apply, quantise to int16 (stored as float for the fbank kernel)
 __global__ void __launch_bounds__(AUG_THREADS) aug_gain_kernel(const double* __restrict__ resampled, long long ld_res,
                                                                const double* __restrict__ partial, int parts,
@@ -75,40 +102,291 @@ __global__ void __launch_bounds__(AUG_THREADS) aug_gain_kernel(const double* __r
                                                                short* __restrict__ wave_i16, long long ld_wave, int* __restrict__ err_flag) {
     const int b = blockIdx.y;
     const int L = new_len[b];
-    __shared__ double s_gain;
-    if (threadIdx.x == 0) {
-        double tot = 0.0;
-        for (int i = 0; i < parts; ++i) tot += partial[(long long)b * parts + i];
-        double ms = (L > 0) ? tot / (double)L : 0.0;
-        const bool unit = (rate[b] == 1.0f);
-        if (unit) ms = (double)(float)ms;                                // numpy float32 mean
-        ms = fmax(1e-20, ms);
-        const double rms_db = 10.0 * log10(ms);
-        double gain_db = (double)target_db[b] - rms_db;
-        if (gain_db > 300.0) { atomicExch(err_flag, 1); gain_db = 300.0; }  // reference raises ValueError
-        s_gain = pow(10.0, gain_db / 20.0);
-    }
-    __syncthreads();
     const bool unit = (rate[b] == 1.0f);
+    __shared__ double s_gain;
+    if (threadIdx.x == 0) s_gain = normalize_gain(partial + (long long)b * parts, parts, L, unit, (double)target_db[b], err_flag);
+    __syncthreads();
     const double gain = s_gain;
-    const float gain32 = (float)gain;
     const double* src = resampled + (long long)b * ld_res;
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < L; j += gridDim.x * blockDim.x) {
-        int q;
-        if (unit) {
-            float v = __fmul_rn((float)src[j], gain32);
-            v = __fmul_rn(v, 32768.0f);
-            v = fminf(fmaxf(v, -32768.0f), 32767.0f);
-            q = (int)v;                                                  // C cast: truncation toward zero
-        } else {
-            double v = __dmul_rn(src[j], gain);
-            v = __dmul_rn(v, 32768.0);
-            v = fmin(fmax(v, -32768.0), 32767.0);
-            q = (int)v;
-        }
+        const int q = quantise(src[j], gain, unit);
         wave[(long long)b * ld_wave + j] = (float)q;
         if (wave_i16) wave_i16[(long long)b * ld_wave + j] = (short)q;
     }
+}
+
+// ------------------------------------------------------------------------------------ noise + reverberation
+//   loader/audio.py:426-513  AudioSegment.{add_noise, convolve_and_normalize}; call sites loader/otf_utt_loader.py:224-228
+// On these paths the gained signal stays in the float64 workspace (float32-valued on the rate == 1.0 branch, where the
+// reference's samples are float32) until the final renormalise + quantise pass.
+
+// fixed-tree CTA reduction; thread 0 writes the CTA's partial
+template <int THREADS>
+PK_DEVICE void cta_partial(double acc, double* __restrict__ out) {
+    __shared__ double red[THREADS];
+    red[threadIdx.x] = acc;
+    __syncthreads();
+    for (int s = THREADS / 2; s > 0; s >>= 1) {
+        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *out = red[0];
+}
+
+// rms_db of a signal from its partial sums of squares; float32 arithmetic on the rate == 1.0 branch like numpy's
+PK_DEVICE double rms_db_of(const double* __restrict__ partial, int parts, int L, bool unit) {
+    double tot = 0.0;
+    for (int i = 0; i < parts; ++i) tot += partial[i];
+    double ms = (L > 0) ? tot / (double)L : 0.0;
+    if (unit) ms = (double)(float)ms;
+    ms = fmax(1e-20, ms);
+    const double db = 10.0 * log10(ms);
+    return unit ? (double)(float)db : db;
+}
+
+// pass B': the gain of pass B, applied in place and kept in float; partial sums of squares of the gained signal
+__global__ void __launch_bounds__(AUG_THREADS) aug_gain_keep_kernel(double* __restrict__ sig, long long ld_sig,
+                                                                    const double* __restrict__ partial, int parts,
+                                                                    const float* __restrict__ rate, const int* __restrict__ new_len,
+                                                                    const float* __restrict__ target_db, double* __restrict__ partial_out,
+                                                                    int* __restrict__ err_flag) {
+    const int b = blockIdx.y;
+    const int L = new_len[b];
+    const bool unit = (rate[b] == 1.0f);
+    __shared__ double s_gain;
+    if (threadIdx.x == 0) s_gain = normalize_gain(partial + (long long)b * parts, parts, L, unit, (double)target_db[b], err_flag);
+    __syncthreads();
+    const double gain = s_gain;
+    double* x = sig + (long long)b * ld_sig;
+    double acc = 0.0;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < L; j += gridDim.x * blockDim.x) {
+        if (unit) {
+            const float v = __fmul_rn((float)x[j], (float)gain);
+            x[j] = (double)v;
+            acc += (double)__fmul_rn(v, v);
+        } else {
+            const double v = __dmul_rn(x[j], gain);
+            x[j] = v;
+            acc += __dmul_rn(v, v);
+        }
+    }
+    cta_partial<AUG_THREADS>(acc, partial_out + (long long)b * gridDim.x + blockIdx.x);
+}
+
+// add_noise: noise gain min(rms_db - noise_rms_db - snr, 300) dB on the float32 noise slice (float64 multiply, float32
+// result, as numpy's in-place float32 *= float64), superimposed; partial sums of squares of the noisy signal
+__global__ void __launch_bounds__(AUG_THREADS) aug_noise_kernel(double* __restrict__ sig, long long ld_sig, const double* __restrict__ partial,
+                                                                int parts, const float* __restrict__ rate, const int* __restrict__ new_len,
+                                                                const short* __restrict__ noise, const int* __restrict__ noise_idx,
+                                                                const long long* __restrict__ noise_off, const double* __restrict__ snr,
+                                                                const double* __restrict__ noise_rms_db, double* __restrict__ partial_out) {
+    const int b = blockIdx.y;
+    const int L = new_len[b];
+    const bool unit = (rate[b] == 1.0f);
+    __shared__ double s_gain;
+    if (threadIdx.x == 0) {
+        const double sig_db = rms_db_of(partial + (long long)b * parts, parts, L, unit);
+        const double nz_db = noise_rms_db[noise_idx[b]];
+        const double diff = unit ? (double)__fsub_rn((float)sig_db, (float)nz_db) : sig_db - nz_db;
+        s_gain = pow(10.0, fmin(diff - snr[b], 300.0) / 20.0);
+    }
+    __syncthreads();
+    const double gain = s_gain;
+    double* x = sig + (long long)b * ld_sig;
+    const short* nz = noise + noise_off[b];
+    double acc = 0.0;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < L; j += gridDim.x * blockDim.x) {
+        const float n = (float)__dmul_rn((double)((float)nz[j] * (1.0f / 32768.0f)), gain);
+        if (unit) {
+            const float v = __fadd_rn((float)x[j], n);
+            x[j] = (double)v;
+            acc += (double)__fmul_rn(v, v);
+        } else {
+            const double v = __dadd_rn(x[j], (double)n);
+            x[j] = v;
+            acc += __dmul_rn(v, v);
+        }
+    }
+    cta_partial<AUG_THREADS>(acc, partial_out + (long long)b * gridDim.x + blockIdx.x);
+}
+
+// renormalise to the pre-convolution rms_db (convolve_and_normalize) when post != nullptr, then quantise as pass B
+__global__ void __launch_bounds__(AUG_THREADS) aug_renorm_quant_kernel(const double* __restrict__ sig, long long ld_sig,
+                                                                       const double* __restrict__ pre, int pre_parts,
+                                                                       const double* __restrict__ post, int post_parts,
+                                                                       const float* __restrict__ rate, const int* __restrict__ new_len,
+                                                                       float* __restrict__ wave, short* __restrict__ wave_i16,
+                                                                       long long ld_wave, int* __restrict__ err_flag) {
+    const int b = blockIdx.y;
+    const int L = new_len[b];
+    const bool unit = (rate[b] == 1.0f);
+    __shared__ double s_gain;
+    if (threadIdx.x == 0) {
+        double gain = 1.0;
+        if (post) {
+            const double t_db = rms_db_of(pre + (long long)b * pre_parts, pre_parts, L, unit);
+            const double c_db = rms_db_of(post + (long long)b * post_parts, post_parts, L, unit);
+            double gain_db = unit ? (double)__fsub_rn((float)t_db, (float)c_db) : t_db - c_db;
+            if (gain_db > 300.0) { atomicExch(err_flag, 1); gain_db = 300.0; }
+            gain = pow(10.0, gain_db / 20.0);
+        }
+        s_gain = gain;
+    }
+    __syncthreads();
+    const double gain = s_gain;
+    const double* src = sig + (long long)b * ld_sig;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < L; j += gridDim.x * blockDim.x) {
+        const int q = quantise(src[j], gain, unit);
+        wave[(long long)b * ld_wave + j] = (float)q;
+        if (wave_i16) wave_i16[(long long)b * ld_wave + j] = (short)q;
+    }
+}
+
+// ---- fftconvolve(x, h, "same") in float64: uniformly partitioned overlap-save, FFT size 2*Lb.
+// y[n] = sum_m h[m] x[n + c - m], c = (M-1)//2, n in [0, N).  With x'[i] = x[i + c] and h_p = h[p*Lb, (p+1)*Lb):
+// output block j (Lb samples) = last Lb samples of IFFT(sum_p H_p . X_{j-p}), X_q = FFT of x'[(q-1)*Lb, (q+1)*Lb).
+// Real inputs: only bins 0..Lb of each spectrum are stored; the inverse restores the rest by Hermitian symmetry.
+constexpr int CONV_THREADS = 512;
+
+struct RirF64 {             // ragged float64 RIRs, one per signal
+    const double* h; long long ld; const int* len;
+    PK_DEVICE int length(int b) const { return len[b]; }
+    PK_DEVICE double at(int b, int i) const { return h[(long long)b * ld + i]; }
+};
+struct RirBank {            // int16 bank; signal b uses RIR idx[b] (float32 samples, x 2^-15)
+    const short* bank; const long long* off; const int* len; const int* idx;
+    PK_DEVICE int length(int b) const { return len[idx[b]]; }
+    PK_DEVICE double at(int b, int i) const { return (double)((float)bank[off[idx[b]] + i] * (1.0f / 32768.0f)); }
+};
+
+struct ConvGeom {
+    int lb, log2n, p_max, j_max, q_max;     // q index = q + p_max - 1, in [0, q_max)
+};
+
+PK_DEVICE double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+
+// in-place radix-2 DIT on bit-reversed input in shared memory; tw[k] = exp(-2 pi i k / n), k < n/2
+template <bool INV>
+PK_DEVICE void fft_smem(double2* buf, int log2n, const double2* __restrict__ tw) {
+    const int half_n = 1 << (log2n - 1);
+    for (int s = 1; s <= log2n; ++s) {
+        const int half = 1 << (s - 1);
+        for (int t = threadIdx.x; t < half_n; t += blockDim.x) {
+            const int pos = t & (half - 1);
+            const int i0 = ((t >> (s - 1)) << s) + pos, i1 = i0 + half;
+            double2 w = tw[pos << (log2n - s)];
+            if (INV) w.y = -w.y;
+            const double2 a = buf[i0], c = cmul(buf[i1], w);
+            buf[i0] = make_double2(a.x + c.x, a.y + c.y);
+            buf[i1] = make_double2(a.x - c.x, a.y - c.y);
+        }
+        __syncthreads();
+    }
+}
+
+PK_DEVICE int brev(int i, int log2n) { return (int)(__brev((unsigned)i) >> (32 - log2n)); }
+
+__global__ void conv_twiddle_kernel(double2* __restrict__ tw, int n) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n / 2) {
+        double s, c;
+        sincospi(2.0 * (double)k / (double)n, &s, &c);
+        tw[k] = make_double2(c, -s);
+    }
+}
+
+// H[b][p] for p < ceil(M_b / Lb)
+template <typename Rir>
+__global__ void __launch_bounds__(CONV_THREADS) conv_rir_spectra_kernel(Rir rir, ConvGeom g, const double2* __restrict__ tw,
+                                                                        double2* __restrict__ H) {
+    extern __shared__ double2 cbuf[];
+    const int p = blockIdx.x, b = blockIdx.y, n = 2 * g.lb;
+    const int M = rir.length(b);
+    if (p * g.lb >= M) return;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int m = p * g.lb + i;
+        cbuf[brev(i, g.log2n)] = make_double2((i < g.lb && m < M) ? rir.at(b, m) : 0.0, 0.0);
+    }
+    __syncthreads();
+    fft_smem<false>(cbuf, g.log2n, tw);
+    double2* dst = H + ((long long)b * g.p_max + p) * (g.lb + 1);
+    for (int k = threadIdx.x; k <= g.lb; k += blockDim.x) dst[k] = cbuf[k];
+}
+
+// X[b][q] for the blocks that some output block reads: -(P_b - 1) <= q < J_b
+template <typename Rir>
+__global__ void __launch_bounds__(CONV_THREADS) conv_signal_spectra_kernel(const double* __restrict__ x, long long ld_x,
+                                                                           const int* __restrict__ n_len, Rir rir, ConvGeom g,
+                                                                           const double2* __restrict__ tw, double2* __restrict__ X) {
+    extern __shared__ double2 cbuf[];
+    const int qi = blockIdx.x, b = blockIdx.y, n = 2 * g.lb;
+    const int q = qi - (g.p_max - 1);
+    const int N = n_len[b], M = rir.length(b);
+    const int J = (N + g.lb - 1) / g.lb, P = (M + g.lb - 1) / g.lb;
+    if (q >= J || q < -(P - 1)) return;
+    const long long base = (long long)(q - 1) * g.lb + (M - 1) / 2;
+    const double* xs = x + (long long)b * ld_x;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const long long s = base + i;
+        cbuf[brev(i, g.log2n)] = make_double2((s >= 0 && s < N) ? xs[s] : 0.0, 0.0);
+    }
+    __syncthreads();
+    fft_smem<false>(cbuf, g.log2n, tw);
+    double2* dst = X + ((long long)b * g.q_max + qi) * (g.lb + 1);
+    for (int k = threadIdx.x; k <= g.lb; k += blockDim.x) dst[k] = cbuf[k];
+}
+
+// output block j: accumulate over partitions per bin, inverse FFT, keep the last Lb samples.  `unit` (nullable): signals with
+// rate == 1.0 are rounded to float32, as the reference's float32 fftconvolve returns.  Optional partial sums of squares
+// per block (0 for blocks past the signal's end).
+template <typename Rir>
+__global__ void __launch_bounds__(CONV_THREADS) conv_accum_inverse_kernel(const double2* __restrict__ H, const double2* __restrict__ X,
+                                                                          const int* __restrict__ n_len, Rir rir, ConvGeom g,
+                                                                          const double2* __restrict__ tw, const float* __restrict__ rate,
+                                                                          double* __restrict__ y, long long ld_y,
+                                                                          double* __restrict__ partial) {
+    extern __shared__ double2 cbuf[];
+    const int j = blockIdx.x, b = blockIdx.y, n = 2 * g.lb;
+    const int N = n_len[b], M = rir.length(b);
+    const int J = (N + g.lb - 1) / g.lb, P = min((M + g.lb - 1) / g.lb, g.p_max);
+    if (j >= J) {
+        if (partial && threadIdx.x == 0) partial[(long long)b * g.j_max + j] = 0.0;
+        return;
+    }
+    const double2* Hb = H + (long long)b * g.p_max * (g.lb + 1);
+    const double2* Xb = X + (long long)b * g.q_max * (g.lb + 1);
+    for (int k = threadIdx.x; k <= g.lb; k += blockDim.x) {
+        double2 acc = make_double2(0.0, 0.0);
+#pragma unroll 2
+        for (int p = 0; p < P; ++p) {
+            const double2 h = Hb[(long long)p * (g.lb + 1) + k];
+            const double2 xv = Xb[(long long)(j - p + g.p_max - 1) * (g.lb + 1) + k];
+            acc.x = fma(h.x, xv.x, fma(-h.y, xv.y, acc.x));
+            acc.y = fma(h.x, xv.y, fma(h.y, xv.x, acc.y));
+        }
+        cbuf[brev(k, g.log2n)] = acc;
+        if (k > 0 && k < g.lb) cbuf[brev(n - k, g.log2n)] = make_double2(acc.x, -acc.y);
+    }
+    __syncthreads();
+    fft_smem<true>(cbuf, g.log2n, tw);
+    const bool unit = rate && rate[b] == 1.0f;
+    const double inv_n = 1.0 / (double)n;
+    double* ys = y + (long long)b * ld_y;
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < g.lb; i += blockDim.x) {
+        const int o = j * g.lb + i;
+        if (o >= N) break;
+        double v = cbuf[g.lb + i].x * inv_n;
+        if (unit) {
+            const float f = (float)v;
+            v = (double)f;
+            acc += (double)__fmul_rn(f, f);
+        } else {
+            acc += v * v;
+        }
+        ys[o] = v;
+    }
+    if (partial) cta_partial<CONV_THREADS>(acc, partial + (long long)b * g.j_max + j);
 }
 
 // ------------------------------------------------------------------------------------ fbank
@@ -241,12 +519,98 @@ extern "C" long long pk_frontend_workspace_bytes(int B, int n_max, int t_max, in
     return b + 1024;
 }
 
-extern "C" int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
-                               const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
-                               int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
-                               const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
-                               int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
-                               long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream) {
+/* ---- float64 same-mode convolution (overlap-save), shared by pk_conv_same_f64 and the front end's reverberation stage.
+ * Workspace: twiddles [Lb] | H [B, P_max, Lb+1] | X [B, J_max + P_max - 1, Lb+1], complex f64, each 256-byte aligned. */
+static const int kRirMaxLen = 65536;
+static long long align256(long long b) { return (b + 255) & ~255LL; }
+
+// block length: a power of two in [1024, 4096], about a quarter of the longest RIR (HBM traffic of the accumulation ~ 16 N M / Lb)
+static int conv_block_len(int m_max) {
+    int lb = 1024;
+    while (lb < 4096 && 4 * lb < m_max) lb <<= 1;
+    return lb;
+}
+static ConvGeom conv_geom(int n_max, int m_max) {
+    ConvGeom g;
+    g.lb = conv_block_len(m_max);
+    g.log2n = 1;
+    while ((1 << g.log2n) < 2 * g.lb) ++g.log2n;
+    g.p_max = (m_max + g.lb - 1) / g.lb;
+    g.j_max = (n_max + g.lb - 1) / g.lb;
+    g.q_max = g.j_max + g.p_max - 1;
+    return g;
+}
+static long long conv_ws_bytes(int B, const ConvGeom& g) {
+    return align256((long long)g.lb * 16) + align256((long long)B * g.p_max * (g.lb + 1) * 16) +
+           align256((long long)B * g.q_max * (g.lb + 1) * 16);
+}
+
+// y [B, ld_y] <- same-mode convolution of x (lengths n_len) with rir; y may alias x.  Partial sums of squares per Lb block into
+// partial [B, J_max] when non-null.
+template <typename Rir>
+static int conv_same_launch(const double* x, long long ld_x, const int* n_len, Rir rir, int B, const ConvGeom& g, const float* rate,
+                            double* y, long long ld_y, double* partial, unsigned char* ws, cudaStream_t st) {
+    double2* tw = reinterpret_cast<double2*>(ws);
+    ws += align256((long long)g.lb * 16);
+    double2* H = reinterpret_cast<double2*>(ws);
+    ws += align256((long long)B * g.p_max * (g.lb + 1) * 16);
+    double2* X = reinterpret_cast<double2*>(ws);
+    const int smem = 2 * g.lb * (int)sizeof(double2);
+    PK_CHECK_CUDA(cudaFuncSetAttribute(conv_rir_spectra_kernel<Rir>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(conv_signal_spectra_kernel<Rir>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(conv_accum_inverse_kernel<Rir>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    conv_twiddle_kernel<<<(g.lb + 255) / 256, 256, 0, st>>>(tw, 2 * g.lb);
+    PK_CHECK_LAUNCH(); count_launch();
+    conv_rir_spectra_kernel<Rir><<<dim3(g.p_max, B), CONV_THREADS, smem, st>>>(rir, g, tw, H);
+    PK_CHECK_LAUNCH(); count_launch();
+    conv_signal_spectra_kernel<Rir><<<dim3(g.q_max, B), CONV_THREADS, smem, st>>>(x, ld_x, n_len, rir, g, tw, X);
+    PK_CHECK_LAUNCH(); count_launch();
+    conv_accum_inverse_kernel<Rir><<<dim3(g.j_max, B), CONV_THREADS, smem, st>>>(H, X, n_len, rir, g, tw, rate, y, ld_y, partial);
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
+extern "C" long long pk_conv_same_f64_workspace_bytes(int B, int n_max, int m_max) {
+    if (B <= 0 || n_max <= 0 || m_max < 1 || m_max > kRirMaxLen) return -1;
+    return conv_ws_bytes(B, conv_geom(n_max, m_max));
+}
+
+extern "C" int pk_conv_same_f64(const double* x, long long ld_x, const int* n_len, const double* h, long long ld_h, const int* m_len,
+                                int B, int n_max, int m_max, double* y, long long ld_y, void* workspace, long long workspace_bytes,
+                                void* stream) {
+    PK_CHECK_ARG(B > 0 && n_max > 0 && m_max >= 1 && m_max <= kRirMaxLen, "bad conv dims (1 <= m_max <= 65536)");
+    const ConvGeom g = conv_geom(n_max, m_max);
+    PK_CHECK_ARG(workspace_bytes >= conv_ws_bytes(B, g), "conv workspace too small");
+    return conv_same_launch(x, ld_x, n_len, RirF64{h, ld_h, m_len}, B, g, nullptr, y, ld_y, nullptr,
+                            reinterpret_cast<unsigned char*>(workspace), reinterpret_cast<cudaStream_t>(stream));
+}
+
+/* Noise / RIR banks of pk_frontend_fwd_noise_rir (either may be absent: noise == nullptr / rir == nullptr). */
+struct NoiseRirArgs {
+    const short* noise; const int* noise_idx; const long long* noise_off; const double* snr; const double* noise_rms_db;
+    const short* rir; const long long* rir_off; const int* rir_len; const int* rir_idx; int rir_max_len;
+};
+
+/* Workspace of the noise / reverberation path: that of pk_frontend_fwd | partial f64 [B, parts] x 2 | conv partial f64 [B, J_max] |
+ * convolution workspace */
+static long long noise_rir_extra_bytes(int B, int n_max, int rir_max_len, ConvGeom* g_out) {
+    const ConvGeom g = conv_geom(n_max, rir_max_len);
+    if (g_out) *g_out = g;
+    return 2 * align256((long long)B * kAugParts * 8) + align256((long long)B * g.j_max * 8) + conv_ws_bytes(B, g);
+}
+
+extern "C" long long pk_frontend_noise_rir_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D, int rir_max_len) {
+    if (rir_max_len < 1 || rir_max_len > kRirMaxLen) return -1;
+    return align256(pk_frontend_workspace_bytes(B, n_max, t_max, n_mel, D)) + noise_rir_extra_bytes(B, n_max, rir_max_len, nullptr);
+}
+
+// the launch sequence of both front-end entry points; nr == nullptr is pk_frontend_fwd (gain and quantisation in one pass)
+static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                           const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx, int rctx,
+                           const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi,
+                           float preemph, int cmn, const float* offset, const float* scale, int f0, int fs, int t0, int ts, void* out,
+                           int out_dtype, short* wave_i16_out, void* workspace, long long workspace_bytes, int* err_flag, float dither,
+                           unsigned int dither_seed, void* stream, const NoiseRirArgs* nr) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int D = n_mel * (lctx + 1 + rctx);
     PK_CHECK_ARG(B > 0 && n_max >= FB_FRAME && t_max > 0 && n_mel > 0 && n_mel <= 256 && D <= 1024, "bad frontend dims");
@@ -260,9 +624,36 @@ extern "C" int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_
     dim3 ga(kAugParts, B);
     aug_resample_kernel<<<ga, AUG_THREADS, 0, st>>>(pcm, ld_pcm, n_samples, rate, new_len, resampled, n_max, partial, kAugParts);
     PK_CHECK_LAUNCH(); count_launch();
-    aug_gain_kernel<<<ga, AUG_THREADS, 0, st>>>(resampled, n_max, partial, kAugParts, rate, new_len, target_db, wave, wave_i16_out, n_max,
-                                               err_flag);
-    PK_CHECK_LAUNCH(); count_launch();
+    if (!nr) {
+        aug_gain_kernel<<<ga, AUG_THREADS, 0, st>>>(resampled, n_max, partial, kAugParts, rate, new_len, target_db, wave, wave_i16_out,
+                                                   n_max, err_flag);
+        PK_CHECK_LAUNCH(); count_launch();
+    } else {
+        PK_CHECK_ARG(nr->rir_max_len >= 1 && nr->rir_max_len <= kRirMaxLen, "rir_max_len must be in [1, 65536]");
+        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_max, n_mel, D));
+        ConvGeom g;
+        PK_CHECK_ARG(workspace_bytes >= base + noise_rir_extra_bytes(B, n_max, nr->rir_max_len, &g), "frontend workspace too small");
+        unsigned char* x = reinterpret_cast<unsigned char*>(workspace) + base;
+        double* part_gain = reinterpret_cast<double*>(x);  x += align256((long long)B * kAugParts * 8);
+        double* part_noisy = reinterpret_cast<double*>(x); x += align256((long long)B * kAugParts * 8);
+        double* part_conv = reinterpret_cast<double*>(x);  x += align256((long long)B * g.j_max * 8);
+        aug_gain_keep_kernel<<<ga, AUG_THREADS, 0, st>>>(resampled, n_max, partial, kAugParts, rate, new_len, target_db, part_gain, err_flag);
+        PK_CHECK_LAUNCH(); count_launch();
+        const double* pre = part_gain;
+        if (nr->noise) {
+            aug_noise_kernel<<<ga, AUG_THREADS, 0, st>>>(resampled, n_max, part_gain, kAugParts, rate, new_len, nr->noise, nr->noise_idx,
+                                                        nr->noise_off, nr->snr, nr->noise_rms_db, part_noisy);
+            PK_CHECK_LAUNCH(); count_launch();
+            pre = part_noisy;
+        }
+        if (nr->rir) {
+            RirBank bank{nr->rir, nr->rir_off, nr->rir_len, nr->rir_idx};
+            if (conv_same_launch(resampled, n_max, new_len, bank, B, g, rate, resampled, n_max, part_conv, x, st)) return 1;
+        }
+        aug_renorm_quant_kernel<<<ga, AUG_THREADS, 0, st>>>(resampled, n_max, pre, kAugParts, nr->rir ? part_conv : nullptr, g.j_max, rate,
+                                                           new_len, wave, wave_i16_out, n_max, err_flag);
+        PK_CHECK_LAUNCH(); count_launch();
+    }
     FbankTables tb{window, reinterpret_cast<const float2*>(twiddle), mel_w, mel_lo, mel_hi};
     fbank_kernel<<<dim3(t_max, B), 256, 0, st>>>(wave, n_max, n_frames, tb, n_mel, preemph, feats, (long long)t_max * n_mel, t_max, dither,
                                                  dither_seed);
@@ -283,6 +674,34 @@ extern "C" int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_
                                                                   offset, scale, f0, fs, t0, ts, reinterpret_cast<float*>(out));
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
+}
+
+extern "C" int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                               const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
+                               int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
+                               const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
+                               int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                               long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream) {
+    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, window, twiddle,
+                           mel_w, mel_lo, mel_hi, preemph, cmn, offset, scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace,
+                           workspace_bytes, err_flag, dither, dither_seed, stream, nullptr);
+}
+
+extern "C" int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                                         const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
+                                         int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
+                                         const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0,
+                                         int fs, int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                                         long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
+                                         const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,
+                                         const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
+                                         const int* rir_idx, int rir_max_len) {
+    PK_CHECK_ARG(!noise || (noise_idx && noise_off && snr && noise_rms_db), "noise bank without its per-utterance draws");
+    PK_CHECK_ARG(!rir || (rir_off && rir_len && rir_idx), "RIR bank without its offsets, lengths or per-utterance draws");
+    const NoiseRirArgs nr{noise, noise_idx, noise_off, snr, noise_rms_db, rir, rir_off, rir_len, rir_idx, rir_max_len};
+    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, window, twiddle,
+                           mel_w, mel_lo, mel_hi, preemph, cmn, offset, scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace,
+                           workspace_bytes, err_flag, dither, dither_seed, stream, &nr);
 }
 
 /* feats-only entry (fbank of already-augmented int16-scaled samples), used by parity tests and by

@@ -47,6 +47,11 @@ class FbankOptions:
         return cls(**kw)
 
 
+def noise_rir_kwargs(raw):
+    """the Frontend keyword arguments for the noise / reverberation draws of a raw batch (empty without them)"""
+    return {k: raw[k] for k in ("noise_idx", "noise_off", "snr", "rir_idx", "rir_max_len") if k in raw}
+
+
 def _mel(f):
     return 1127.0 * math.log(1.0 + f / 700.0)
 
@@ -85,6 +90,7 @@ class Frontend:
         self.window, self.twiddle, self.mel_w, self.mel_lo, self.mel_hi = t(win), t(tw), t(w.astype(np.float32)), t(lo), t(hi_i)
         self.err = torch.zeros(1, dtype=torch.int32, device=device)
         self._ws = None
+        self.noise = self.rir = None           # AudioBank defaults for on-the-fly noise / reverberation (loader/audio_bank.py)
         self.dither_seed = 0x243F6A88          # advanced once per batch: every batch draws fresh dither noise
 
     @staticmethod
@@ -95,24 +101,67 @@ class Frontend:
         return new_len, frames
 
     def __call__(self, pcm, n_samples, rate, target_db, new_len, n_frames, t_max, out_dtype=torch.float32, cmn=True,
-                 offset=None, scale=None, specaug=(0, 0, 0, 0), want_wave=False):
+                 offset=None, scale=None, specaug=(0, 0, 0, 0), want_wave=False, noise=None, noise_idx=None, noise_off=None,
+                 snr=None, rir=None, rir_idx=None, rir_max_len=None):
         """pcm int16 [B, n_max] (device); n_samples/new_len/n_frames int32 [B], rate/target_db f32 [B] (device);
-        -> feats [B, t_max, D] (out_dtype) [, augmented int16 wave]."""
+        -> feats [B, t_max, D] (out_dtype) [, augmented int16 wave].
+
+        On-the-fly noise (loader/audio.py:467-513 add_noise) runs when ``noise_idx`` is given: noise_idx int32 [B] segment of
+        ``noise`` (an ``AudioBank``, default ``self.noise``), noise_off int64 [B] offset inside that segment, snr f64 [B] dB.
+        Reverberation (convolve_and_normalize, :450-465) runs when ``rir_idx`` int32 [B] is given, with ``rir`` (default
+        ``self.rir``); rir_max_len: host int >= the longest drawn RIR (computed from the bank when omitted)."""
         B, n_max = pcm.shape
-        need = int(lib.pk_frontend_workspace_bytes(B, n_max, t_max, self.n_mel, self.D))
+        aug = noise_idx is not None or rir_idx is not None
+        if aug:
+            rir_max_len = self._rir_max_len(rir, rir_idx, rir_max_len)
+            need = int(lib.pk_frontend_noise_rir_workspace_bytes(B, n_max, t_max, self.n_mel, self.D, rir_max_len))
+            if need < 0:
+                raise ValueError("rir_max_len %d outside [1, 65536]" % rir_max_len)
+        else:
+            need = int(lib.pk_frontend_workspace_bytes(B, n_max, t_max, self.n_mel, self.D))
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         out = torch.empty(B, t_max, self.D, dtype=out_dtype, device=self.device)
         wave = torch.zeros(B, n_max, dtype=torch.int16, device=self.device) if want_wave else None
         P = K._P
         f0, fs, t0, ts = specaug
-        check(lib.pk_frontend_fwd(P(pcm), ctypes.c_longlong(pcm.stride(0)), P(n_samples), P(rate), P(new_len), P(target_db),
-                                  P(n_frames), B, n_max, t_max, self.n_mel, self.lctx, self.rctx, P(self.window), P(self.twiddle),
-                                  P(self.mel_w), P(self.mel_lo), P(self.mel_hi), ctypes.c_float(self.opts.preemphasis_coefficient),
-                                  int(cmn), P(offset), P(scale), int(f0), int(fs), int(t0), int(ts), P(out), K._dt(out), P(wave),
-                                  P(self._ws), ctypes.c_longlong(need), P(self.err), ctypes.c_float(self.opts.dither),
-                                  ctypes.c_uint32(self._next_dither_seed()), K._stream()), "pk_frontend_fwd")
+        args = (P(pcm), ctypes.c_longlong(pcm.stride(0)), P(n_samples), P(rate), P(new_len), P(target_db),
+                P(n_frames), B, n_max, t_max, self.n_mel, self.lctx, self.rctx, P(self.window), P(self.twiddle),
+                P(self.mel_w), P(self.mel_lo), P(self.mel_hi), ctypes.c_float(self.opts.preemphasis_coefficient),
+                int(cmn), P(offset), P(scale), int(f0), int(fs), int(t0), int(ts), P(out), K._dt(out), P(wave),
+                P(self._ws), ctypes.c_longlong(need), P(self.err), ctypes.c_float(self.opts.dither),
+                ctypes.c_uint32(self._next_dither_seed()), K._stream())
+        if not aug:
+            check(lib.pk_frontend_fwd(*args), "pk_frontend_fwd")
+            return (out, wave) if want_wave else out
+        dev = lambda t, dt: torch.as_tensor(t).to(device=self.device, dtype=dt, non_blocking=True)  # noqa: E731
+        nz = (None,) * 5
+        if noise_idx is not None:
+            bank = noise if noise is not None else self.noise
+            if bank is None:
+                raise ValueError("noise draws given without a noise bank")
+            samples, offs, _, rms = bank.device(self.device)
+            idx = dev(noise_idx, torch.int32)
+            start = offs[idx.long()] + dev(noise_off, torch.int64)                 # absolute bank offset of the first sample
+            nz = (samples, idx, start, dev(snr, torch.float64), rms)
+        rr = (None,) * 4
+        if rir_idx is not None:
+            bank = rir if rir is not None else self.rir
+            samples, offs, lens, _ = bank.device(self.device)
+            rr = (samples, offs, lens, dev(rir_idx, torch.int32))
+        check(lib.pk_frontend_fwd_noise_rir(*args, *[P(t) for t in nz], *[P(t) for t in rr], int(rir_max_len)),
+              "pk_frontend_fwd_noise_rir")
         return (out, wave) if want_wave else out
+
+    def _rir_max_len(self, rir, rir_idx, rir_max_len):
+        if rir_idx is None:
+            return 1
+        bank = rir if rir is not None else self.rir
+        if bank is None:
+            raise ValueError("RIR draws given without an RIR bank")
+        if rir_max_len is None:
+            rir_max_len = int(bank.lengths[torch.as_tensor(rir_idx).cpu().numpy()].max())
+        return int(rir_max_len)
 
     def _next_dither_seed(self):
         self.dither_seed = (self.dither_seed * 1664525 + 1013904223) & 0xFFFFFFFF

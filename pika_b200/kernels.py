@@ -436,3 +436,21 @@ def beam_xf_slots(st, prev_ks, K):
 def ce_grad(z, tok, coef, scale, dz, n):
     rows, ld = z.shape
     check(lib.pk_ce_grad(_P(z), _I(_dt(z)), _L(ld), _P(tok), _P(coef), _F(scale), _P(dz), _L(rows), _I(n), _stream()), "pk_ce_grad")
+
+
+def conv_same_f64(x, n_len, h, m_len, y=None):
+    """scipy.signal.fftconvolve(x[b, :n_len[b]], h[b, :m_len[b]], "same") per row, float64 (pk_conv_same_f64).
+    x [B, n] f64, h [B, m] f64, n_len / m_len int32 [B] on the device; host-side bounds are the row widths.  -> y [B, n] f64
+    (entries past n_len[b] are left untouched)."""
+    assert x.dtype == torch.float64 and h.dtype == torch.float64 and x.stride(1) == 1 and h.stride(1) == 1
+    B, n = x.shape
+    m = h.shape[1]
+    if y is None:
+        y = torch.zeros_like(x)
+    need = int(lib.pk_conv_same_f64_workspace_bytes(B, n, m))
+    if need < 0:
+        raise ValueError("pk_conv_same_f64: RIR width %d outside [1, 65536]" % m)
+    ws = torch.empty(need, dtype=torch.uint8, device=x.device)
+    check(lib.pk_conv_same_f64(_P(x), x.stride(0), _P(n_len), _P(h), h.stride(0), _P(m_len), B, n, m, _P(y), y.stride(0), _P(ws), need,
+                               _stream()), "pk_conv_same_f64")
+    return y

@@ -8,6 +8,12 @@ draw the augmentation parameters from the SAME random streams in the SAME order 
 (``random.randint`` for the speed rate, ``numpy.random.uniform`` for the gain target, :221-223), apply the TU
 filter (:247) from the frame count the front end will produce, and assemble padded batches.
 
+With a noise bank (``--noise_lst``) and / or an RIR bank (``--rir_lst``) each utterance also draws, in the order of the
+reference's commented-out example (:224-228): ``scipy.stats.truncnorm.rvs`` for the SNR (numpy's global stream), then
+``random.randint`` for the noise segment and for the noise offset, then ``random.randint`` for the RIR.  One documented
+deviation: the reference's ``add_noise`` draws a float start time from a fresh, unseeded ``random.Random()``; here the offset
+is an integer sample index from the module's ``random`` stream.
+
 ``dataloader`` yields, like the reference (:272-289), 4-tuples ``(data, target, lens, ali_lens)``; ``data`` is
 either the reference's float feature tensor [B,Tmax,D] (``args.raw_batches`` false: features computed on the GPU
 and returned as a CPU tensor) or, for the fused trainer path, a dict of raw-PCM tensors for ``TrainStep``.
@@ -20,7 +26,7 @@ from threading import Thread
 import numpy as np
 import torch
 
-from ..frontend import FbankOptions, Frontend
+from ..frontend import FbankOptions, Frontend, noise_rir_kwargs
 from . import kaldi_io
 
 
@@ -55,6 +61,35 @@ def register(parser):
     parser.add_argument('--verbose', action='store_true', help='printing out warnings')
 
 
+def snr_params(snr_range):
+    """``--snr_range lo,hi`` -> (mu, sigma) of the truncated normal on [lo, hi]; empty = the reference example's 0,20 dB
+    (mu 10, sigma 10, loader/otf_utt_loader.py:191-193)"""
+    if not snr_range:
+        lo, hi = 0.0, 20.0
+    else:
+        p = [float(v) for v in snr_range.split(',')]
+        if len(p) != 2 or not p[1] > p[0]:
+            raise ValueError("--snr_range expects 'lo,hi' with hi > lo, got %r" % snr_range)
+        lo, hi = p
+    return (lo + hi) / 2.0, (hi - lo) / 2.0
+
+
+def draw_noise_rir(new_len, noise, rir, snr_mu_sigma):
+    """the per-utterance noise / reverberation draws, after the speed and gain draws: (snr, k, off, r); None where a bank is absent.
+    ``off`` is clamped at 0 for an utterance longer than the noise segment (it cannot pass the --max_len filter: the bank keeps
+    only segments that cover every utterance that can)."""
+    snr = k = off = r = None
+    if noise:
+        from scipy.stats import truncnorm
+        mu, sigma = snr_mu_sigma
+        snr = float(truncnorm.rvs(-1.0, 1.0, loc=mu, scale=sigma))
+        k = randint(0, len(noise) - 1)
+        off = randint(0, max(0, int(noise.lengths[k]) - new_len))
+    if rir:
+        r = randint(0, len(rir) - 1)
+    return snr, k, off, r
+
+
 def put_thread(q, generator, *gen_args):
     for item in generator(*gen_args):
         q.put(item)
@@ -69,6 +104,7 @@ def otf_utt_generator(data_triplets, rir, noise, args):
     batch_size = args.batch_size
     speed_rate = [float(r) for r in args.speed_rate.split(',')]
     gain_lo, gain_hi = [-float(g) for g in args.gain_range.split(',')]
+    snr_mu_sigma = snr_params(args.snr_range) if noise else None
     pcm, tgt, meta = [], [], []
     batch_idx = 0
     for mrk_fn, seq_fn, ali_rspec in data_triplets:
@@ -77,6 +113,8 @@ def otf_utt_generator(data_triplets, rir, noise, args):
             assert uttid == uttid1
             spr = speed_rate[randint(0, len(speed_rate) - 1)]
             target_db = np.random.uniform(gain_lo, gain_hi)
+            new_len, frames = Frontend.lengths([audio_np.shape[0]], [spr])
+            draws = draw_noise_rir(new_len[0], noise, rir, snr_mu_sigma)
             ali = np.array(ali)
             if args.reverse_labels:
                 ali = ali[::-1]
@@ -84,21 +122,22 @@ def otf_utt_generator(data_triplets, rir, noise, args):
                 ali = np.concatenate(([args.SOS], ali))
             if args.EOS >= 0:
                 ali = np.concatenate((ali, [args.EOS]))
-            new_len, frames = Frontend.lengths([audio_np.shape[0]], [spr])
             utt_len = frames[0]
             if utt_len > 0 and utt_len <= args.max_len and ali.shape[0] * utt_len // 3 <= args.TU_limit:
                 pcm.append(audio_np)
                 tgt.append(ali.astype(np.int32))
-                meta.append((audio_np.shape[0], spr, target_db, new_len[0], utt_len))
+                meta.append((audio_np.shape[0], spr, target_db, new_len[0], utt_len) + draws)
             batch_idx += 1
             if batch_idx == batch_size:
-                yield assemble(pcm, tgt, meta, args)
+                yield assemble(pcm, tgt, meta, args, rir)
                 pcm, tgt, meta, batch_idx = [], [], [], 0
     yield None
 
 
-def assemble(pcm, tgt, meta, args):
-    """padded raw batch (or the reference's empty-batch tuple, loader/otf_utt_loader.py:283-287)"""
+def assemble(pcm, tgt, meta, args, rir=None):
+    """padded raw batch (or the reference's empty-batch tuple, loader/otf_utt_loader.py:283-287).  meta rows:
+    (n_samples, rate, target_db, new_len, n_frames[, snr, noise_idx, noise_off, rir_idx]); the noise keys (noise_idx, noise_off,
+    snr) and the RIR keys (rir_idx, and the host-side rir_max_len) are added only when those draws were made."""
     if not pcm:
         return None, None, torch.IntTensor([0]), torch.IntTensor([0])
     B = len(pcm)
@@ -117,6 +156,13 @@ def assemble(pcm, tgt, meta, args):
                new_len=torch.tensor([m[3] for m in meta], dtype=torch.int32),
                n_frames=torch.tensor([m[4] for m in meta], dtype=torch.int32),
                t_max=max(m[4] for m in meta))
+    if len(meta[0]) > 5 and meta[0][5] is not None:
+        raw.update(noise_idx=torch.tensor([m[6] for m in meta], dtype=torch.int32),
+                   noise_off=torch.tensor([m[7] for m in meta], dtype=torch.int64),
+                   snr=torch.tensor([m[5] for m in meta], dtype=torch.float64))
+    if len(meta[0]) > 5 and meta[0][8] is not None:
+        raw.update(rir_idx=torch.tensor([m[8] for m in meta], dtype=torch.int32),
+                   rir_max_len=int(max(rir.lengths[m[8]] for m in meta)))
     lens = raw["n_frames"].clone()
     ali_lens = torch.tensor([len(t) for t in tgt], dtype=torch.int32)
     return raw, target, lens, ali_lens
@@ -135,12 +181,16 @@ def _frontend_for(args, device):
     return _frontends[key]
 
 
-def raw_to_features(raw, args, device="cuda"):
+def raw_to_features(raw, args, device="cuda", noise=None, rir=None):
     """reference-shaped float features [B,Tmax,D] on the CPU from a raw batch (GPU front end, then D2H)"""
     fe = _frontend_for(args, device)
+    if noise:
+        fe.noise = noise
+    if rir:
+        fe.rir = rir
     dev = {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in raw.items()}
     out = fe(dev["pcm"], dev["n_samples"], dev["rate"], dev["target_db"], dev["new_len"], dev["n_frames"], dev["t_max"],
-             out_dtype=torch.float32, cmn=False)
+             out_dtype=torch.float32, cmn=False, **noise_rir_kwargs(dev))
     return out.cpu()
 
 
@@ -148,7 +198,7 @@ def dataloader(data_lst, rir, noise, args):
     """
     Args:
         data_lst: list of mrk and seq of input audios, and label ark
-        rir, noise: unused lists (as in the shipped reference recipes)
+        rir, noise: ``AudioBank`` (loader/audio_bank.py) for on-the-fly reverberation / noise, or empty lists for none
     """
     data_triplets = kaldi_io.read_lst(data_lst)
     num_per_worker = (len(data_triplets) + args.num_workers - 1) // args.num_workers
@@ -172,7 +222,7 @@ def dataloader(data_lst, rir, noise, args):
         if raw is None or raw_mode:
             yield raw, target, lens, ali_lens
         else:
-            data = raw_to_features(raw, args)
+            data = raw_to_features(raw, args, noise=noise, rir=rir)
             if not args.batch_first:
                 data, target = data.transpose(0, 1).contiguous(), target.t().contiguous()
             yield data, target, lens, ali_lens

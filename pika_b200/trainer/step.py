@@ -6,6 +6,7 @@ BMUF block sync every ``sync_period`` batches.
 """
 
 from .. import engine
+from ..frontend import noise_rir_kwargs
 from .flat import lr_at
 from .bmuf import SUCCESS
 
@@ -29,7 +30,8 @@ class TrainStep:
         self.num_done = 0
 
     def features(self, batch):
-        """batch: dict of device tensors (pcm int16 [B,n], n_samples, rate, target_db, new_len, n_frames) + t_max"""
+        """batch: dict of device tensors (pcm int16 [B,n], n_samples, rate, target_db, new_len, n_frames) + t_max, and the
+        noise / reverberation draws when the loader made them (loader/otf_utt_loader.py: assemble)"""
         a = self.args
         sa = (0, 0, 0, 0)
         if self.spec is not None:
@@ -39,7 +41,7 @@ class TrainStep:
         cmn = bool(a.cmn) and (self.offset is not None or bool(getattr(a, "cmn_without_stats", False)))
         return self.frontend(batch["pcm"], batch["n_samples"], batch["rate"], batch["target_db"], batch["new_len"],
                              batch["n_frames"], batch["t_max"], out_dtype=engine.act_dtype(), cmn=cmn,
-                             offset=self.offset, scale=self.scale, specaug=sa)
+                             offset=self.offset, scale=self.scale, specaug=sa, **noise_rir_kwargs(batch))
 
     def __call__(self, batch):
         """-> per-utterance costs [B] (device).  Mirrors :71-123 of the reference trainer."""

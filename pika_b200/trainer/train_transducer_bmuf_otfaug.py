@@ -17,6 +17,7 @@ import sys
 import torch
 
 from ..frontend import FbankOptions, Frontend
+from ..loader.audio_bank import AudioBank
 from ..loader import kaldi_io
 from ..utils.logger import Logger
 from ..utils.spec_augment import SpecAugment
@@ -143,7 +144,9 @@ def main(argv=None):
     assert args.cuda and torch.cuda.is_available(), "pika_b200 trains on the GPU (there is no CPU fallback)"
     torch.cuda.set_device(args.local_rank)
     dev = torch.device("cuda", args.local_rank)
-    args.rir, args.noise = [], []
+    # on-the-fly reverberation and noise (trainer/train_transducer_bmuf_otfaug.py:272-282): banks read once, uploaded once
+    args.rir = AudioBank.rir(args.rir_lst) if args.rir_lst else []
+    args.noise = AudioBank.noise(args.noise_lst, args.max_len) if args.noise_lst else []
     args.data_lst = args.data_lst.replace('WORKER-ID', str(args.local_rank))
     args.log = args.log.replace('WORKER-ID', str(args.local_rank))
     log_f = open(args.log, 'w')
@@ -171,6 +174,8 @@ def main(argv=None):
     # opts.dither is honoured (egs/fbank.conf: dither=1): counter-based Gaussian dither in the fbank kernel; set dither=0 in the
     # feature config for bit-reproducible features (Kaldi's own RNG stream is not reproduced, DESIGN.md)
     args.frontend = Frontend(opts, args.lctx, args.rctx, dev)
+    args.frontend.noise = args.noise or None
+    args.frontend.rir = args.rir or None
     args.offset = args.scale = None
     if args.cmvn_stats:
         try:

@@ -19,6 +19,7 @@ import torch
 from ..decoder.beam_transducer import GlobalScorer
 from ..decoder.transducer_decoder import TransducerDecoder
 from ..frontend import FbankOptions, Frontend
+from ..loader.audio_bank import AudioBank
 from ..loader import kaldi_io
 from ..utils.logger import Logger
 from ..utils.spec_augment import SpecAugment
@@ -116,7 +117,9 @@ def main(argv=None):
     assert args.cuda and torch.cuda.is_available(), "pika_b200 trains on the GPU (there is no CPU fallback)"
     torch.cuda.set_device(args.local_rank)
     dev = torch.device("cuda", args.local_rank)
-    args.rir, args.noise = [], []
+    # on-the-fly reverberation and noise (trainer/train_transducer_bmuf_otfaug.py:272-282): banks read once, uploaded once
+    args.rir = AudioBank.rir(args.rir_lst) if args.rir_lst else []
+    args.noise = AudioBank.noise(args.noise_lst, args.max_len) if args.noise_lst else []
     args.data_lst = args.data_lst.replace('WORKER-ID', str(args.local_rank))
     args.log = args.log.replace('WORKER-ID', str(args.local_rank))
     log_f = open(args.log, 'w')
@@ -134,6 +137,8 @@ def main(argv=None):
     bmuf_trainer = BmufTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr, flat=flat)
     opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
     args.frontend = Frontend(opts, args.lctx, args.rctx, dev)
+    args.frontend.noise = args.noise or None
+    args.frontend.rir = args.rir or None
     args.offset = args.scale = None
     if args.cmvn_stats:
         try:
