@@ -256,6 +256,26 @@ int pk_sgd_nesterov_clip(float* p, const float* g, float* buf, long long n, floa
 int pk_bmuf_delta(const float* glob, const float* local, float* delta, long long n, void* stream);
 int pk_bmuf_update(float* glob, float* local, float* delta_prev, const float* delta_sum, long long n, int world,
                    float block_momentum, float block_lr, void* stream);
+/* pk_absmax + pk_adam_clip: clip_grad_norm_(params, max_norm, inf) + optim.Adam(lr, betas, eps, weight_decay=0,
+ * amsgrad=False).step() (trainer/bmuf.py:204,215 -- the local optimiser of BmufAdamTrainer) over (p, g, exp_avg, exp_avg_sq).
+ * The clip and its NaN rule are pk_sgd_nesterov_clip's (max_norm <= 0: no clip).  The caller forms the bias corrections
+ * 1 - beta1^step and sqrt(1 - beta2^step) in double; step may be fractional after a BMUF-Adam sync (trainer/bmuf.py:311).
+ * Element formula as torch's CUDA Adam: m.lerp_(g, 1-beta1); v = beta2*v + (1-beta2)*g*g;
+ * p -= (lr/bias_correction1) * m / (sqrt(v)/bias_correction2_sqrt + eps).
+ * p_out2 (may be NULL): also receives the new p -- BlockAdamTrainer's copy of the global vector into the model
+ * (trainer/bmuf.py:163-166) in the same pass. */
+int pk_adam_clip(float* p, const float* g, float* exp_avg, float* exp_avg_sq, float* p_out2, long long n, double lr,
+                 double beta1, double beta2, double eps, double bias_correction1, double bias_correction2_sqrt,
+                 float max_norm, const float* absmax, const int* nan_flag, void* stream);
+/* BmufAdamTrainer.update_and_sync (trainer/bmuf.py:273-321), the master update replicated on every rank after an all-reduce.
+ * msg = [delta_sum; exp_avg_sum; exp_avg_sq_sum] (3n floats, the summed pk_bmuf_delta output and local moments).  Updates the
+ * global parameters glob and delta_prev (block momentum, as pk_bmuf_update), the filtered global moments exp_avg_g /
+ * exp_avg_sq_g, writes local := glob, and overwrites msg's two moment slots with the new local moments.  beta1_tau = beta1^tau,
+ * beta1_rho = beta1^(rho*block_momentum) (likewise beta2), formed by the caller in double; tau = sync_period and rho is the
+ * already-updated block-momentum sum of :273. */
+int pk_bmuf_adam_update(float* glob, float* local, float* delta_prev, float* exp_avg_g, float* exp_avg_sq_g, float* msg,
+                        long long n, int world, double block_momentum, double block_lr, double beta1_tau, double beta1_rho,
+                        double beta2_tau, double beta2_rho, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * On-the-fly front end (pika_b200/csrc/frontend.cu): int16 PCM -> speed perturbation + RMS gain +

@@ -83,6 +83,9 @@ _sig("pk_rnnt_loss_fwd_bwd_lse", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i
 _sig("pk_frontend_noise_rir_workspace_bytes", [_i, _i, _i, _i, _i, _i], ctypes.c_longlong)
 _sig("pk_conv_same_f64_workspace_bytes", [_i, _i, _i], ctypes.c_longlong)
 _sig("pk_conv_same_f64", [_vp, _ll, _vp, _vp, _ll, _vp, _i, _i, _i, _vp, _ll, _vp, _ll, _vp])
+_d = ctypes.c_double
+_sig("pk_adam_clip", [_vp, _vp, _vp, _vp, _vp, _ll, _d, _d, _d, _d, _d, _d, _f, _vp, _vp, _vp])
+_sig("pk_bmuf_adam_update", [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _d, _d, _d, _d, _d, _d, _vp])
 
 
 def check(rc, what=""):

@@ -30,5 +30,5 @@ int num_sms() {
 }  // namespace pk
 
 extern "C" const char* pk_last_error(void) { return pk::g_err; }
-extern "C" int pk_version(void) { return 103; }
+extern "C" int pk_version(void) { return 104; }
 extern "C" long long pk_launch_count(void) { return pk::g_launches.load(); }

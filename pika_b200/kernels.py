@@ -351,6 +351,28 @@ def bmuf_update(glob, local, delta_prev, delta_sum, world, bm, blr):
                              _stream()), "pk_bmuf_update")
 
 
+def adam_clip(p, g, exp_avg, exp_avg_sq, lr, betas, eps, step, max_norm=-1.0, absmax_t=None, nan_flag=None, p_out2=None):
+    """clip (when max_norm > 0, from pk_absmax's absmax_t / nan_flag) + one Adam step at ``step`` (the already-incremented,
+    possibly fractional step count); the bias corrections are formed here in double, as torch.optim.Adam forms them"""
+    for t in (g, exp_avg, exp_avg_sq) + ((p_out2,) if p_out2 is not None else ()):
+        assert t.numel() == p.numel() and t.dtype == torch.float32 and t.is_contiguous()
+    beta1, beta2 = betas
+    bc1 = 1 - beta1 ** step
+    bc2_sqrt = (1 - beta2 ** step) ** 0.5
+    on = max_norm > 0
+    check(lib.pk_adam_clip(_P(p), _P(g), _P(exp_avg), _P(exp_avg_sq), _P(p_out2), p.numel(), lr, beta1, beta2, eps, bc1, bc2_sqrt,
+                           max_norm, _P(absmax_t if on else None), _P(nan_flag if on else None), _stream()), "pk_adam_clip")
+
+
+def bmuf_adam_update(glob, local, delta_prev, exp_avg_g, exp_avg_sq_g, msg, world, bm, blr, beta1_tau, beta1_rho, beta2_tau,
+                     beta2_rho):
+    """msg: [delta_sum; exp_avg_sum; exp_avg_sq_sum] (3n); the powers of beta are formed by the caller in double"""
+    n = glob.numel()
+    assert msg.numel() == 3 * n and all(t.numel() == n for t in (local, delta_prev, exp_avg_g, exp_avg_sq_g))
+    check(lib.pk_bmuf_adam_update(_P(glob), _P(local), _P(delta_prev), _P(exp_avg_g), _P(exp_avg_sq_g), _P(msg), n, world, bm, blr,
+                                  beta1_tau, beta1_rho, beta2_tau, beta2_rho, _stream()), "pk_bmuf_adam_update")
+
+
 _lstm_ws = {}
 
 

@@ -22,8 +22,8 @@ from ..loader import kaldi_io
 from ..utils.logger import Logger
 from ..utils.spec_augment import SpecAugment
 from .. import engine
-from .bmuf import BmufTrainer
-from .flat import FlatParams, SgdNesterovClip, lr_at
+from .bmuf import BlockAdamTrainer, BmufAdamTrainer, BmufTrainer
+from .flat import AdamClip, FlatParams, SgdNesterovClip, lr_at
 from .step import TrainStep
 
 MASTER_NODE = 0
@@ -36,7 +36,11 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
     lr = lr_at(args.initial_lr, args.final_lr, epoch * args.num_batches_per_epoch, total_num_batches)
     log_f.write('===Using Learning Rate {}===\n'.format(lr))
     args.epoch = epoch
-    optimizer = SgdNesterovClip(bmuf_trainer.flat, lr, args.momentum, args.grad_clip)
+    if args.block_sync == 'bmuf_adam':
+        optimizer = bmuf_trainer.optim                        # one local Adam for the whole run: moments and step persist
+        optimizer.reset(lr)
+    else:
+        optimizer = SgdNesterovClip(bmuf_trainer.flat, lr, args.momentum, args.grad_clip)
     loss_logger = Logger(args.log, args.log_per_n_frames, ['Loss'])
     spec = SpecAugment(args.max_freq_span, args.max_time_span) if args.spec_augment else None
     model.train(training)
@@ -122,6 +126,11 @@ def build_parser():
     parser.add_argument('--block_momentum', type=float, default=0.9)
     parser.add_argument('--block_lr', type=float, default=1.0)
     parser.add_argument('--sync_period', type=int, default=100)
+    parser.add_argument('--block_sync', choices=['bmuf', 'bmuf_adam', 'block_adam'], default='bmuf',
+                        help='block trainer of trainer/bmuf.py: bmuf = BmufTrainer (Nesterov block momentum, local SGD; the '
+                             'reference recipe); bmuf_adam = BmufAdamTrainer (local Adam at the scheduled learning rate, moments '
+                             'averaged and filtered at every sync); block_adam = BlockAdamTrainer (local SGD, the summed block '
+                             'delta applied by Adam at --block_lr)')
     parser.add_argument('--spec_augment', action='store_true')
     parser.add_argument('--max_freq_span', type=int, default=15)
     parser.add_argument('--max_time_span', type=int, default=35)
@@ -161,7 +170,14 @@ def main(argv=None):
         model = torch.load(args.init_model, map_location=lambda storage, loc: storage, weights_only=False)
     model.to(dev)
     flat = FlatParams(model)
-    bmuf_trainer = BmufTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr, flat=flat)
+    if args.block_sync == 'bmuf_adam':
+        lr0 = lr_at(args.initial_lr, args.final_lr, 0, args.num_epochs * args.num_batches_per_epoch)
+        bmuf_trainer = BmufAdamTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr,
+                                       args.sync_period, AdamClip(flat, lr0, max_norm=args.grad_clip), flat=flat)
+    elif args.block_sync == 'block_adam':
+        bmuf_trainer = BlockAdamTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_lr, flat=flat)
+    else:
+        bmuf_trainer = BmufTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr, flat=flat)
     num_param = sum(p.numel() for p in model.parameters())
     log_f.write('*' * 60 + '\n')
     log_f.write('model proto: {}\ninput  dim: {},\toutput dim: {},\nhidden dim: {},\tnum of enc_layers: {}\n'

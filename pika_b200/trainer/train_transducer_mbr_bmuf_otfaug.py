@@ -106,6 +106,8 @@ def main(argv=None):
     loader_module = importlib.import_module('pika_b200.loader.' + args.loader + '_loader')
     loader_module.register(parser)
     args = parser.parse_args(argv)
+    if args.block_sync != 'bmuf':        # inherited from the RNN-T parser; the MBR trainer runs BmufTrainer only, as the reference's
+        parser.error('--block_sync %s: the MBR trainer supports only bmuf' % args.block_sync)
     if args.lm:
         raise NotImplementedError("pika_b200: --lm (neural LM fusion) is outside the hot path")
     args.input_dim = loader_module.get_inputdim(args)
