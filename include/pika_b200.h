@@ -170,8 +170,9 @@ int pk_attention_bwd_bits(const void* q, const void* k, const void* v, long long
                           long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
                           void* stream);
 /* nn.BatchNorm1d over rows [rows, C] (trainer/model/rnnt_tdnn_transformer.py:41,58-59,69,76-82,85):
- * train: batch statistics incl. padded frames, running stats updated (momentum 0.1); eval: running stats.
- * stats_ws: pk_colstats_ws_floats(C) + 2*C floats scratch.  mean/rstd [C] are saved for the backward. */
+ * train: batch statistics incl. padded frames, running stats updated with the given momentum (unbiased variance); eval: running
+ * stats.  stats_ws: pk_colstats_ws_floats(C) + 2*C floats scratch.  mean/rstd [C] are saved for the backward.
+ * x, y, stats_ws (and dy, dx, ws of the backward, x of pk_colsum) must be 16-byte aligned. */
 long long pk_colstats_ws_floats(int C);
 int pk_bn_fwd(const void* x, void* y, int dtype, long long rows, int C, const float* w, const float* b, float eps,
               int train, float momentum, float* run_mean, float* run_var, float* mean, float* rstd, float* stats_ws,

@@ -76,7 +76,11 @@ __global__ void cast_split_kernel(const S* __restrict__ src, long long ld_src, _
 // =============================================================================== column statistics
 // sums[c] += sum_r f(x[r,c]); sums2[c] += sum_r x[r,c]*g[r,c]  (g = x for BN stats, x_hat for BN/LN bwd)
 // Block: 128 threads x 8 channels = 1024 channels per pass; rows split across blockIdx.y.
-template <typename T, int MODE>   // MODE 0: (sum x, sum x^2); 1: (sum dy, sum dy*xhat) with xhat=(x-mean)*rstd
+// MODE 0: (sum x, sum x^2); 1: (sum dy, sum dy*xhat) with xhat=(x-mean)*rstd;
+// 2: (sum d, sum d^2) with d = x - x[0,c]: the BN statistics.  Shifting by a value of the channel keeps s2/n - (s1/n)^2 accurate when
+//    the channel's mean is large against its spread (an almost-always-on ReLU channel): unshifted f32 sums lose that variance to
+//    cancellation.  Every row slice shifts by the same row 0, so the partials still add.
+template <typename T, int MODE>
 __global__ void __launch_bounds__(128, 4) colstats_kernel(const T* __restrict__ x, const T* __restrict__ aux, long long rows, int C,
                                                        const float* __restrict__ mean, const float* __restrict__ rstd,
                                                        float* __restrict__ s1) {
@@ -86,11 +90,12 @@ __global__ void __launch_bounds__(128, 4) colstats_kernel(const T* __restrict__ 
     const long long r0 = (long long)blockIdx.y * rows_per;
     const long long r1 = min(rows, r0 + rows_per);
     float a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, b[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    float mu[8], rs[8];
+    float mu[8], rs[8], piv[8];
     if (MODE == 1) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) { mu[e] = mean[c0 + e]; rs[e] = rstd[c0 + e]; }
     }
+    if (MODE == 2) V8<T>::load(x + c0, piv);
     constexpr int UR = 8;                       // independent 16-byte loads in flight per thread
     long long r = r0;
     for (; r + UR <= r1; r += UR) {
@@ -104,8 +109,9 @@ __global__ void __launch_bounds__(128, 4) colstats_kernel(const T* __restrict__ 
         for (int k = 0; k < UR; ++k) {
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
+                if (MODE == 2) f[k][e] -= piv[e];
                 a[e] += f[k][e];
-                b[e] += (MODE == 0) ? f[k][e] * f[k][e] : f[k][e] * (g[k][e] - mu[e]) * rs[e];
+                b[e] += (MODE == 1) ? f[k][e] * (g[k][e] - mu[e]) * rs[e] : f[k][e] * f[k][e];
             }
         }
     }
@@ -115,8 +121,9 @@ __global__ void __launch_bounds__(128, 4) colstats_kernel(const T* __restrict__ 
         if (MODE == 1) V8<T>::load(aux + r * C + c0, g);
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
+            if (MODE == 2) f[e] -= piv[e];
             a[e] += f[e];
-            b[e] += (MODE == 0) ? f[e] * f[e] : f[e] * (g[e] - mu[e]) * rs[e];
+            b[e] += (MODE == 1) ? f[e] * (g[e] - mu[e]) * rs[e] : f[e] * f[e];
         }
     }
     // partial sums of this row-slice: part[(blockIdx.y * 2 + {0,1}) * C + c]
@@ -148,16 +155,19 @@ __global__ void __launch_bounds__(256) colstats_reduce_kernel(const float* __res
     }
 }
 
-// mean/rstd from (sum, sumsq); optional running-stat update (nn.BatchNorm1d, momentum 0.1, unbiased var)
-__global__ void bn_finalize_kernel(const float* __restrict__ s1, const float* __restrict__ s2, long long rows, int C, float eps,
-                                   float momentum, float* __restrict__ mean, float* __restrict__ rstd,
+// mean/rstd from the shifted sums of colstats MODE 2 (s1 = sum d, s2 = sum d^2, d = x - x[0,c]); optional running-stat update
+// (nn.BatchNorm1d: unbiased var, the caller's momentum)
+template <typename T>
+__global__ void bn_finalize_kernel(const T* __restrict__ x, const float* __restrict__ s1, const float* __restrict__ s2, long long rows,
+                                   int C, float eps, float momentum, float* __restrict__ mean, float* __restrict__ rstd,
                                    float* __restrict__ run_mean, float* __restrict__ run_var) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     const float n = (float)rows;
-    const float m = s1[c] / n;
-    float var = s2[c] / n - m * m;
+    const float d = s1[c] / n;                                  // mean - x[0,c]
+    float var = s2[c] / n - d * d;
     var = fmaxf(var, 0.f);
+    const float m = to_f32<T>(x[c]) + d;
     mean[c] = m;
     rstd[c] = rsqrtf(var + eps);
     if (run_mean) {
@@ -281,7 +291,7 @@ static inline dim3 col_grid(long long rows, int C) {
     return dim3(gx, (unsigned)gy);
 }
 
-// =============================================================================== LayerNorm (C <= 8192, C % 8 == 0)
+// =============================================================================== LayerNorm (C <= 1024, C % 8 == 0)
 // one warp per row
 template <typename T>
 __global__ void __launch_bounds__(256) ln_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, long long rows, int C,
@@ -1218,16 +1228,23 @@ extern "C" int pk_cast_split(const void* src, int src_dtype, long long ld_src, v
     DONE();
 }
 
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 /* BatchNorm1d over rows of x [rows, C].  stats_ws: pk_colstats_ws_floats(C) + 2*C floats of scratch. */
 extern "C" int pk_bn_fwd(const void* x, void* y, int dtype, long long rows, int C, const float* w, const float* b, float eps,
                          int train, float momentum, float* run_mean, float* run_var, float* mean, float* rstd, float* stats_ws,
                          void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8 and rows > 0");
+    PK_CHECK_ARG(aligned16(x) && aligned16(y) && (!train || aligned16(stats_ws)), "pk_bn_fwd: x, y, stats_ws must be 16-byte aligned");
     cudaStream_t st = STREAM(stream);
     if (train) {
         float* sums = stats_ws + pk_colstats_ws_floats(C);
-        PK_DISPATCH_T(dtype, { int rc = run_colstats<T, 0>((const T*)x, nullptr, rows, C, nullptr, nullptr, stats_ws, sums, sums + C, st); if (rc) return rc; });
-        bn_finalize_kernel<<<(C + 255) / 256, 256, 0, st>>>(sums, sums + C, rows, C, eps, momentum, mean, rstd, run_mean, run_var);
+        PK_DISPATCH_T(dtype, {
+            int rc = run_colstats<T, 2>((const T*)x, nullptr, rows, C, nullptr, nullptr, stats_ws, sums, sums + C, st);
+            if (rc) return rc;
+            bn_finalize_kernel<T><<<(C + 255) / 256, 256, 0, st>>>((const T*)x, sums, sums + C, rows, C, eps, momentum, mean, rstd, run_mean,
+                                                                 run_var);
+        });
     } else {
         bn_eval_stats_kernel<<<(C + 255) / 256, 256, 0, st>>>(run_mean, run_var, C, eps, mean, rstd);
     }
@@ -1240,7 +1257,8 @@ extern "C" int pk_bn_fwd(const void* x, void* y, int dtype, long long rows, int 
 extern "C" int pk_bn_bwd(const void* dy, const void* x, void* dx, int dtype, long long rows, int C, const float* w,
                          const float* mean, const float* rstd, int train, int relu_mask, float* dw, float* db, float* ws,
                          void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8 and rows > 0");
+    PK_CHECK_ARG(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned16(ws), "pk_bn_bwd: dy, x, dx, ws must be 16-byte aligned");
     cudaStream_t st = STREAM(stream);
     PK_DISPATCH_T(dtype, { int rc = run_colstats<T, 1>((const T*)dy, (const T*)x, rows, C, mean, rstd, ws, db, dw, st); if (rc) return rc; });
     PK_DISPATCH_T(dtype, (bn_bwd_apply_kernel<T><<<col_grid(rows, C), 128, 0, st>>>((const T*)dy, (const T*)x, (T*)dx, rows, C, mean, rstd, w,
@@ -1249,7 +1267,8 @@ extern "C" int pk_bn_bwd(const void* dy, const void* x, void* dx, int dtype, lon
 }
 
 extern "C" int pk_colsum(const void* x, int dtype, long long rows, int C, float* out, float* ws, void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8 and rows > 0");
+    PK_CHECK_ARG(aligned16(x) && aligned16(ws), "pk_colsum: x, ws must be 16-byte aligned");
     cudaStream_t st = STREAM(stream);
     PK_DISPATCH_T(dtype, { int rc = run_colstats<T, 0>((const T*)x, nullptr, rows, C, nullptr, nullptr, ws, out, nullptr, st); if (rc) return rc; });
     return 0;
@@ -1257,14 +1276,16 @@ extern "C" int pk_colsum(const void* x, int dtype, long long rows, int C, float*
 
 extern "C" int pk_layernorm_fwd(const void* x, void* y, int dtype, long long rows, int C, const float* w, const float* b, float eps,
                                 float* mean, float* rstd, void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0 && C <= 1024, "C must be a multiple of 8, <= 1024");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0 && C <= 1024, "C must be a multiple of 8, <= 1024, and rows > 0");
+    PK_CHECK_ARG(aligned16(x) && aligned16(y), "pk_layernorm_fwd: x, y must be 16-byte aligned");
     const int grid = grid_for(rows, 8);
     PK_DISPATCH_T(dtype, (ln_fwd_kernel<T><<<grid, 256, 0, STREAM(stream)>>>((const T*)x, (T*)y, rows, C, w, b, eps, mean, rstd)));
     DONE();
 }
 extern "C" int pk_layernorm_bwd(const void* dy, const void* x, void* dx, int dtype, long long rows, int C, const float* w,
                                 const float* mean, const float* rstd, float* dw, float* db, void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0 && C <= 1024, "C must be a multiple of 8, <= 1024");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0 && C <= 1024, "C must be a multiple of 8, <= 1024, and rows > 0");
+    PK_CHECK_ARG(aligned16(dy) && aligned16(x) && aligned16(dx), "pk_layernorm_bwd: dy, x, dx must be 16-byte aligned");
     cudaStream_t st = STREAM(stream);
     PK_CHECK_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * C, st));
     PK_CHECK_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * C, st));
@@ -1437,7 +1458,8 @@ extern "C" int pk_embedding_bwd(const long long* idx, const void* dout, int dtyp
 }
 
 extern "C" int pk_gather_rows(const void* src, const int* idx, void* dst, int dtype, long long rows, int C, void* stream) {
-    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8");
+    PK_CHECK_ARG(C % 8 == 0 && rows > 0, "C must be a multiple of 8 and rows > 0");
+    PK_CHECK_ARG(aligned16(src) && aligned16(dst), "pk_gather_rows: src, dst must be 16-byte aligned");
     PK_DISPATCH_T(dtype, (gather_rows_kernel<T><<<(unsigned)rows, 128, 0, STREAM(stream)>>>((const T*)src, idx, (T*)dst, rows, C)));
     DONE();
 }

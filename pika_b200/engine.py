@@ -391,10 +391,12 @@ class BatchNormFn(torch.autograd.Function):
         mean = torch.empty(C, dtype=torch.float32, device=x.device)
         rstd = torch.empty_like(mean)
         ws = torch.empty(2 * C, dtype=torch.float32, device=x.device)
-        K.bn_fwd(x, y, bn.weight.detach(), bn.bias.detach(), bn.eps, train, bn.momentum if bn.momentum is not None else 0.1,
-                 bn.running_mean, bn.running_var, mean, rstd, ws)
         if train and bn.num_batches_tracked is not None:
             bn.num_batches_tracked += 1
+        momentum = bn.momentum
+        if momentum is None:            # nn.BatchNorm1d's cumulative average: 1 / num_batches_tracked after the increment (a host read)
+            momentum = 1.0 / float(bn.num_batches_tracked) if train and bn.num_batches_tracked is not None else 0.0
+        K.bn_fwd(x, y, bn.weight.detach(), bn.bias.detach(), bn.eps, train, momentum, bn.running_mean, bn.running_var, mean, rstd, ws)
         ctx.save_for_backward(x, mean, rstd)
         ctx.bn, ctx.train = bn, train
         return y
