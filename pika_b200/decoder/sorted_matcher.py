@@ -10,17 +10,12 @@ update, final costs) runs inside ``pk_beam_advance_lm`` (pika_b200/csrc/beam.cu)
 ``arcs(state)`` (iterable of arcs with ``ilabel``, ``weight.value``, ``nextstate``) and ``final(state).value`` -- or a ready
 ``(arcs, finals)`` pair: ``arcs[state]`` = list of ``(ilabel, weight, nextstate)``, ``finals[state]`` = cost (inf = not final).
 """
-import ctypes
 import math
 
 import numpy as np
 import torch
 
-
-class LmFst(ctypes.Structure):
-    _fields_ = [("arc_off", ctypes.c_void_p), ("arc_ilabel", ctypes.c_void_p), ("arc_weight", ctypes.c_void_p),
-                ("arc_next", ctypes.c_void_p), ("finals", ctypes.c_void_p), ("backoff_id", ctypes.c_int),
-                ("n_disambig", ctypes.c_int), ("disambig_ids", ctypes.c_int * 4)]
+from .._lib import LmFst
 
 
 class SortedMatcher(object):

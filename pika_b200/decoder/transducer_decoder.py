@@ -18,7 +18,6 @@ The back-pointers are walked once at the end (decoder/transducer_decoder.py:204-
 Like the reference, every utterance keeps advancing until ALL utterances of the batch are done, so late
 finishes can still enter an utterance's n-best list.
 """
-import ctypes
 import os
 
 import numpy as np
@@ -27,7 +26,7 @@ import torch
 from .. import engine
 from .. import kernels as K
 from .. import _lib
-from .._lib import PikaError, check, lib
+from .._lib import BeamXfState, PikaError, check, lib
 
 _USE_GRAPH = os.environ.get("PK_DECODE_GRAPH", "1") != "0"      # 0: issue every launch of the beam loop from the host (debugging)
 _POLL = 4                                                        # graph replays (= 8 beam steps) between looks at the done counter
@@ -174,9 +173,9 @@ class _XfBuffers:
         self.rel = [f32(*l.self_attn.relative_positions_embeddings.weight.shape) if getattr(l.self_attn, "max_relative_positions", 0) > 0
                     else None for l in pn.transformer]
         self.eps = [(l.layer_norm.eps, l.feed_forward.layer_norm.eps) for l in pn.transformer] + [pn.layer_norm.eps]
-        P = lambda t: t.data_ptr()                                                      # noqa: E731
-        self.st, self.st_init = (K.BeamXfState(P(ws.next_ys), P(ws.step_ctx), P(ws.hyp_tok), P(ws.hyp_len), P(self.slot), P(self.pool),
-                                               self.n_entries, dec.blk, rows, S + 1, self.layers, D, K._dt(self.pool), init)
+        P = K._P
+        self.st, self.st_init = (BeamXfState(P(ws.next_ys), P(ws.step_ctx), P(ws.hyp_tok), P(ws.hyp_len), P(self.slot), P(self.pool),
+                                             self.n_entries, dec.blk, rows, S + 1, self.layers, D, K._dt(self.pool), init)
                                  for init in (0, 1))
 
     def stage(self, dec):
@@ -294,17 +293,16 @@ class TransducerDecoder():
         check(lib.pk_beam_gate(P(ws.pre), P(ws.hj), K._dt(ws.hj), rows, H, st()), "pk_beam_gate")
         engine.gemm_parts([engine.stage_act(ws.hj)], [ws.w2], ws.logits[:, :V], bias=ws.b2)
         # log_softmax(sm_scale * logits) is not materialised: one pass leaves the row log-sum-exp, pk_beam_advance forms the log-probs
-        check(lib.pk_row_lse(P(ws.logits), K._dt(ws.logits), ctypes.c_longlong(ws.ldv), P(ws.row_lse), ctypes.c_longlong(rows), V,
-                             ctypes.c_float(self.sm_scale), st()), "pk_row_lse")
-        common = (P(ws.logits), ws.ldv, P(ws.row_lse), ctypes.c_float(self.sm_scale), P(t_idx), P(ws.nf), P(ws.ml), P(ws.scores), P(ws.next_ys), P(ws.prev_ks), P(ws.hyp_tok), P(ws.hyp_len),
+        check(lib.pk_row_lse(P(ws.logits), K._dt(ws.logits), ws.ldv, P(ws.row_lse), rows, V, self.sm_scale, st()), "pk_row_lse")
+        common = (P(ws.logits), ws.ldv, P(ws.row_lse), self.sm_scale, P(t_idx), P(ws.nf), P(ws.ml), P(ws.scores), P(ws.next_ys), P(ws.prev_ks), P(ws.hyp_tok), P(ws.hyp_len),
                   P(ws.fin_score), P(ws.fin_step), P(ws.fin_k), P(ws.fin_count), P(ws.eos_top), P(ws.done), P(ws.not_done), ws.B, Kb, V,
                   ws.Scap + 1, ws.cap, P(ws.step_ctx), blk, self.n_best, int(bool(self.beam_prune)))
         if ws.lm is None:
             check(lib.pk_beam_advance(*common, st()), "pk_beam_advance")
         else:
             lm = ws.lm
-            check(lib.pk_beam_advance_lm(*common, ctypes.byref(lm["fst"]), ctypes.c_double(self.lm_scorer_scale),
-                                         ctypes.c_double(float(getattr(self.args, "nonblk_reward", 0.0))), P(lm["set_state"]), P(lm["set_cost"]),
+            check(lib.pk_beam_advance_lm(*common, lm["fst"], self.lm_scorer_scale,
+                                         float(getattr(self.args, "nonblk_reward", 0.0)), P(lm["set_state"]), P(lm["set_cost"]),
                                          P(lm["set_n"]), P(lm["lm_scores"]), self.lm_max_states, P(lm["err"]), st()), "pk_beam_advance_lm")
         if self.xf:
             K.beam_xf_slots(ws.xf.st, ws.prev_ks, Kb)

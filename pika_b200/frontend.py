@@ -4,7 +4,6 @@ Replaces the CPU chain of loader/otf_utt_loader.py:218-250 (AudioSegment augment
 Fbank -> splice) plus trainer/train_transducer_bmuf_otfaug.py:86-93 (CMN/CMVN, SpecAugment).
 Feature options are Kaldi's, read from a Kaldi-style config file such as egs/fbank.conf.
 """
-import ctypes
 import math
 
 import numpy as np
@@ -125,12 +124,11 @@ class Frontend:
         wave = torch.zeros(B, n_max, dtype=torch.int16, device=self.device) if want_wave else None
         P = K._P
         f0, fs, t0, ts = specaug
-        args = (P(pcm), ctypes.c_longlong(pcm.stride(0)), P(n_samples), P(rate), P(new_len), P(target_db),
+        args = (P(pcm), pcm.stride(0), P(n_samples), P(rate), P(new_len), P(target_db),
                 P(n_frames), B, n_max, t_max, self.n_mel, self.lctx, self.rctx, P(self.window), P(self.twiddle),
-                P(self.mel_w), P(self.mel_lo), P(self.mel_hi), ctypes.c_float(self.opts.preemphasis_coefficient),
+                P(self.mel_w), P(self.mel_lo), P(self.mel_hi), self.opts.preemphasis_coefficient,
                 int(cmn), P(offset), P(scale), int(f0), int(fs), int(t0), int(ts), P(out), K._dt(out), P(wave),
-                P(self._ws), ctypes.c_longlong(need), P(self.err), ctypes.c_float(self.opts.dither),
-                ctypes.c_uint32(self._next_dither_seed()), K._stream())
+                P(self._ws), need, P(self.err), self.opts.dither, self._next_dither_seed(), K._stream())
         if not aug:
             check(lib.pk_frontend_fwd(*args), "pk_frontend_fwd")
             return (out, wave) if want_wave else out
@@ -172,8 +170,8 @@ class Frontend:
         B = wave_f32.shape[0]
         feats = torch.zeros(B, t_max, self.n_mel, dtype=torch.float32, device=self.device)
         P = K._P
-        check(lib.pk_fbank(P(wave_f32), ctypes.c_longlong(wave_f32.stride(0)), P(n_frames), B, t_max, self.n_mel, P(self.window),
-                           P(self.twiddle), P(self.mel_w), P(self.mel_lo), P(self.mel_hi),
-                           ctypes.c_float(self.opts.preemphasis_coefficient), P(feats), ctypes.c_float(self.opts.dither if dither is None else dither),
-                           ctypes.c_uint32(self._next_dither_seed() if seed is None else seed), K._stream()), "pk_fbank")
+        check(lib.pk_fbank(P(wave_f32), wave_f32.stride(0), P(n_frames), B, t_max, self.n_mel, P(self.window),
+                           P(self.twiddle), P(self.mel_w), P(self.mel_lo), P(self.mel_hi), self.opts.preemphasis_coefficient, P(feats),
+                           self.opts.dither if dither is None else dither,
+                           (self._next_dither_seed() if seed is None else seed) & 0xFFFFFFFF, K._stream()), "pk_fbank")
         return feats

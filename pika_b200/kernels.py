@@ -2,8 +2,6 @@
 
 torch is used here only for device memory, streams and shape bookkeeping.
 """
-import ctypes
-
 import torch
 
 from . import _lib
@@ -12,7 +10,7 @@ from ._lib import (ACT_NONE, ACT_RELU, AUX_ADD, AUX_MASK_NZ, AUX_NONE, PK_BF16, 
 
 
 def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _dt(t):
@@ -23,8 +21,9 @@ def _dt(t):
     raise TypeError("unsupported dtype %s" % t.dtype)
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+def _P(t):
+    """a tensor's device address, or NULL for None"""
+    return t.data_ptr() if t is not None else None
 
 
 def _fill_view(v, t):
@@ -92,7 +91,7 @@ def gemm(a, b, c, a_mn=False, b_mn=False, a_sel=(SEL_ZB0, SEL_ZB1), b_sel=(SEL_Z
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and c.dim() == 2
         assert tuple(row_lse.shape) == (row_lse_parts(c.shape[-2], c.shape[-1], block_n), c.shape[-2], 2)
         d.row_lse = row_lse.data_ptr()
-    check(lib.pk_gemm_bf16(ctypes.byref(d), _stream()), "pk_gemm_bf16")
+    check(lib.pk_gemm_bf16(d, _stream()), "pk_gemm_bf16")
     return c
 
 
@@ -119,25 +118,20 @@ def rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=None, grad_scale
         dlogits = torch.empty_like(logits)
     if row_lse is not None:
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (B * T * U1, 2)
-        check(lib.pk_rnnt_loss_fwd_bwd_lse(_ptr(logits), _dt(logits), _ptr(labels), _ptr(frame_lens), _ptr(label_lens),
-                                           B, T, U1, V, ldv, max(labels.stride(0), 1), _ptr(grad_scale), _ptr(costs),
-                                           _ptr(dlogits if want_grad else None), _ptr(colsum), _ptr(ws), ws_bytes,
-                                           _ptr(row_lse), int(row_lse.shape[0]), _stream()), "pk_rnnt_loss_fwd_bwd_lse")
+        check(lib.pk_rnnt_loss_fwd_bwd_lse(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens),
+                                           B, T, U1, V, ldv, max(labels.stride(0), 1), _P(grad_scale), _P(costs),
+                                           _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes,
+                                           _P(row_lse), int(row_lse.shape[0]), _stream()), "pk_rnnt_loss_fwd_bwd_lse")
         return costs, dlogits
-    check(lib.pk_rnnt_loss_fwd_bwd(_ptr(logits), _dt(logits), _ptr(labels), _ptr(frame_lens), _ptr(label_lens),
-                                   B, T, U1, V, ldv, max(labels.stride(0), 1), _ptr(grad_scale), _ptr(costs),
-                                   _ptr(dlogits if want_grad else None), _ptr(colsum), _ptr(ws), ws_bytes, _stream()),
+    check(lib.pk_rnnt_loss_fwd_bwd(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens),
+                                   B, T, U1, V, ldv, max(labels.stride(0), 1), _P(grad_scale), _P(costs),
+                                   _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes, _stream()),
           "pk_rnnt_loss_fwd_bwd")
     return costs, dlogits
 
 
 # ------------------------------------------------------------------------------------------------
-# thin wrappers for the memory-bound kernels (argument marshalling only)
-_P = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
-_L = ctypes.c_longlong
-_I = ctypes.c_int
-_F = ctypes.c_float
-_U = ctypes.c_uint32
+# thin wrappers for the memory-bound kernels
 
 
 def cast_split(src, hi, lo=None, cols_pad=None, scale=1.0):
@@ -145,8 +139,8 @@ def cast_split(src, hi, lo=None, cols_pad=None, scale=1.0):
     rows, cols = src.shape
     cols_pad = cols_pad or cols
     assert hi.shape[-1] == cols_pad and hi.stride(-1) == 1 and src.stride(-1) == 1
-    check(lib.pk_cast_split(_P(src), _I(_dt(src)), _L(src.stride(0)), _P(hi), _P(lo), _L(hi.stride(0)), _L(rows),
-                            _I(cols), _I(cols_pad), _F(scale), _stream()), "pk_cast_split")
+    check(lib.pk_cast_split(_P(src), _dt(src), src.stride(0), _P(hi), _P(lo), hi.stride(0), rows, cols, cols_pad, scale, _stream()),
+          "pk_cast_split")
 
 
 def attention_lse_stride(T):
@@ -169,9 +163,7 @@ def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0, keep_bits=Non
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and out.is_contiguous() and out.shape == (B, T, D)
     assert lse.dtype == torch.float32 and lse.numel() == B * heads * attention_lse_stride(T)
     base, es = qkv.data_ptr(), 2
-    vp = ctypes.c_void_p
-    args = (vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(lse), _I(B), _I(T), _I(heads), _I(D // heads),
-            _F(alpha), _F(drop_p), _U(seed & 0xFFFFFFFF))
+    args = (base, base + D * es, base + 2 * D * es, D3, _P(out), D, _P(lse), B, T, heads, D // heads, alpha, drop_p, seed & 0xFFFFFFFF)
     if keep_bits is None:
         check(lib.pk_attention_fwd(*args, _stream()), "pk_attention_fwd")
         return
@@ -186,11 +178,10 @@ def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0, k
     assert dout.is_contiguous() and dqkv.is_contiguous() and dqkv.shape == qkv.shape and dout.dtype == torch.bfloat16
     ws = torch.zeros(B * heads * attention_lse_stride(T), dtype=torch.float32, device=qkv.device)     # D scratch (the kernel writes its padding too)
     base, gb, es = qkv.data_ptr(), dqkv.data_ptr(), 2
-    vp = ctypes.c_void_p
-    args = (vp(base), vp(base + D * es), vp(base + 2 * D * es), _L(D3), _P(out), _L(D), _P(dout), _L(D), _P(lse), _P(ws),
-            vp(gb), vp(gb + D * es), vp(gb + 2 * D * es), _L(D3), _I(B), _I(T), _I(heads), _I(D // heads), _F(alpha), _F(drop_p))
+    args = (base, base + D * es, base + 2 * D * es, D3, _P(out), D, _P(dout), D, _P(lse), _P(ws),
+            gb, gb + D * es, gb + 2 * D * es, D3, B, T, heads, D // heads, alpha, drop_p)
     if keep_bits is None:
-        check(lib.pk_attention_bwd(*args, _U(seed & 0xFFFFFFFF), _stream()), "pk_attention_bwd")
+        check(lib.pk_attention_bwd(*args, seed & 0xFFFFFFFF, _stream()), "pk_attention_bwd")
     else:
         check(lib.pk_attention_bwd_bits(*args, _P(keep_bits), _stream()), "pk_attention_bwd_bits")
 
@@ -202,7 +193,6 @@ def col_ws(C, device):
     """persistent scratch for the two-stage column reductions (per device, per C)"""
     key = (C, str(device))
     if key not in _col_ws:
-        lib.pk_colstats_ws_floats.restype = ctypes.c_longlong
         _col_ws[key] = torch.empty(int(lib.pk_colstats_ws_floats(C)) + 2 * C, dtype=torch.float32, device=device)
     return _col_ws[key]
 
@@ -210,38 +200,37 @@ def col_ws(C, device):
 def bn_fwd(x, y, w, b, eps, train, momentum, run_mean, run_var, mean, rstd, ws=None):
     rows, C = x.shape
     ws = col_ws(C, x.device)
-    check(lib.pk_bn_fwd(_P(x), _P(y), _I(_dt(x)), _L(rows), _I(C), _P(w), _P(b), _F(eps), _I(int(train)), _F(momentum),
+    check(lib.pk_bn_fwd(_P(x), _P(y), _dt(x), rows, C, _P(w), _P(b), eps, int(train), momentum,
                         _P(run_mean), _P(run_var), _P(mean), _P(rstd), _P(ws), _stream()), "pk_bn_fwd")
 
 
 def bn_bwd(dy, x, dx, w, mean, rstd, train, relu_mask, dw, db):
     rows, C = x.shape
-    check(lib.pk_bn_bwd(_P(dy), _P(x), _P(dx), _I(_dt(x)), _L(rows), _I(C), _P(w), _P(mean), _P(rstd), _I(int(train)),
-                        _I(int(relu_mask)), _P(dw), _P(db), _P(col_ws(C, x.device)), _stream()), "pk_bn_bwd")
+    check(lib.pk_bn_bwd(_P(dy), _P(x), _P(dx), _dt(x), rows, C, _P(w), _P(mean), _P(rstd), int(train),
+                        int(relu_mask), _P(dw), _P(db), _P(col_ws(C, x.device)), _stream()), "pk_bn_bwd")
 
 
 def colsum(x, out):
     rows, C = x.shape
     assert x.is_contiguous()
-    check(lib.pk_colsum(_P(x), _I(_dt(x)), _L(rows), _I(C), _P(out), _P(col_ws(C, x.device)), _stream()), "pk_colsum")
+    check(lib.pk_colsum(_P(x), _dt(x), rows, C, _P(out), _P(col_ws(C, x.device)), _stream()), "pk_colsum")
 
 
 def layernorm_fwd(x, y, w, b, eps, mean, rstd):
     rows, C = x.shape
-    check(lib.pk_layernorm_fwd(_P(x), _P(y), _I(_dt(x)), _L(rows), _I(C), _P(w), _P(b), _F(eps), _P(mean), _P(rstd),
-                               _stream()), "pk_layernorm_fwd")
+    check(lib.pk_layernorm_fwd(_P(x), _P(y), _dt(x), rows, C, _P(w), _P(b), eps, _P(mean), _P(rstd), _stream()), "pk_layernorm_fwd")
 
 
 def layernorm_bwd(dy, x, dx, w, mean, rstd, dw, db):
     rows, C = x.shape
-    check(lib.pk_layernorm_bwd(_P(dy), _P(x), _P(dx), _I(_dt(x)), _L(rows), _I(C), _P(w), _P(mean), _P(rstd), _P(dw),
-                               _P(db), _stream()), "pk_layernorm_bwd")
+    check(lib.pk_layernorm_bwd(_P(dy), _P(x), _P(dx), _dt(x), rows, C, _P(w), _P(mean), _P(rstd), _P(dw), _P(db), _stream()),
+          "pk_layernorm_bwd")
 
 
 def softmax_fwd(S, P, Pd, n, drop_p, seed):
     rows = S.numel() // S.shape[-1]
-    check(lib.pk_softmax_fwd(_P(S), _L(S.shape[-1]), _P(P), _P(Pd), _I(_dt(P)), _L(P.shape[-1]), _L(rows), _I(n),
-                             _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_softmax_fwd")
+    check(lib.pk_softmax_fwd(_P(S), S.shape[-1], _P(P), _P(Pd), _dt(P), P.shape[-1], rows, n, drop_p, seed & 0xFFFFFFFF, _stream()),
+          "pk_softmax_fwd")
 
 
 def softmax_masked_fwd(S, P, Pd, n, q_len, heads, causal, key_pad, drop_p, seed):
@@ -249,15 +238,14 @@ def softmax_masked_fwd(S, P, Pd, n, q_len, heads, causal, key_pad, drop_p, seed)
     rows = S.numel() // S.shape[-1]
     if key_pad is not None:
         assert key_pad.dtype == torch.uint8 and key_pad.is_contiguous() and key_pad.shape[-1] == n
-    check(lib.pk_softmax_masked_fwd(_P(S), _L(S.shape[-1]), _P(P), _P(Pd), _I(_dt(P)), _L(P.shape[-1]), _L(rows), _I(n), _I(q_len),
-                                    _I(heads), _I(int(bool(causal))), _P(key_pad), _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()),
-          "pk_softmax_masked_fwd")
+    check(lib.pk_softmax_masked_fwd(_P(S), S.shape[-1], _P(P), _P(Pd), _dt(P), P.shape[-1], rows, n, q_len, heads, int(bool(causal)),
+                                    _P(key_pad), drop_p, seed & 0xFFFFFFFF, _stream()), "pk_softmax_masked_fwd")
 
 
 def softmax_bwd(dPd, P, dS, n, drop_p, seed):
     rows = P.numel() // P.shape[-1]
-    check(lib.pk_softmax_bwd(_P(dPd), _L(dPd.shape[-1]), _P(P), _L(P.shape[-1]), _P(dS), _I(_dt(P)), _L(rows), _I(n),
-                             _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_softmax_bwd")
+    check(lib.pk_softmax_bwd(_P(dPd), dPd.shape[-1], _P(P), P.shape[-1], _P(dS), _dt(P), rows, n, drop_p, seed & 0xFFFFFFFF, _stream()),
+          "pk_softmax_bwd")
 
 
 def softmax_masked_relpos_fwd(S, QR, P, Pd, Pb, n, heads, causal, key_pad, max_rel, drop_p, seed):
@@ -267,88 +255,82 @@ def softmax_masked_relpos_fwd(S, QR, P, Pd, Pb, n, heads, causal, key_pad, max_r
     if key_pad is not None:
         assert key_pad.dtype == torch.uint8 and key_pad.is_contiguous() and key_pad.shape[-1] == n
     assert QR.dtype == torch.float32 and Pb.dtype == torch.float32 and QR.stride(-1) == 1 and Pb.stride() == QR.stride()
-    check(lib.pk_softmax_masked_relpos_fwd(_P(S), _L(S.shape[-1]), _P(QR), _L(QR.stride(0)), _P(P), _P(Pd), _I(_dt(P)), _L(P.shape[-1]),
-                                           _L(rows), _I(n), _I(n), _I(heads), _I(int(bool(causal))), _P(key_pad), _I(max_rel), _P(Pb),
-                                           _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()), "pk_softmax_masked_relpos_fwd")
+    check(lib.pk_softmax_masked_relpos_fwd(_P(S), S.shape[-1], _P(QR), QR.stride(0), _P(P), _P(Pd), _dt(P), P.shape[-1],
+                                           rows, n, n, heads, int(bool(causal)), _P(key_pad), max_rel, _P(Pb),
+                                           drop_p, seed & 0xFFFFFFFF, _stream()), "pk_softmax_masked_relpos_fwd")
 
 
 def softmax_relpos_bwd(dPd, G, P, dS, dSb, n, heads, max_rel, drop_p, seed):
     """pk_softmax_bwd with the relative-position value terms G = dO R^T added along the band; writes the bucket sums dSb of dS"""
     rows = P.numel() // P.shape[-1]
     assert G.dtype == torch.float32 and dSb.dtype == torch.float32 and G.stride(-1) == 1 and dSb.stride() == G.stride()
-    check(lib.pk_softmax_relpos_bwd(_P(dPd), _L(dPd.shape[-1]), _P(G), _L(G.stride(0)), _P(P), _L(P.shape[-1]), _P(dS), _I(_dt(P)),
-                                    _L(rows), _I(n), _I(n), _I(heads), _I(max_rel), _P(dSb), _F(drop_p), _U(seed & 0xFFFFFFFF), _stream()),
+    check(lib.pk_softmax_relpos_bwd(_P(dPd), dPd.shape[-1], _P(G), G.stride(0), _P(P), P.shape[-1], _P(dS), _dt(P),
+                                    rows, n, n, heads, max_rel, _P(dSb), drop_p, seed & 0xFFFFFFFF, _stream()),
           "pk_softmax_relpos_bwd")
 
 
 def dropout(x, y, p, seed):
-    check(lib.pk_dropout(_P(x), _P(y), _I(_dt(x)), _L(x.numel()), _F(p), _U(seed & 0xFFFFFFFF), _stream()), "pk_dropout")
+    check(lib.pk_dropout(_P(x), _P(y), _dt(x), x.numel(), p, seed & 0xFFFFFFFF, _stream()), "pk_dropout")
 
 
 def mask_nz(dy, y, dx, scale):
-    check(lib.pk_mask_nz(_P(dy), _P(y), _P(dx), _I(_dt(y)), _L(y.numel()), _F(scale), _stream()), "pk_mask_nz")
+    check(lib.pk_mask_nz(_P(dy), _P(y), _P(dx), _dt(y), y.numel(), scale, _stream()), "pk_mask_nz")
 
 
 def add(a, b, o):
-    check(lib.pk_add(_P(a), _P(b), _P(o), _I(_dt(a)), _L(a.numel()), _stream()), "pk_add")
+    check(lib.pk_add(_P(a), _P(b), _P(o), _dt(a), a.numel(), _stream()), "pk_add")
 
 
 def log_softmax(x, y, n, scale=1.0):
     rows = x.numel() // x.shape[-1]
-    check(lib.pk_log_softmax(_P(x), _I(_dt(x)), _L(x.shape[-1]), _P(y), _L(rows), _I(n), _F(scale), _stream()),
-          "pk_log_softmax")
+    check(lib.pk_log_softmax(_P(x), _dt(x), x.shape[-1], _P(y), rows, n, scale, _stream()), "pk_log_softmax")
 
 
 def joint_gate_fwd(ex, py, h, B, T, U1, H):
-    check(lib.pk_joint_gate_fwd(_P(ex), _P(py), _P(h), _I(_dt(ex)), _I(B), _I(T), _I(U1), _I(H), _I(h.stride(0)), _stream()),
-          "pk_joint_gate_fwd")
+    check(lib.pk_joint_gate_fwd(_P(ex), _P(py), _P(h), _dt(ex), B, T, U1, H, h.stride(0), _stream()), "pk_joint_gate_fwd")
 
 
 def joint_gate_bwd(ex, py, dh, dex, dpy, B, T, U1, H):
-    check(lib.pk_joint_gate_bwd(_P(ex), _P(py), _P(dh), _P(dex), _P(dpy), _I(_dt(ex)), _I(B), _I(T), _I(U1), _I(H),
-                                _stream()), "pk_joint_gate_bwd")
+    check(lib.pk_joint_gate_bwd(_P(ex), _P(py), _P(dh), _P(dex), _P(dpy), _dt(ex), B, T, U1, H, _stream()), "pk_joint_gate_bwd")
 
 
 def lstm_cell_fwd(gx, gh, c_prev, c_out, h_out, gates_save, B, H):
-    check(lib.pk_lstm_cell_fwd(_P(gx), _L(gx.stride(0)), _P(gh), _L(gh.stride(0) if gh is not None else 0), _P(c_prev),
-                               _P(c_out), _P(h_out), _I(_dt(h_out)), _L(h_out.stride(0)), _P(gates_save), _I(B), _I(H),
-                               _stream()), "pk_lstm_cell_fwd")
+    check(lib.pk_lstm_cell_fwd(_P(gx), gx.stride(0), _P(gh), gh.stride(0) if gh is not None else 0, _P(c_prev), _P(c_out), _P(h_out),
+                               _dt(h_out), h_out.stride(0), _P(gates_save), B, H, _stream()), "pk_lstm_cell_fwd")
 
 
 def lstm_cell_bwd(dh_out, dh_rec, dc_next, gates, c, c_prev, dgates, dc_prev, B, H):
-    check(lib.pk_lstm_cell_bwd(_P(dh_out), _L(dh_out.stride(0) if dh_out is not None else 0), _P(dh_rec), _P(dc_next),
-                               _P(gates), _P(c), _P(c_prev), _P(dgates), _I(_dt(dgates)), _P(dc_prev), _I(B), _I(H),
-                               _stream()), "pk_lstm_cell_bwd")
+    check(lib.pk_lstm_cell_bwd(_P(dh_out), dh_out.stride(0) if dh_out is not None else 0, _P(dh_rec), _P(dc_next), _P(gates), _P(c),
+                               _P(c_prev), _P(dgates), _dt(dgates), _P(dc_prev), B, H, _stream()), "pk_lstm_cell_bwd")
 
 
 def embedding_fwd(idx, table, out):
     n, ld = out.shape
-    check(lib.pk_embedding_fwd(_P(idx), _P(table), _I(table.shape[1]), _P(out), _I(_dt(out)), _I(ld), _L(n), _stream()),
-          "pk_embedding_fwd")
+    check(lib.pk_embedding_fwd(_P(idx), _P(table), table.shape[1], _P(out), _dt(out), ld, n, _stream()), "pk_embedding_fwd")
 
 
 def embedding_bwd(idx, dout, dtable, padding_idx):
     n, ld = dout.shape
-    check(lib.pk_embedding_bwd(_P(idx), _P(dout), _I(_dt(dout)), _I(ld), _I(dtable.shape[1]), _P(dtable), _L(n),
-                               _L(padding_idx if padding_idx is not None else -1), _stream()), "pk_embedding_bwd")
+    check(lib.pk_embedding_bwd(_P(idx), _P(dout), _dt(dout), ld, dtable.shape[1], _P(dtable), n,
+                               padding_idx if padding_idx is not None else -1, _stream()), "pk_embedding_bwd")
 
 
 def absmax(x, out, nan_flag=None):
-    check(lib.pk_absmax(_P(x), _L(x.numel()), _P(out), _P(nan_flag), _stream()), "pk_absmax")
+    check(lib.pk_absmax(_P(x), x.numel(), _P(out), _P(nan_flag), _stream()), "pk_absmax")
 
 
 def sgd_nesterov_clip(p, g, buf, lr, momentum, max_norm, absmax_t, first, nan_flag=None):
-    check(lib.pk_sgd_nesterov_clip(_P(p), _P(g), _P(buf), _L(p.numel()), _F(lr), _F(momentum), _F(max_norm), _P(absmax_t),
-                                   _P(nan_flag), _I(int(first)), _stream()), "pk_sgd_nesterov_clip")
+    check(lib.pk_sgd_nesterov_clip(_P(p), _P(g), _P(buf), p.numel(), lr, momentum, max_norm, _P(absmax_t), _P(nan_flag), int(first),
+                                   _stream()), "pk_sgd_nesterov_clip")
 
 
 def bmuf_delta(glob, local, delta):
-    check(lib.pk_bmuf_delta(_P(glob), _P(local), _P(delta), _L(glob.numel()), _stream()), "pk_bmuf_delta")
+    check(lib.pk_bmuf_delta(_P(glob), _P(local), _P(delta), glob.numel(), _stream()), "pk_bmuf_delta")
 
 
 def bmuf_update(glob, local, delta_prev, delta_sum, world, bm, blr):
-    check(lib.pk_bmuf_update(_P(glob), _P(local), _P(delta_prev), _P(delta_sum), _L(glob.numel()), _I(world), _F(bm), _F(blr),
-                             _stream()), "pk_bmuf_update")
+    check(lib.pk_bmuf_update(_P(glob), _P(local), _P(delta_prev), _P(delta_sum), glob.numel(), world, bm, blr, _stream()),
+          "pk_bmuf_update")
 
 
 def adam_clip(p, g, exp_avg, exp_avg_sq, lr, betas, eps, step, max_norm=-1.0, absmax_t=None, nan_flag=None, p_out2=None):
@@ -379,15 +361,12 @@ _lstm_ws = {}
 def _lstm_scratch(H, device):
     key = (H, str(device))
     if key not in _lstm_ws:
-        lib.pk_lstm_seq_workspace_bytes.restype = ctypes.c_longlong
         _lstm_ws[key] = torch.zeros(int(lib.pk_lstm_seq_workspace_bytes(H)), dtype=torch.uint8, device=device)
     return _lstm_ws[key]
 
 
 def _lens_arg(lens, B):
-    if lens is None:
-        return ctypes.c_void_p(0)
-    assert lens.dtype == torch.int32 and lens.is_contiguous() and lens.numel() == B
+    assert lens is None or (lens.dtype == torch.int32 and lens.is_contiguous() and lens.numel() == B)
     return _P(lens)
 
 
@@ -398,8 +377,8 @@ def lstm_seq_fwd_ex(gx, w_hh, out, gates_save, cs, lens=None, reverse=False):
     H = G4 // 4
     assert gx.is_contiguous() and w_hh.dtype == torch.bfloat16 and w_hh.is_contiguous() and w_hh.shape[0] == n_dir * G4
     assert out.stride(2) == 1 and out.stride(0) == U * out.stride(1) and out.shape[-1] == n_dir * H
-    check(lib.pk_lstm_seq_fwd_ex(_P(gx), _P(w_hh), _P(out), _I(_dt(out)), _I(out.stride(1)), _P(gates_save), _P(cs), _lens_arg(lens, B),
-                                 _I(B), _I(U), _I(H), _I(n_dir), _I(int(reverse)), _P(_lstm_scratch(n_dir * H, gx.device)), _stream()),
+    check(lib.pk_lstm_seq_fwd_ex(_P(gx), _P(w_hh), _P(out), _dt(out), out.stride(1), _P(gates_save), _P(cs), _lens_arg(lens, B),
+                                 B, U, H, n_dir, int(reverse), _P(_lstm_scratch(n_dir * H, gx.device)), _stream()),
           "pk_lstm_seq_fwd_ex")
 
 
@@ -409,55 +388,47 @@ def lstm_seq_bwd_ex(dout, gates_save, cs, w_hh, dG, lens=None, reverse=False):
     H = G4 // 4
     assert dout.stride(2) == 1 and dout.stride(0) == U * dout.stride(1) and dout.shape[-1] == n_dir * H
     assert dG.dtype == torch.bfloat16 and dG.is_contiguous() and w_hh.shape[0] == n_dir * G4
-    check(lib.pk_lstm_seq_bwd_ex(_P(dout), _I(_dt(dout)), _I(dout.stride(1)), _P(gates_save), _P(cs), _P(w_hh), _P(dG), _lens_arg(lens, B),
-                                 _I(B), _I(U), _I(H), _I(n_dir), _I(int(reverse)), _P(_lstm_scratch(n_dir * H, dout.device)), _stream()),
+    check(lib.pk_lstm_seq_bwd_ex(_P(dout), _dt(dout), dout.stride(1), _P(gates_save), _P(cs), _P(w_hh), _P(dG), _lens_arg(lens, B),
+                                 B, U, H, n_dir, int(reverse), _P(_lstm_scratch(n_dir * H, dout.device)), _stream()),
           "pk_lstm_seq_bwd_ex")
 
 
 def gather_rows(src, idx, dst):
     rows, C = dst.shape
-    check(lib.pk_gather_rows(_P(src), _P(idx), _P(dst), _I(_dt(src)), _L(rows), _I(C), _stream()), "pk_gather_rows")
+    check(lib.pk_gather_rows(_P(src), _P(idx), _P(dst), _dt(src), rows, C, _stream()), "pk_gather_rows")
 
 
 def scatter_add_rows(src, idx, dst):
     rows, C = src.shape
     assert dst.dtype == torch.float32
-    check(lib.pk_scatter_add_rows(_P(src), _P(idx), _P(dst), _I(_dt(src)), _L(rows), _I(C), _stream()), "pk_scatter_add_rows")
-
-
-class BeamXfState(ctypes.Structure):
-    """pk_beam_xf_state (include/pika_b200.h): the device buffers of the transformer prediction net's incremental beam step"""
-    _fields_ = [("next_ys", ctypes.c_void_p), ("step_ctx", ctypes.c_void_p), ("hyp_tok", ctypes.c_void_p), ("hyp_len", ctypes.c_void_p),
-                ("slot", ctypes.c_void_p), ("pool", ctypes.c_void_p), ("n_entries", ctypes.c_longlong), ("blk", ctypes.c_int),
-                ("rows", ctypes.c_int), ("S1", ctypes.c_int), ("layers", ctypes.c_int), ("D", ctypes.c_int), ("dtype", ctypes.c_int),
-                ("init", ctypes.c_int)]
+    check(lib.pk_scatter_add_rows(_P(src), _P(idx), _P(dst), _dt(src), rows, C, _stream()), "pk_scatter_add_rows")
 
 
 def beam_xf_taps(st, layer, embed, x_cur, taps):
     """taps [rows, 5 * ldc]: the causal conv's im2col row of every row's new position (layer 0: embedding rows of ``embed`` f32)"""
     assert embed.dtype == torch.float32 and embed.is_contiguous() and taps.is_contiguous()
-    check(lib.pk_beam_xf_taps(ctypes.byref(st), _I(layer), _P(embed), _I(embed.shape[1]), _P(x_cur), _P(taps), _I(taps.shape[1] // 5),
+    check(lib.pk_beam_xf_taps(st, layer, _P(embed), embed.shape[1], _P(x_cur), _P(taps), taps.shape[1] // 5,
                               _stream()), "pk_beam_xf_taps")
 
 
 def beam_xf_attn(st, layer, qkv, heads, rel, out):
     """qkv [rows, 3D] -> out [rows, D]: single-query attention over each row's cached positions; rel: f32 [2m+1, 64] or None"""
     assert qkv.is_contiguous() and out.is_contiguous() and (rel is None or (rel.dtype == torch.float32 and rel.is_contiguous()))
-    check(lib.pk_beam_xf_attn(ctypes.byref(st), _I(layer), _P(qkv), _I(heads), _P(rel), _I(0 if rel is None else rel.shape[0] // 2), _P(out),
+    check(lib.pk_beam_xf_attn(st, layer, _P(qkv), heads, _P(rel), 0 if rel is None else rel.shape[0] // 2, _P(out),
                               _stream()), "pk_beam_xf_attn")
 
 
 def beam_xf_select(st, x, h):
-    check(lib.pk_beam_xf_select(ctypes.byref(st), _P(x), _P(h), _I(h.shape[-1]), _stream()), "pk_beam_xf_select")
+    check(lib.pk_beam_xf_select(st, _P(x), _P(h), h.shape[-1], _stream()), "pk_beam_xf_select")
 
 
 def beam_xf_slots(st, prev_ks, K):
-    check(lib.pk_beam_xf_slots(ctypes.byref(st), _P(prev_ks), _I(K), _stream()), "pk_beam_xf_slots")
+    check(lib.pk_beam_xf_slots(st, _P(prev_ks), K, _stream()), "pk_beam_xf_slots")
 
 
 def ce_grad(z, tok, coef, scale, dz, n):
     rows, ld = z.shape
-    check(lib.pk_ce_grad(_P(z), _I(_dt(z)), _L(ld), _P(tok), _P(coef), _F(scale), _P(dz), _L(rows), _I(n), _stream()), "pk_ce_grad")
+    check(lib.pk_ce_grad(_P(z), _dt(z), ld, _P(tok), _P(coef), scale, _P(dz), rows, n, _stream()), "pk_ce_grad")
 
 
 def conv_same_f64(x, n_len, h, m_len, y=None):

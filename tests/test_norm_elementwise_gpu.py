@@ -71,7 +71,6 @@ def _abi(name, *args):
 
 def _ws_floats(C):
     from pika_b200 import _lib
-    _lib.lib.pk_colstats_ws_floats.restype = ctypes.c_longlong
     return int(_lib.lib.pk_colstats_ws_floats(C))
 
 
