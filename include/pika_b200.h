@@ -91,6 +91,11 @@ typedef struct {
                                          sum_j 2^(c_ij*log2(e) - max)) over the ROUNDED bf16 outputs -- the first pass of the fused
                                          log-softmax + RNN-T loss (pk_rnnt_loss_fwd_bwd_lse) computed while the logits tile is still in registers.
                                          Needs a 2-D bf16 C with N % 8 == 0, K-major operands, block_n 256. */
+    const int* a_rows_dev;            /* optional device int32: only the first *a_rows_dev rows of A take part, read by the kernel, so
+                                         the count needs no host synchronisation (the compacted joint gradient rows).  K-major A: C rows
+                                         from *a_rows_dev on are undefined, whole BM-row tiles past it are skipped.  MN-major A (rows
+                                         are K): the reduction stops at *a_rows_dev rounded up to 64, whose tail rows of A and B must
+                                         hold zeros; the split-K splits share that shortened reduction.  One pair, kz_count 1, 2-D C. */
 } pk_gemm_desc;
 
 int pk_gemm_bf16(const pk_gemm_desc* desc, void* stream);
@@ -125,6 +130,21 @@ int pk_rnnt_loss_fwd_bwd_lse(const void* logits, int dtype, const int* labels, c
                              const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                              const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
                              long long workspace_bytes, const float* row_lse, int n_parts, void* stream);
+/* Same (row_lse may be NULL), bf16 only, with the gradient stored for the kept rows alone.  A row is skipped when |gb| + |gl| < 2^-136
+ * for its blank / label occupancy terms: every entry of its bf16 gradient is then +-0, so it adds nothing to the fc2 GEMMs or the
+ * bias gradient.  Outputs, all in device memory:
+ *   row_map [B*T*U1] int32: the row's index among the kept rows (kept rows in (b, t, u) order), or -1
+ *   row_count [1] int32: R' = the number of kept rows
+ *   dz_c [B*T*U1, ldv]: rows [0, R') hold the kept rows' gradients (dlogits rebuilt as dlogits[r] = row_map[r] < 0 ? 0 : dz_c[row_map[r]]);
+ *        rows [R', R' rounded up to 64) are written as zeros.  Must not alias logits.
+ *   h_c [B*T*U1, H]: h_c[row_map[r]] = h[r] for the kept rows (the fc2 wgrad's other operand), zeros in the same tail rows as dz_c
+ *   dlogits_colsum as above: the same sum in the same order as the dense form (a skipped row adds +-0 there).
+ * H % 8 == 0, H <= 2048. */
+int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const int* labels, const int* frame_lens,
+                                 const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
+                                 const float* grad_scale, float* costs, void* dz_c, float* dlogits_colsum, void* workspace,
+                                 long long workspace_bytes, const float* row_lse, int n_parts, const void* h, int H,
+                                 void* h_c, int* row_map, int* row_count, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Memory-bound layers around the GEMMs (pika_b200/csrc/elementwise.cu).  `dtype` is the
@@ -231,8 +251,10 @@ int pk_log_softmax(const void* x, int dtype, long long ld, float* y, long long r
 /* h has row pitch ld_h = H or H+8; with H+8 the pad columns are written as (1,0,..,0) so that the fc2 bias gradient
  * falls out of the fc2 wgrad GEMM as one extra column */
 int pk_joint_gate_fwd(const void* ex, const void* py, void* h, int dtype, int B, int T, int U1, int H, int ld_h, void* stream);
-int pk_joint_gate_bwd(const void* ex, const void* py, const void* dh, void* dex, void* dpy, int dtype, int B, int T, int U1,
-                      int H, void* stream);
+/* dh_map: NULL (dh is [B*T*U1, H]) or a row map of pk_rnnt_loss_fwd_bwd_compact: the dh row of joint row r is dh[dh_map[r]], zeros
+ * when dh_map[r] < 0 (dh then holds the compacted rows). */
+int pk_joint_gate_bwd(const void* ex, const void* py, const void* dh, const int* dh_map, void* dex, void* dpy, int dtype, int B, int T,
+                      int U1, int H, void* stream);
 /* one LSTM time step, pointwise part (nn.LSTM, gate order i,f,g,o; trainer/model/transducer.py:56-61) */
 int pk_lstm_cell_fwd(const float* gx, long long ld_gx, const float* gh, long long ld_gh, const float* c_prev, float* c_out,
                      void* h_out, int dtype, long long ld_h, float* gates_save, int B, int H, void* stream);

@@ -80,6 +80,7 @@ class GemmDesc(ctypes.Structure):
         ("block_n", ctypes.c_int),
         ("k_splits", ctypes.c_int),
         ("row_lse", ctypes.c_void_p),
+        ("a_rows_dev", ctypes.c_void_p),
     ]
 
 

@@ -896,11 +896,22 @@ __global__ void __launch_bounds__(128) joint_gate_fwd_sliced_kernel(const T* __r
         }
     }
 }
+// dh row of joint row r: dh[r], or with a row map (compacted joint gradient, pk_rnnt_loss_fwd_bwd_compact) dh[map[r]], zeros when
+// map[r] < 0.  A zero row adds +-0 to every sum below, so the sums equal the dense ones apart from the sign of a zero.
+template <typename T> PK_DEVICE typename V8<T>::Raw load_dh_mapped(const T* dh, int m, int H, int c0) {
+    if (m >= 0) return V8<T>::load_raw(dh + (long long)m * H + c0);
+    return typename V8<T>::Raw{};
+}
+template <typename T> PK_DEVICE typename V8<T>::Raw load_dh_row(const T* dh, const int* map, long long r, int H, int c0) {
+    if (map == nullptr) return V8<T>::load_raw(dh + r * H + c0);
+    return load_dh_mapped<T>(dh, __ldg(map + r), H, c0);
+}
+
 // backward, reduction over u:  dex[b,t,:] = sum_u (d1, dg);    d1 = dh*g*(1-a^2), dg = dh*a*g*(1-g)
 template <typename T>
 __global__ void __launch_bounds__(128) joint_gate_bwd_ex_kernel(const T* __restrict__ ex, const T* __restrict__ py,
-                                                                const T* __restrict__ dh, T* __restrict__ dex, int B, int Tt,
-                                                                int U1, int H) {
+                                                                const T* __restrict__ dh, const int* __restrict__ dh_map,
+                                                                T* __restrict__ dex, int B, int Tt, int U1, int H) {
     const int bt = blockIdx.x;
     const int b = bt / Tt;
     for (int c0 = threadIdx.x * 8; c0 < H; c0 += blockDim.x * 8) {
@@ -912,7 +923,7 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_ex_kernel(const T* __restr
             const T* pr = py + ((long long)b * U1 + u) * 2 * H;
             V8<T>::load(pr + c0, p1);
             V8<T>::load(pr + H + c0, pg);
-            V8<T>::load(dh + ((long long)bt * U1 + u) * H + c0, d);
+            V8<T>::unpack(load_dh_row<T>(dh, dh_map, (long long)bt * U1 + u, H, c0), d);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
                 const float a = jt_tanh<T>(e1[e] + p1[e]), g = jt_sigmoid<T>(eg[e] + pg[e]);
@@ -927,8 +938,8 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_ex_kernel(const T* __restr
 // backward, reduction over t: one CTA per (b,u)
 template <typename T>
 __global__ void __launch_bounds__(128) joint_gate_bwd_py_kernel(const T* __restrict__ ex, const T* __restrict__ py,
-                                                                const T* __restrict__ dh, T* __restrict__ dpy, int B, int Tt,
-                                                                int U1, int H) {
+                                                                const T* __restrict__ dh, const int* __restrict__ dh_map,
+                                                                T* __restrict__ dpy, int B, int Tt, int U1, int H) {
     const int bu = blockIdx.x;
     const int b = bu / U1, u = bu - b * U1;
     for (int c0 = threadIdx.x * 8; c0 < H; c0 += blockDim.x * 8) {
@@ -940,7 +951,7 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_py_kernel(const T* __restr
             const long long bt = (long long)b * Tt + t;
             V8<T>::load(ex + bt * 2 * H + c0, e1);
             V8<T>::load(ex + bt * 2 * H + H + c0, eg);
-            V8<T>::load(dh + (bt * U1 + u) * H + c0, d);
+            V8<T>::unpack(load_dh_row<T>(dh, dh_map, bt * U1 + u, H, c0), d);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
                 const float a = jt_tanh<T>(e1[e] + p1[e]), g = jt_sigmoid<T>(eg[e] + pg[e]);
@@ -960,7 +971,8 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_py_kernel(const T* __restr
 // the prologue.  dh is read once (the two-pass form read it twice) and every tanh / sigmoid is evaluated once instead of twice.
 template <typename T, int UI>
 __global__ void __launch_bounds__(128) joint_gate_bwd_fused_kernel(const T* __restrict__ ex, const T* __restrict__ py, const T* __restrict__ dh,
-                                                                   T* __restrict__ dex, T* __restrict__ dpy, int B, int Tt, int U1, int H) {
+                                                                   const int* __restrict__ dh_map, T* __restrict__ dex, T* __restrict__ dpy,
+                                                                   int B, int Tt, int U1, int H) {
     extern __shared__ __align__(16) uint8_t jg_smem[];
     T* s_py = reinterpret_cast<T*>(jg_smem);                   // [2 parts][4 channel groups][U1][8]: conflict-free 16-byte rows per lane
     const int slices = H / 32;
@@ -981,13 +993,15 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_fused_kernel(const T* __re
     __syncthreads();
     const T* s_p1 = s_py + (long long)(ct * U1) * 8;
     const T* s_pg = s_py + (long long)((4 + ct) * U1) * 8;
-    const T* dh_b = dh + (long long)b * Tt * U1 * H + c0;
+    const long long row_b = (long long)b * Tt * U1;            // joint row of (b, 0, 0)
     const T* ex_b = ex + (long long)b * Tt * 2 * H + c0;
     typename V8<T>::Raw dn[UI], e1n, egn;                      // next frame's operands, fetched one frame ahead (kept packed)
+    int mn[UI];                                                // with a row map: its entries for the frame after next
 #pragma unroll
     for (int i = 0; i < UI; ++i) {
         const int u = lane + 32 * i;
-        if (u < U1) dn[i] = V8<T>::load_raw(dh_b + (long long)u * H);
+        if (u < U1) dn[i] = load_dh_row<T>(dh, dh_map, row_b + u, H, c0);
+        mn[i] = (dh_map != nullptr && u < U1 && Tt > 1) ? __ldg(dh_map + row_b + U1 + u) : -1;
     }
     e1n = V8<T>::load_raw(ex_b);
     egn = V8<T>::load_raw(ex_b + H);
@@ -1002,7 +1016,14 @@ __global__ void __launch_bounds__(128) joint_gate_bwd_fused_kernel(const T* __re
 #pragma unroll
             for (int i = 0; i < UI; ++i) {
                 const int u = lane + 32 * i;
-                if (u < U1) dn[i] = V8<T>::load_raw(dh_b + ((long long)(t + 1) * U1 + u) * H);
+                if (u < U1) {
+                    if (dh_map == nullptr) {
+                        dn[i] = V8<T>::load_raw(dh + (row_b + (long long)(t + 1) * U1 + u) * H + c0);
+                    } else {                                   // the map entry came one frame earlier: no dependent load here
+                        dn[i] = load_dh_mapped<T>(dh, mn[i], H, c0);
+                        if (t + 2 < Tt) mn[i] = __ldg(dh_map + row_b + (long long)(t + 2) * U1 + u);
+                    }
+                }
             }
             e1n = V8<T>::load_raw(ex_b + (long long)(t + 1) * 2 * H);
             egn = V8<T>::load_raw(ex_b + (long long)(t + 1) * 2 * H + H);
@@ -1408,25 +1429,27 @@ extern "C" int pk_joint_gate_fwd(const void* ex, const void* py, void* h, int dt
 }
 
 template <typename T, int UI>
-static void launch_gate_bwd_fused(const void* ex, const void* py, const void* dh, void* dex, void* dpy, int B, int T_, int U1, int H, cudaStream_t st) {
+static void launch_gate_bwd_fused(const void* ex, const void* py, const void* dh, const int* dh_map, void* dex, void* dpy, int B, int T_, int U1, int H,
+                                  cudaStream_t st) {
     const int smem = U1 * 64 * (int)sizeof(T);
     // (capping the registers for 3 CTAs per SM instead of 2 -- 168 registers, 84 spilled bytes at UI = 5 -- measured slower: 1.77 vs 1.40 ms)
-    joint_gate_bwd_fused_kernel<T, UI><<<B * (H / 32), 128, smem, st>>>((const T*)ex, (const T*)py, (const T*)dh, (T*)dex, (T*)dpy, B, T_, U1, H);
+    joint_gate_bwd_fused_kernel<T, UI><<<B * (H / 32), 128, smem, st>>>((const T*)ex, (const T*)py, (const T*)dh, dh_map, (T*)dex, (T*)dpy, B, T_, U1,
+                                                                     H);
 }
-extern "C" int pk_joint_gate_bwd(const void* ex, const void* py, const void* dh, void* dex, void* dpy, int dtype, int B, int T_, int U1,
-                                 int H, void* stream) {
+extern "C" int pk_joint_gate_bwd(const void* ex, const void* py, const void* dh, const int* dh_map, void* dex, void* dpy, int dtype, int B,
+                                 int T_, int U1, int H, void* stream) {
     PK_CHECK_ARG(H % 8 == 0, "H must be a multiple of 8");
     const int ui = (U1 + 31) / 32;
     if (H % 32 == 0 && ui <= 5) {
         cudaStream_t st = STREAM(stream);
-#define PK_GATE_CASE(N) case N: { PK_DISPATCH_T(dtype, (launch_gate_bwd_fused<T, N>(ex, py, dh, dex, dpy, B, T_, U1, H, st))); } break;
+#define PK_GATE_CASE(N) case N: { PK_DISPATCH_T(dtype, (launch_gate_bwd_fused<T, N>(ex, py, dh, dh_map, dex, dpy, B, T_, U1, H, st))); } break;
         switch (ui) { PK_GATE_CASE(1) PK_GATE_CASE(2) PK_GATE_CASE(3) PK_GATE_CASE(4) PK_GATE_CASE(5) }
 #undef PK_GATE_CASE
         DONE();
     }
-    PK_DISPATCH_T(dtype, (joint_gate_bwd_ex_kernel<T><<<B * T_, 128, 0, STREAM(stream)>>>((const T*)ex, (const T*)py, (const T*)dh, (T*)dex, B, T_, U1, H)));
+    PK_DISPATCH_T(dtype, (joint_gate_bwd_ex_kernel<T><<<B * T_, 128, 0, STREAM(stream)>>>((const T*)ex, (const T*)py, (const T*)dh, dh_map, (T*)dex, B, T_, U1, H)));
     PK_CHECK_LAUNCH(); count_launch();
-    PK_DISPATCH_T(dtype, (joint_gate_bwd_py_kernel<T><<<B * U1, 128, 0, STREAM(stream)>>>((const T*)ex, (const T*)py, (const T*)dh, (T*)dpy, B, T_, U1, H)));
+    PK_DISPATCH_T(dtype, (joint_gate_bwd_py_kernel<T><<<B * U1, 128, 0, STREAM(stream)>>>((const T*)ex, (const T*)py, (const T*)dh, dh_map, (T*)dpy, B, T_, U1, H)));
     DONE();
 }
 

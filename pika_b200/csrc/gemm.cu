@@ -51,6 +51,7 @@ struct GemmParams {
     float aux_scale;
     float* row_lse;                     // optional [tiles_n][M][2] per-row (max*log2e, sum 2^(x*log2e-max)) partials of the bf16 output
     uint64_t pol_a, pol_b, pol_c;       // L2 eviction priorities of the three streams
+    const int* a_rows_dev;              // optional: rows of A counted on the device (pk_gemm_desc.a_rows_dev)
 };
 
 // EPI_WARPS: warps 1-3 TMA-store a whole BM x BN bf16 C tile from shared memory (bf16 C, EPI_PLAIN / EPI_LSE).
@@ -139,8 +140,19 @@ __global__ void __launch_bounds__(GemmCfg<BN, epi_warps<CF32, EPI>()>::THREADS, 
     __syncthreads();
 
     const int out_tiles = p.tiles_m * p.tiles_n * p.zb0 * p.zb1;
-    const int num_units = out_tiles * p.k_splits;                       // work units = tiles x K-splits
-    const int k_iters_total = p.n_pairs * p.kz_count * p.num_k_blocks;
+    int num_units = out_tiles * p.k_splits;                             // work units = tiles x K-splits
+    int k_iters_total = p.n_pairs * p.kz_count * p.num_k_blocks;
+    int ips = p.iters_per_split;
+    if (p.a_rows_dev != nullptr) {
+        // the host allows this with one pair, kz_count 1 and a 2-D C, so units run m-tile-major and the k-blocks are K / BK
+        const int rows = *p.a_rows_dev;
+        if (A_MN) {                                                     // rows are K: shorten the reduction, re-cut it into the splits
+            k_iters_total = min(k_iters_total, (rows + BK - 1) / BK);
+            ips = max(1, (k_iters_total + p.k_splits - 1) / p.k_splits);
+        } else {                                                        // rows are M: drop the tiles past the last row
+            num_units = min(num_units, (rows + BM - 1) / BM * p.tiles_n);
+        }
+    }
 
     if (warp < 4) {
         setmaxnreg_dec<40>();
@@ -154,7 +166,7 @@ __global__ void __launch_bounds__(GemmCfg<BN, epi_warps<CF32, EPI>()>::THREADS, 
         for (int unit = worker; unit < num_units; unit += n_workers) {
             const UnitCoord u = decode_unit(p, unit);
             const int m0 = u.mb * BM, n0 = u.nb * BN;
-            const int i0 = u.split * p.iters_per_split, i1 = min(k_iters_total, i0 + p.iters_per_split);
+            const int i0 = u.split * ips, i1 = min(k_iters_total, i0 + ips);
             // position in the flattened (pair, kz, k-block) space: decoded once per unit, then advanced by counters
             int pr = i0 / kzb;
             int rem = i0 - pr * kzb;
@@ -291,7 +303,11 @@ __global__ void __launch_bounds__(GemmCfg<BN, epi_warps<CF32, EPI>()>::THREADS, 
     };
     for (int unit = worker; unit < num_units; unit += n_workers) {
         const UnitCoord u = decode_unit(p, unit);
-        const int k_iters = min(k_iters_total, (u.split + 1) * p.iters_per_split) - u.split * p.iters_per_split;
+        const int k_iters = max(0, min(k_iters_total, (u.split + 1) * ips) - u.split * ips);
+        if (k_iters == 0) {                            // a split past a device-side row count: its share of C is zero
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        }
         int prev = -1;
         for (int k = 0; k < k_iters; ++k) {
             mbar_wait(&full_bar[stage], phase);
@@ -648,6 +664,10 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
     gp.aux_sm = d->aux_stride[0]; gp.aux_s0 = d->aux_stride[1]; gp.aux_s1 = d->aux_stride[2];
     gp.aux_scale = d->aux_scale;
     gp.row_lse = d->row_lse;
+    gp.a_rows_dev = d->a_rows_dev;
+    PK_CHECK_ARG(d->a_rows_dev == nullptr || (d->n_pairs == 1 && d->kz_count == 1 && gp.zb0 == 1 && gp.zb1 == 1 &&
+                                              (d->a_mn_major || d->k_splits <= 1)),
+                 "a_rows_dev needs one pair, kz_count 1, a 2-D C and, for a K-major A, no split-K");
     PK_CHECK_ARG(d->row_lse == nullptr || (d->c_dtype == PK_BF16 && N % 8 == 0 && gp.zb0 == 1 && gp.zb1 == 1 && bn == 256 &&
                                            gp.drop_thresh == 0u && gp.aux_mode == PK_AUX_NONE),
                  "row_lse needs a 2-D bf16 C with N % 8 == 0, block_n = 256, no dropout / aux");
@@ -670,7 +690,8 @@ extern "C" int pk_gemm_bf16(const pk_gemm_desc* d, void* stream_v) {
     int splits = 1;
     const bool plain_epi = d->bias == nullptr && d->act == PK_ACT_NONE && d->drop_p == 0.f && gp.aux_mode == PK_AUX_NONE;
     if (d->k_splits > 0) splits = d->k_splits;
-    else if (gp.c_is_f32 && plain_epi && gp.zb0 == 1 && gp.zb1 == 1 && k_iters_total >= 16 && out_tiles < 6 * workers_max) {
+    else if (gp.c_is_f32 && plain_epi && gp.zb0 == 1 && gp.zb1 == 1 && k_iters_total >= 16 && out_tiles < 6 * workers_max &&
+             (d->a_rows_dev == nullptr || d->a_mn_major)) {
         // the split count (>= 8 k-blocks each, <= 16) that wastes the least of the last wave, preferring fewer splits on ties
         const int w = workers_max;
         double best = 0.0;

@@ -340,25 +340,133 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
     }
 }
 
+// ------------------------------------------------------------------------------------ row compaction
+// Every entry of a row's gradient, -softmax * (gb + gl) plus gb / gl in the blank / label column, is at most |gb| + |gl| in
+// magnitude (gb and gl share a sign).  When |gb| + |gl| < 2^-136 every entry is below 2^-134 -- half the smallest bf16 subnormal,
+// with room for the f32 rounding of the products -- and the stored bf16 row is all +-0: the row adds nothing to the fc2 dgrad,
+// wgrad or bias gradient.  Both terms are then f32 subnormals, whose bit patterns are proportional to their values, so the test
+// is an integer sum of the magnitude bits and does not depend on how the compiler treats subnormal arithmetic.
+PK_DEVICE bool grad_row_kept(float gb, float gl) {
+    return (__float_as_uint(gb) & 0x7fffffffu) + (__float_as_uint(gl) & 0x7fffffffu) >= 0x2000u;   // 0x2000 = 2^-136 as a subnormal
+}
+
+// map[r] = index of row r among the kept rows (ascending, so kept rows stay in (b, t, u) order), or -1.  Three launches: kept rows
+// per SCAN_TILE-row tile, an exclusive scan of the tile counts in one CTA, then the map.
+constexpr int SCAN_THREADS = 1024;
+constexpr int SCAN_PER_THREAD = 4;
+constexpr int SCAN_TILE = SCAN_THREADS * SCAN_PER_THREAD;
+
+PK_DEVICE int block_exclusive_scan(int v, int* s_warp, int* total) {   // SCAN_THREADS threads; s_warp: 32 ints
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) s_warp[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        int s = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, s, o);
+            if (lane >= o) s += y;
+        }
+        s_warp[lane] = s;                                   // inclusive warp totals
+    }
+    __syncthreads();
+    const int r = x - v + (w > 0 ? s_warp[w - 1] : 0);
+    *total = s_warp[31];
+    __syncthreads();                                        // s_warp may be reused by the caller's next scan
+    return r;
+}
+
+PK_DEVICE int tile_kept(const float* gb, const float* gl, long long rows, long long r0, bool (&keep)[SCAN_PER_THREAD]) {
+    int n = 0;
+#pragma unroll
+    for (int k = 0; k < SCAN_PER_THREAD; ++k) {
+        const long long r = r0 + (long long)threadIdx.x * SCAN_PER_THREAD + k;
+        keep[k] = r < rows && grad_row_kept(gb[r], gl[r]);
+        n += keep[k];
+    }
+    return n;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) grad_rows_count_kernel(const float* __restrict__ gb, const float* __restrict__ gl,
+                                                                       long long rows, int* __restrict__ tile_count) {
+    __shared__ int s_warp[32];
+    bool keep[SCAN_PER_THREAD];
+    int total;
+    block_exclusive_scan(tile_kept(gb, gl, rows, (long long)blockIdx.x * SCAN_TILE, keep), s_warp, &total);
+    if (threadIdx.x == 0) tile_count[blockIdx.x] = total;
+}
+
+// exclusive scan of the tile counts in place, *count = kept rows; then zero the rows [count, count rounded up to 64) of dz_c and h_c,
+// which the wgrad's last 64-row k-block reads
+template <typename T>
+__global__ void __launch_bounds__(SCAN_THREADS) grad_rows_scan_kernel(int* __restrict__ tile_count, int n_tiles, int* __restrict__ count,
+                                                                      long long rows, T* dz_c, int ldv, T* h_c, int H) {
+    __shared__ int s_warp[32];
+    __shared__ int s_carry;
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    for (int i0 = 0; i0 < n_tiles; i0 += SCAN_THREADS) {
+        const int i = i0 + threadIdx.x;
+        const int v = i < n_tiles ? tile_count[i] : 0;
+        int total;
+        const int ex = block_exclusive_scan(v, s_warp, &total);
+        if (i < n_tiles) tile_count[i] = s_carry + ex;
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry += total;
+        __syncthreads();
+    }
+    const long long kept = s_carry;
+    if (threadIdx.x == 0) *count = (int)kept;
+    const long long tail = min(rows, (kept + 63) / 64 * 64);
+    for (long long r = kept; r < tail; ++r) {
+        for (int c = threadIdx.x; c < ldv; c += SCAN_THREADS) dz_c[r * ldv + c] = from_f32<T>(0.f);
+        for (int c = threadIdx.x; c < H; c += SCAN_THREADS) h_c[r * H + c] = from_f32<T>(0.f);
+    }
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) grad_rows_map_kernel(const float* __restrict__ gb, const float* __restrict__ gl,
+                                                                     long long rows, const int* __restrict__ tile_off, int* __restrict__ map) {
+    __shared__ int s_warp[32];
+    bool keep[SCAN_PER_THREAD];
+    const long long r0 = (long long)blockIdx.x * SCAN_TILE;
+    int total;
+    int idx = tile_off[blockIdx.x] + block_exclusive_scan(tile_kept(gb, gl, rows, r0, keep), s_warp, &total);
+#pragma unroll
+    for (int k = 0; k < SCAN_PER_THREAD; ++k) {
+        const long long r = r0 + (long long)threadIdx.x * SCAN_PER_THREAD + k;
+        if (r < rows) map[r] = keep[k] ? idx++ : -1;
+    }
+}
+
 // ------------------------------------------------------------------------------------ pass 3
 // One CTA walks a contiguous block of joint nodes; thread i owns the 16-byte column groups i, i+256, ... of every
 // row (32 columns per thread -> V <= 8192), so the column sums of dlogits (= the fc2 bias
 // gradient) accumulate in registers for free.  GRAD_RU rows are in flight per thread.
+// COMPACT: a row r with row_map[r] < 0 is neither read nor written; a kept row's gradient goes to row row_map[r] of dlogits (= dz_c)
+// and its joint activations h[r] are copied to h_c[row_map[r]].  The CTA blocks and the column sums are those of the dense form.
 constexpr int GRAD_THREADS = 256;
 template <typename T> struct GradCfg { static constexpr int MAXG = 32 / Vec16<T>::N; };   // 16-byte groups per thread: V <= 8192 for bf16 and f32
-template <typename T, int GRAD_RU, int MINB>
+template <typename T, int GRAD_RU, int MINB, bool COMPACT>
 __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* logits, const int* __restrict__ labels,
                                                                     const int* __restrict__ label_lens, RnntDims d,
                                                                     const float* __restrict__ lse_in, const float* __restrict__ gb_in,
                                                                     const float* __restrict__ gl_in, T* dlogits, float* __restrict__ colsum,
-                                                                    long long rows_per_cta) {
+                                                                    long long rows_per_cta, const int* __restrict__ row_map,
+                                                                    const T* __restrict__ h, T* __restrict__ h_c, int H) {
     constexpr int VN = Vec16<T>::N;
     constexpr int GRAD_MAXG = GradCfg<T>::MAXG;
-    extern __shared__ float gsm[];                          // per-row scalars of this CTA's block: gb, gl, lse*log2e, label
+    extern __shared__ float gsm[];                          // per-row scalars of this CTA's block: gb, gl, lse*log2e, label (, map)
     float* s_gb = gsm;
     float* s_gl = gsm + rows_per_cta;
     float* s_l2 = gsm + 2 * rows_per_cta;
     int* s_y = reinterpret_cast<int*>(gsm + 3 * rows_per_cta);
+    int* s_map = reinterpret_cast<int*>(gsm + 4 * rows_per_cta);
     const long long rows = (long long)d.B * d.T * d.U1;
     const long long r0 = (long long)blockIdx.x * rows_per_cta;
     const long long r1 = min(rows, r0 + rows_per_cta);
@@ -372,8 +480,10 @@ __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* 
         const int u = (int)(row % d.U1);
         const int b = (int)(row / ((long long)d.T * d.U1));
         s_y[i] = (u < label_lens[b]) ? labels[(size_t)b * d.ld_labels + u] : -1;
+        if (COMPACT) s_map[i] = row_map[row];
     }
     __syncthreads();
+    const int h_vec = COMPACT ? H / 8 : 0;                  // 16-byte groups of an h row (bf16): one per thread, H <= 2048
     float cs[GRAD_MAXG][VN];
 #pragma unroll
     for (int gq = 0; gq < GRAD_MAXG; ++gq)
@@ -381,16 +491,18 @@ __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* 
         for (int e = 0; e < VN; ++e) cs[gq][e] = 0.f;
     for (long long rb = r0; rb < r1; rb += GRAD_RU) {
         uint4 q[GRAD_RU][GRAD_MAXG];
+        uint4 hq[GRAD_RU];
 #pragma unroll
         for (int k = 0; k < GRAD_RU; ++k) {
             const long long row = rb + k;
-            if (row < r1 && (s_gb[row - r0] != 0.f || s_gl[row - r0] != 0.f)) {
+            if (row < r1 && (COMPACT ? s_map[row - r0] >= 0 : (s_gb[row - r0] != 0.f || s_gl[row - r0] != 0.f))) {
                 const uint4* vp = reinterpret_cast<const uint4*>(logits + row * (long long)d.ldv);
 #pragma unroll
                 for (int gq = 0; gq < GRAD_MAXG; ++gq) {
                     const int i = tid + gq * GRAD_THREADS;
                     if (i < nvec_ld) q[k][gq] = ld_plain(vp + i);
                 }
+                if (COMPACT && tid < h_vec) hq[k] = ld_stream(reinterpret_cast<const uint4*>(h + row * (long long)H) + tid);
             }
         }
 #pragma unroll
@@ -398,7 +510,13 @@ __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* 
             const long long row = rb + k;
             if (row >= r1) continue;
             const float gb = s_gb[row - r0], gl = s_gl[row - r0];
-            uint4* op = reinterpret_cast<uint4*>(dlogits + row * (long long)d.ldv);
+            long long orow = row;
+            if (COMPACT) {
+                orow = s_map[row - r0];
+                if (orow < 0) continue;                 // all-zero gradient row: not stored
+                if (tid < h_vec) st_stream(reinterpret_cast<uint4*>(h_c + orow * H) + tid, hq[k]);
+            }
+            uint4* op = reinterpret_cast<uint4*>(dlogits + orow * (long long)d.ldv);
             if (gb == 0.f && gl == 0.f) {               // padded (or zero-probability) node: zeros, nothing read
 #pragma unroll
                 for (int gq = 0; gq < GRAD_MAXG; ++gq) {
@@ -499,7 +617,7 @@ static void rnnt_grad_grid(long long rows, long long* rpc_out, int* ggrid_out) {
     const int gcta = pk::num_sms() * 3 * 4;
     long long rpc = (rows + gcta - 1) / gcta;
     rpc = (rpc + ru - 1) / ru * ru;
-    if (rpc > 2048) rpc = 2048;                      // 16 bytes of shared memory per row
+    if (rpc > 2048) rpc = 2048;                      // 16 (compacted: 20) bytes of shared memory per row
     *rpc_out = rpc; *ggrid_out = (int)((rows + rpc - 1) / rpc);
 }
 extern "C" long long pk_rnnt_loss_colsum_workspace_bytes(int B, int T, int U1, int ldv) {
@@ -511,7 +629,8 @@ extern "C" long long pk_rnnt_loss_colsum_workspace_bytes(int B, int T, int U1, i
 static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, const int* frame_lens,
                           const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                           const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
-                          long long workspace_bytes, const float* row_lse, int n_parts, void* stream_v) {
+                          long long workspace_bytes, const float* row_lse, int n_parts, int* row_map, int* row_count,
+                          const void* h, int H, void* h_c, void* stream_v) {
     using namespace pk;
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
     PK_CHECK_ARG(dtype == PK_F32 || dtype == PK_BF16, "bad dtype");
@@ -575,12 +694,28 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
                          "workspace too small for the column sums (add pk_rnnt_loss_colsum_workspace_bytes)");
             cs_part = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + base_bytes);
         }
-        const size_t gsmem = (size_t)rpc * 16;
-#define PK_GRAD_LAUNCH(TT, RU, MB)                                                                                         \
-        rnnt_grad_kernel<TT, RU, MB><<<ggrid, GRAD_THREADS, gsmem, stream>>>(reinterpret_cast<const TT*>(logits), labels, label_lens, d, lse, \
-                                                                            gb, gl, reinterpret_cast<TT*>(dlogits), cs_part, rpc)
-        if (dtype == PK_BF16) PK_GRAD_LAUNCH(__nv_bfloat16, 2, 3);
-        else PK_GRAD_LAUNCH(float, 2, 2);
+        if (row_map != nullptr) {
+            // the scan's tile counts live in the alpha / beta area of the workspace, which nothing reads after the lattice
+            const int n_tiles = (int)((rows + SCAN_TILE - 1) / SCAN_TILE);
+            int* tile_count = reinterpret_cast<int*>(alpha);
+            grad_rows_count_kernel<<<n_tiles, SCAN_THREADS, 0, stream>>>(gb, gl, rows, tile_count);
+            PK_CHECK_LAUNCH(); count_launch();
+            grad_rows_scan_kernel<__nv_bfloat16><<<1, SCAN_THREADS, 0, stream>>>(tile_count, n_tiles, row_count, rows,
+                                                                                 reinterpret_cast<__nv_bfloat16*>(dlogits), ldv,
+                                                                                 reinterpret_cast<__nv_bfloat16*>(h_c), H);
+            PK_CHECK_LAUNCH(); count_launch();
+            grad_rows_map_kernel<<<n_tiles, SCAN_THREADS, 0, stream>>>(gb, gl, rows, tile_count, row_map);
+            PK_CHECK_LAUNCH(); count_launch();
+        }
+        const size_t gsmem = (size_t)rpc * (row_map != nullptr ? 20 : 16);
+#define PK_GRAD_LAUNCH(TT, RU, MB, CP)                                                                                     \
+        rnnt_grad_kernel<TT, RU, MB, CP><<<ggrid, GRAD_THREADS, gsmem, stream>>>(reinterpret_cast<const TT*>(logits), labels, label_lens, d, \
+                                                                                lse, gb, gl, reinterpret_cast<TT*>(dlogits), cs_part, rpc,  \
+                                                                                row_map, reinterpret_cast<const TT*>(h),                    \
+                                                                                reinterpret_cast<TT*>(h_c), H)
+        if (row_map != nullptr) PK_GRAD_LAUNCH(__nv_bfloat16, 2, 3, true);
+        else if (dtype == PK_BF16) PK_GRAD_LAUNCH(__nv_bfloat16, 2, 3, false);
+        else PK_GRAD_LAUNCH(float, 2, 2, false);
 #undef PK_GRAD_LAUNCH
         PK_CHECK_LAUNCH(); count_launch();
         if (dlogits_colsum) {
@@ -596,7 +731,7 @@ extern "C" int pk_rnnt_loss_fwd_bwd(const void* logits, int dtype, const int* la
                                     const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
                                     long long workspace_bytes, void* stream) {
     return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
-                          dlogits_colsum, workspace, workspace_bytes, nullptr, 0, stream);
+                          dlogits_colsum, workspace, workspace_bytes, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr, stream);
 }
 
 extern "C" int pk_rnnt_loss_fwd_bwd_lse(const void* logits, int dtype, const int* labels, const int* frame_lens,
@@ -605,5 +740,19 @@ extern "C" int pk_rnnt_loss_fwd_bwd_lse(const void* logits, int dtype, const int
                                         long long workspace_bytes, const float* row_lse, int n_parts, void* stream) {
     PK_CHECK_ARG(row_lse != nullptr, "row_lse is null");
     return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
-                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, stream);
+                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, nullptr, nullptr, nullptr, 0, nullptr, stream);
+}
+
+extern "C" int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const int* labels, const int* frame_lens,
+                                            const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
+                                            const float* grad_scale, float* costs, void* dz_c, float* dlogits_colsum, void* workspace,
+                                            long long workspace_bytes, const float* row_lse, int n_parts, const void* h, int H,
+                                            void* h_c, int* row_map, int* row_count, void* stream) {
+    PK_CHECK_ARG(dtype == PK_BF16, "the compacted gradient is bf16 only");
+    PK_CHECK_ARG(dz_c != nullptr && row_map != nullptr && row_count != nullptr && h != nullptr && h_c != nullptr, "null pointer");
+    PK_CHECK_ARG(H > 0 && H % 8 == 0 && H / 8 <= pk::GRAD_THREADS, "H must be a multiple of 8, <= 2048");
+    PK_CHECK_ARG(dz_c != logits, "dz_c must not alias the logits");
+    PK_CHECK_ARG((reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(h_c) & 15) == 0, "h / h_c not 16B aligned");
+    return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dz_c,
+                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, row_map, row_count, h, H, h_c, stream);
 }

@@ -748,6 +748,11 @@ def _ldv(V):
 _FUSED_LSE = True
 
 
+# bf16 training: store the joint gradient only for the rows where it is not all zeros and run the fc2 GEMMs and the gate backward
+# on those rows alone (rnnt_loss_compact).  The dense path stays for the fp32-class mode; tests set False to compare the two
+_COMPACT_GRAD = True
+
+
 # measurement hook (bench.py): when set to a dict, single launches of the step are bracketed by CUDA events on the launching stream,
 # e.g. EVENT_TAPS["fc2_fwd"] = [(start, end), ...] -- the duration of that kernel INSIDE a real step, not in a loop of its own
 EVENT_TAPS = None
@@ -800,23 +805,29 @@ def _joint_forward(enc, pred, model, want_lse=False):
     return logits, state
 
 
-def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None):
-    """dlogits [B,T,U1,ldv] (padding columns zero) -> (d_enc, d_pred); parameter grads written in place."""
+def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None, compact=None):
+    """dlogits [B,T,U1,ldv] (padding columns zero) -> (d_enc, d_pred); parameter grads written in place.
+    compact = (h_c, row_map, row_count) of rnnt_loss_compact: dlogits and h_c hold only the kept rows, the GEMMs run over row_count
+    of them and the gate backward reads dh through row_map."""
     B, T, U1, H, V, ldv = st["dims"]
     R = B * T * U1
     fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
     dl_parts = [p.view(R, ldv) for p in stage_act(dlogits)]
     dl_v = [p[:, :V] for p in dl_parts]
     dh = _new((R, H), like=dlogits)
-    gemm_parts([dl_v], [st["w2"]], dh, b_mn=True)
-    gemm_parts([dl_v], [st["h_parts"]], grad_of(fc2.weight), a_mn=True, b_mn=True)
+    h_parts, row_map, rows = st.get("h_parts"), None, None
+    if compact is not None:
+        h_c, row_map, rows = compact
+        h_parts = [h_c]
+    gemm_parts([dl_v], [st["w2"]], dh, b_mn=True, a_rows_dev=rows)
+    gemm_parts([dl_v], [h_parts], grad_of(fc2.weight), a_mn=True, b_mn=True, a_rows_dev=rows)
     if db2 is None:
         db2 = torch.empty(ldv, dtype=torch.float32, device=dlogits.device)
         K.colsum(dlogits.view(R, ldv), db2)
     grad_of(fc2.bias).copy_(db2[:V])
     dex = _new((B * T, 2 * H), like=dlogits)
     dpy = _new((B * U1, 2 * H), like=dlogits)
-    K.joint_gate_bwd(st["ex"], st["py"], dh, dex, dpy, B, T, U1, H)
+    K.joint_gate_bwd(st["ex"], st["py"], dh, dex, dpy, B, T, U1, H, dh_map=row_map)
     del dh
     dex_parts, dpy_parts = stage_act(dex), stage_act(dpy)
     g1, gg = grad_of(fc1.weight), grad_of(fcg.weight)
@@ -887,10 +898,20 @@ class JointLossFn(torch.autograd.Function):
             costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, want_grad=False, row_lse=st.pop("row_lse"))
             return costs
         db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=logits.device)
-        with _Tap("rnnt_loss"):
-            costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, dlogits=logits, colsum=db2,
-                                           row_lse=st.pop("row_lse"))
-        d_enc, d_pred = _joint_backward(logits, st, model, db2=db2)
+        compact = None
+        if _COMPACT_GRAD and logits.dtype == torch.bfloat16 and len(st["w2"]) == 1 and len(st["h_parts"]) == 1:
+            with _Tap("rnnt_loss"):
+                costs, dz_c, h_c, row_map, rows = K.rnnt_loss_compact(logits, labels, frame_lens, label_lens, st["h_parts"][0], V=V,
+                                                                      colsum=db2, row_lse=st.pop("row_lse"))
+            logits, compact = dz_c, (h_c, row_map, rows)          # the logits and h are released here: dz_c and h_c replace them
+            del dz_c, h_c
+            st.pop("h_parts")
+        else:
+            with _Tap("rnnt_loss"):
+                costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, dlogits=logits, colsum=db2,
+                                               row_lse=st.pop("row_lse"))
+        d_enc, d_pred = _joint_backward(logits, st, model, db2=db2, compact=compact)
+        del compact
         del logits, st
         ctx.save_for_backward(d_enc, d_pred)
         ctx.model = model

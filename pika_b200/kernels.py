@@ -42,13 +42,14 @@ def _fill_view(v, t):
 
 def gemm(a, b, c, a_mn=False, b_mn=False, a_sel=(SEL_ZB0, SEL_ZB1), b_sel=(SEL_ZB0, SEL_ZB1), kz_count=1,
          a_row_off=None, b_row_off=None, alpha=1.0, bias=None, act=ACT_NONE, drop_p=0.0, drop_seed=0,
-         aux=None, aux_mode=AUX_NONE, aux_scale=1.0, accumulate=False, block_n=0, k_splits=0, row_lse=None):
+         aux=None, aux_mode=AUX_NONE, aux_scale=1.0, accumulate=False, block_n=0, k_splits=0, row_lse=None, a_rows_dev=None):
     """C = epilogue(alpha * sum_p A_p @ B_p^T) on the wgmma tensor cores (include/pika_b200.h).
 
     a, b: a bf16 view or a list of views (pairs).  Views are torch tensors of <= 4 dims laid out
     (z3, z2, rows, contiguous):  K-major A = (.., M, K), MN-major A = (.., K, M); same for B with N.
     c: (zb1, zb0, M, N) view, bf16 or f32.  aux: tensor broadcast-compatible with c's logical shape,
     given as a view with the same number of dims as c.
+    a_rows_dev: int32 device tensor [1]; only that many leading rows of A take part (pk_gemm_desc.a_rows_dev).
     """
     a = a if isinstance(a, (list, tuple)) else [a]
     b = b if isinstance(b, (list, tuple)) else [b]
@@ -91,6 +92,9 @@ def gemm(a, b, c, a_mn=False, b_mn=False, a_sel=(SEL_ZB0, SEL_ZB1), b_sel=(SEL_Z
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and c.dim() == 2
         assert tuple(row_lse.shape) == (row_lse_parts(c.shape[-2], c.shape[-1], block_n), c.shape[-2], 2)
         d.row_lse = row_lse.data_ptr()
+    if a_rows_dev is not None:
+        assert a_rows_dev.dtype == torch.int32 and a_rows_dev.is_cuda
+        d.a_rows_dev = a_rows_dev.data_ptr()
     check(lib.pk_gemm_bf16(d, _stream()), "pk_gemm_bf16")
     return c
 
@@ -128,6 +132,35 @@ def rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=None, grad_scale
                                    _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes, _stream()),
           "pk_rnnt_loss_fwd_bwd")
     return costs, dlogits
+
+
+def rnnt_loss_compact(logits, labels, frame_lens, label_lens, h, V=None, colsum=None, row_lse=None):
+    """bf16 logits [B,T,U1,ldv], joint activations h [B*T*U1, H] -> (costs [B], dz_c [R, ldv], h_c [R, H], row_map [R], row_count [1]).
+    Only the rows whose gradient is not all zeros are stored: dz_c / h_c rows [0, row_count) hold them in row order, row_map[r] is the
+    row's index there or -1.  dz_c is a new buffer as large as the logits (the two are alive together while the gradient is formed)."""
+    B, T, U1, ldv = logits.shape
+    V = ldv if V is None else V
+    R, H = B * T * U1, h.shape[-1]
+    assert logits.is_contiguous() and logits.dtype == torch.bfloat16 and labels.dtype == torch.int32 and labels.dim() == 2
+    assert frame_lens.dtype == torch.int32 and label_lens.dtype == torch.int32
+    assert h.is_contiguous() and h.dtype == torch.bfloat16 and h.numel() == R * H
+    ws_bytes = int(lib.pk_rnnt_loss_workspace_bytes(B, T, U1))
+    if colsum is not None:
+        ws_bytes += int(lib.pk_rnnt_loss_colsum_workspace_bytes(B, T, U1, ldv))
+    dev = logits.device
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    costs = torch.empty(B, dtype=torch.float32, device=dev)
+    dz_c = torch.empty(R, ldv, dtype=torch.bfloat16, device=dev)
+    h_c = torch.empty(R, H, dtype=torch.bfloat16, device=dev)
+    row_map = torch.empty(R, dtype=torch.int32, device=dev)
+    row_count = torch.empty(1, dtype=torch.int32, device=dev)
+    if row_lse is not None:
+        assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (R, 2)
+    check(lib.pk_rnnt_loss_fwd_bwd_compact(_P(logits), PK_BF16, _P(labels), _P(frame_lens), _P(label_lens), B, T, U1, V, ldv,
+                                           max(labels.stride(0), 1), None, _P(costs), _P(dz_c), _P(colsum), _P(ws), ws_bytes,
+                                           _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _P(h), H, _P(h_c),
+                                           _P(row_map), _P(row_count), _stream()), "pk_rnnt_loss_fwd_bwd_compact")
+    return costs, dz_c, h_c, row_map, row_count
 
 
 # ------------------------------------------------------------------------------------------------
@@ -290,8 +323,9 @@ def joint_gate_fwd(ex, py, h, B, T, U1, H):
     check(lib.pk_joint_gate_fwd(_P(ex), _P(py), _P(h), _dt(ex), B, T, U1, H, h.stride(0), _stream()), "pk_joint_gate_fwd")
 
 
-def joint_gate_bwd(ex, py, dh, dex, dpy, B, T, U1, H):
-    check(lib.pk_joint_gate_bwd(_P(ex), _P(py), _P(dh), _P(dex), _P(dpy), _dt(ex), B, T, U1, H, _stream()), "pk_joint_gate_bwd")
+def joint_gate_bwd(ex, py, dh, dex, dpy, B, T, U1, H, dh_map=None):
+    """dh_map [B*T*U1] int32 (rnnt_loss_compact): dh holds the kept rows only, row r of the joint is dh[dh_map[r]] or zeros"""
+    check(lib.pk_joint_gate_bwd(_P(ex), _P(py), _P(dh), _P(dh_map), _P(dex), _P(dpy), _dt(ex), B, T, U1, H, _stream()), "pk_joint_gate_bwd")
 
 
 def lstm_cell_fwd(gx, gh, c_prev, c_out, h_out, gates_save, B, H):
