@@ -451,6 +451,7 @@ long long pk_lstm_seq_workspace_bytes(int H);
  * lens: int32 [B] on the device, or NULL (every sequence runs all U steps).  Sequence b with length L_b is processed at
  * t = s (forward) or t = L_b - 1 - s (reverse) for steps s < L_b, from a zero state; the kernel runs max_b L_b steps.
  * Outputs and dG rows at t >= L_b are written as zeros.  ws: pk_lstm_seq_workspace_bytes(n_dir * H) bytes, zero-initialised.
+ * w_hh (fwd), dG (bwd) and ws must be 16-byte aligned; H a multiple of 64 with n_dir * H/8 <= #SMs; B, U >= 1; ldo >= n_dir * H.
  * The prediction net's layer is the lens = NULL, n_dir = 1, reverse = 0, ldo = H case. */
 int pk_lstm_seq_fwd_ex(const float* gx, const void* w_hh_bf16, void* out, int out_dtype, int ldo, float* gates_save, float* cs,
                        const int* lens, int B, int U, int H, int n_dir, int reverse, void* ws, void* stream);

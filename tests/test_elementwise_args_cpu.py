@@ -1,10 +1,12 @@
 """Argument rejection of the memory-bound entry points of csrc/elementwise.cu: misaligned 16-byte vector operands, C % 8 != 0,
-LayerNorm C > 1024, rows == 0, a drop probability of 0.  Each rejected call must return < 0 with a pk_last_error message naming the
-problem, and launch nothing.
+LayerNorm C > 1024, rows == 0, a drop probability of 0.  And of the persistent LSTM recurrence (csrc/lstm_seq.cu,
+pk_lstm_seq_fwd_ex / _bwd_ex): a w_hh, workspace or dG that is not 16-byte aligned (16-byte loads and cp.async.bulk sources),
+B == 0, U == 0, n_dir == 3, H % 64 != 0, n_dir * H/8 above the SM count, ldo < n_dir * H.  Each rejected call must return < 0 with
+a pk_last_error message naming the problem, and launch nothing.
 
 The calls run in a subprocess that sees no CUDA device (CUDA_VISIBLE_DEVICES=""), with made-up device addresses: should a check
 regress, the call gets as far as a launch and fails with "no device" rather than the expected message, instead of running a kernel on
-a bogus pointer."""
+a bogus pointer.  With no device the SM count the LSTM check compares against is the H100's 132."""
 import json
 import os
 import subprocess
@@ -49,7 +51,18 @@ def _gather(src=A, dst=A, C=256, rows=64):
     return ("pk_gather_rows", P(src), P(A), P(dst), I(BF16), L(rows), I(C))
 
 
+def _lstm_fwd(w_hh=A, ws=A, B=32, U=10, H=256, n_dir=1, ldo=None):
+    ldo = n_dir * H if ldo is None else ldo
+    return ("pk_lstm_seq_fwd_ex", P(A), P(w_hh), P(A), I(BF16), I(ldo), P(A), P(A), P(0), I(B), I(U), I(H), I(n_dir), I(0), P(ws))
+
+
+def _lstm_bwd(dG=A, ws=A, B=32, U=10, H=256, n_dir=1, ldo=None):
+    ldo = n_dir * H if ldo is None else ldo
+    return ("pk_lstm_seq_bwd_ex", P(A), I(BF16), I(ldo), P(A), P(A), P(A), P(dG), P(0), I(B), I(U), I(H), I(n_dir), I(0), P(ws))
+
+
 ALIGN = "16-byte aligned"
+SMS = "#SMs"
 CASES = [
     ("bn_fwd-x", ALIGN, _bn_fwd(x=M)),
     ("bn_fwd-y", ALIGN, _bn_fwd(y=M, dtype=BF16)),
@@ -87,6 +100,24 @@ CASES = [
     ("scatter_add_rows-rows0", "rows must be > 0", ("pk_scatter_add_rows", P(A), P(A), P(A), I(F32), L(0), I(13))),
     ("ce_grad-n>ld", "bad shape", ("pk_ce_grad", P(A), I(F32), L(32), P(A), P(A), F(1.0), P(A), L(4), I(33))),
     ("cast_split-cols_pad<cols", "bad shape", ("pk_cast_split", P(A), I(F32), L(64), P(A), P(A), L(64), L(4), I(64), I(56), F(1.0))),
+    ("lstm_fwd-w_hh", ALIGN, _lstm_fwd(w_hh=M)),
+    ("lstm_fwd-ws", ALIGN, _lstm_fwd(ws=M)),
+    ("lstm_fwd-B0", "empty batch", _lstm_fwd(B=0)),
+    ("lstm_fwd-U0", "U must be >= 1", _lstm_fwd(U=0)),
+    ("lstm_fwd-n_dir3", "n_dir must be 1 or 2", _lstm_fwd(n_dir=3)),
+    ("lstm_fwd-H%64", "multiple of 64", _lstm_fwd(H=200)),
+    ("lstm_fwd-H1088", SMS, _lstm_fwd(H=1088)),
+    ("lstm_fwd-bidir-H576", SMS, _lstm_fwd(H=576, n_dir=2)),
+    ("lstm_fwd-ldo<n_dir*H", "ldo must be >= n_dir * H", _lstm_fwd(H=256, n_dir=2, ldo=504)),
+    ("lstm_bwd-dG", ALIGN, _lstm_bwd(dG=M)),
+    ("lstm_bwd-ws", ALIGN, _lstm_bwd(ws=M)),
+    ("lstm_bwd-B0", "empty batch", _lstm_bwd(B=0)),
+    ("lstm_bwd-U0", "U must be >= 1", _lstm_bwd(U=0)),
+    ("lstm_bwd-n_dir3", "n_dir must be 1 or 2", _lstm_bwd(n_dir=3)),
+    ("lstm_bwd-H%64", "multiple of 64", _lstm_bwd(H=200)),
+    ("lstm_bwd-H1088", SMS, _lstm_bwd(H=1088)),
+    ("lstm_bwd-bidir-H576", SMS, _lstm_bwd(H=576, n_dir=2)),
+    ("lstm_bwd-ldo<n_dir*H", "ldo must be >= n_dir * H", _lstm_bwd(H=512, ldo=448)),
 ]
 
 _CHILD = r"""

@@ -290,7 +290,8 @@ def test_dropout_linear_backward_uses_forward_mask():
     assert rel(x2.grad, gx2) < TOL
 
 
-@pytest.mark.parametrize("B,U,H", [(5, 12, 128), (32, 40, 256), (64, 20, 256), (45, 9, 128)])     # > 32 sequences: one cooperative launch per 32
+@pytest.mark.parametrize("B,U,H", [(5, 12, 128), (32, 40, 256), (64, 20, 256), (45, 9, 128),    # > 32 sequences: one cooperative launch per 32
+                                   (32, 150, 1024)])                                          # the benchmark's prediction net: 128 CTAs
 def test_lstm_persistent_kernel_bf16(B, U, H):
     """bf16 production path: the cooperative persistent LSTM kernels (lstm_seq.cu) vs torch fp32 nn.LSTM with
     bf16-rounded weights; bf16 activations/recurrent operands -> 2e-2 outputs, 6e-2 gradients (norm-relative)."""

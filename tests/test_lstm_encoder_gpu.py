@@ -89,9 +89,10 @@ def check_case(lens, out, ref, dx, grads, lstm, tol_out, tol_grad):
 
 @pytest.mark.parametrize("B", [5, 32, 45])
 @pytest.mark.parametrize("bi", [False, True])
-@pytest.mark.parametrize("H", [128, 256, 512])
+@pytest.mark.parametrize("H", [128, 256, 512, 200])
 def test_ragged_lstm_layer_bf16_matches_packed_torch(H, bi, B):
-    """bf16 production path: one cooperative launch for both directions (B > 32: several launches); same bounds as
+    """bf16 production path: one cooperative launch for both directions (B > 32: several launches); H = 200 (not a multiple of
+    64) takes the bf16 per-step path instead, a recurrent GEMM and a fused cell kernel per step.  Same bounds as
     test_lstm_persistent_kernel_bf16"""
     check_case(*layer_case("bf16", H, bi, B, seed=H + B + int(bi)), tol_out=2e-2, tol_grad=6e-2)
 
