@@ -306,9 +306,16 @@ int pk_bmuf_adam_update(float* glob, float* local, float* delta_prev, float* exp
  * Replaces loader/audio.py (AudioSegment.change_speed/normalize/_convert_*), the PyKaldi
  * Fbank.compute_features call and splice() in loader/otf_utt_loader.py:28-46,195-201,218-234,262-270,
  * and trainer/train_transducer_bmuf_otfaug.py:86-93 + utils/spec_augment.py:10-20.
- *   pcm [B, ld_pcm] int16; n_samples, new_len (= int(n/rate)), n_frames (= 1+(new_len-400)/160) [B] int32
+ *   pcm [B, ld_pcm] int16; n_samples, new_len (= int(n/rate)) [B] int32
+ *   n_frames [B] int32: fbank frames of new_len samples; snip_edges: 0 if new_len < frame_len, else 1+(new_len-frame_len)/frame_shift;
+ *     otherwise (new_len + frame_shift/2) / frame_shift, frame t starting at t*frame_shift + frame_shift/2 - frame_len/2 with the
+ *     samples outside [0, new_len) reflected about the edges (Kaldi's ExtractWindow)
+ *   t_max: output rows; stride: output row t is spliced fbank frame min(t, ceil(n_frames/stride)-1)*stride, i.e.
+ *     splice(feats)[::stride] padded with its last row.  Workspace queries take t_max*stride, the fbank frames held in between.
  *   rate, target_db [B] f32 (host-drawn, as the reference draws them in the loader thread)
- *   window [400], twiddle [256 x (re,im)], mel_w [n_mel,256], mel_lo/hi [n_mel]: host-built tables
+ *   window [frame_len], twiddle [N/2 x (re,im)] = exp(-2 pi i k / N), mel_w [n_mel, N/2], mel_lo/hi [n_mel]: host-built tables for
+ *     the FFT size N = 2^log2_nfft, 128 <= N <= 2048, 1 <= frame_len <= N; n_max >= frame_len when snip_edges is set
+ *   remove_dc: subtract each window's mean (Kaldi --remove-dc-offset); preemph: --preemphasis-coefficient
  *   offset/scale [D] CMVN (NULL = off); cmn: subtract the per-utterance mean over the PADDED time axis
  *   (f0,fs,t0,ts): SpecAugment freq/time mask start and span (span 0 = off), shared by the batch
  *   out [B, t_max, D] f32|bf16; wave_i16_out [B, n_max] optional copy of the augmented samples
@@ -320,13 +327,16 @@ int pk_bmuf_adam_update(float* glob, float* local, float* delta_prev, float* exp
 long long pk_frontend_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D);
 int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                     const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
-                    int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
-                    const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
+                    int rctx, int stride, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
+                    const int* mel_hi, int frame_len, int frame_shift, int log2_nfft, int snip_edges, int remove_dc,
+                    float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
                     int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
                     long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream);
-int pk_fbank(const float* wave, long long ld_wave, const int* n_frames, int B, int t_max, int n_mel, const float* window,
-             const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, float preemph, float* feats,
-             float dither, unsigned int dither_seed, void* stream);
+/* pk_fbank: the fbank stage alone (no stride); n_samples [B] (the reflected edges' bound) may be NULL when snip_edges is set */
+int pk_fbank(const float* wave, long long ld_wave, const int* n_samples, const int* n_frames, int B, int t_max, int n_mel,
+             const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len,
+             int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, float* feats, float dither,
+             unsigned int dither_seed, void* stream);
 
 /* Front end with on-the-fly noise and reverberation (loader/audio.py:426-513 AudioSegment.add_noise / convolve_and_normalize,
  * loader/otf_utt_loader.py:224-228), per utterance: speed -> normalize(target_db) -> add_noise -> convolve_and_normalize -> int16
@@ -344,8 +354,9 @@ int pk_fbank(const float* wave, long long ld_wave, const int* n_frames, int B, i
 long long pk_frontend_noise_rir_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D, int rir_max_len);
 int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                               const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
-                              int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
-                              const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
+                              int rctx, int stride, const float* window, const float* twiddle, const float* mel_w,
+                              const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift, int log2_nfft, int snip_edges,
+                              int remove_dc, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
                               int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
                               long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
                               const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,

@@ -18,7 +18,6 @@
 namespace pk {
 void count_launch();
 
-constexpr int FB_FRAME = 400, FB_SHIFT = 160, FB_NFFT = 512, FB_BINS = 256;
 constexpr int AUG_THREADS = 256;
 
 // ------------------------------------------------------------------------------------ augmentation
@@ -390,13 +389,23 @@ __global__ void __launch_bounds__(CONV_THREADS) conv_accum_inverse_kernel(const 
 }
 
 // ------------------------------------------------------------------------------------ fbank
+// FFT sizes 2^7 .. 2^11: 8 to 48 kHz at frames up to 42 ms (--round-to-power-of-two)
+constexpr int FB_LOG2_MIN = 7, FB_LOG2_MAX = 11;
+
 struct FbankTables {
-    const float* window;    // [400] Hamming
-    const float2* twiddle;  // [256] exp(-2 pi i k / 512)
-    const float* mel_w;     // [n_mel][256]
+    const float* window;    // [frame_len] window function
+    const float2* twiddle;  // [N/2] exp(-2 pi i k / N)
+    const float* mel_w;     // [n_mel][N/2]
     const int* mel_lo;      // [n_mel] first non-zero bin
     const int* mel_hi;      // [n_mel] one past the last non-zero bin
 };
+
+struct FrameGeom {          // Kaldi FrameExtractionOptions, in samples
+    int frame_len, frame_shift, snip_edges, remove_dc;
+};
+
+// N/2 butterflies per stage, one per thread; at least 256 threads so that every mel bin (n_mel <= 256) has one
+constexpr int fbank_threads(int log2n) { return (1 << (log2n - 1)) < 256 ? 256 : (1 << (log2n - 1)); }
 
 // standard normal from two counter-based hashes (Box-Muller); one draw per (utterance, frame, sample), as Kaldi's Dither() draws
 // one RandGauss() per sample of every extracted window (feat/feature-window.cc: Dither) -- its RNG stream itself is not reproducible
@@ -407,96 +416,144 @@ PK_DEVICE float dither_gauss(uint64_t idx, uint32_t seed) {
     return sqrtf(-2.f * __logf(u1)) * __cosf(6.283185307179586f * u2);
 }
 
-__global__ void __launch_bounds__(256) fbank_kernel(const float* __restrict__ wave, long long ld_wave, const int* __restrict__ n_frames,
-                                                    FbankTables tb, int n_mel, float preemph, float* __restrict__ feats,
-                                                    long long ld_b, int t_max, float dither, uint32_t dither_seed) {
+// Kaldi's ExtractWindow at snip_edges = false: samples outside [0, n) are reflected about the signal's edges until inside
+PK_DEVICE long long reflect_index(long long s, long long n) {
+    while (s < 0 || s >= n) s = s < 0 ? -s - 1 : 2 * n - 1 - s;
+    return s;
+}
+
+// one CTA per (frame, utterance), a full SM's worth of threads resident.  n_len: samples per utterance (read only when
+// snip_edges = 0).  THREADS >= N/2, so every loop below has a trip count known at compile time.  The arithmetic is spelled out with
+// explicit roundings: DC removal fused into the subtraction of the window's sum times -1/frame_len, pre-emphasis as
+// fma(-c, prev, cur), the complex products and |X|^2 with the first product fused -- the same operations, in the same order, at
+// every FFT size.
+template <int LOG2N>
+__global__ void __launch_bounds__(fbank_threads(LOG2N), 2048 / fbank_threads(LOG2N)) fbank_kernel(const float* __restrict__ wave, long long ld_wave,
+                                                                     const int* __restrict__ n_len, const int* __restrict__ n_frames,
+                                                                     FbankTables tb, FrameGeom g, int n_mel, float preemph,
+                                                                     float* __restrict__ feats, long long ld_b, int t_max, float dither,
+                                                                     uint32_t dither_seed) {
+    constexpr int N = 1 << LOG2N, NB = N / 2, THREADS = fbank_threads(LOG2N), WARPS = THREADS / 32;
+    constexpr int PER_THREAD = (N + THREADS - 1) / THREADS;
     const int t = blockIdx.x, b = blockIdx.y;
     if (t >= n_frames[b]) return;
-    __shared__ float2 buf[FB_NFFT];
-    __shared__ float frame[FB_FRAME];
-    __shared__ float red[8];
-    __shared__ float power[FB_BINS];
-    const int tid = threadIdx.x;
-    const float* src = wave + (long long)b * ld_wave + (long long)t * FB_SHIFT;
+    __shared__ float2 buf[N];
+    __shared__ float frame[N];
+    __shared__ float red[WARPS];
+    __shared__ float power[NB];
+    const int tid = threadIdx.x, L = g.frame_len;
+    const float* src = wave + (long long)b * ld_wave;
+    const uint64_t key = ((uint64_t)b * (uint64_t)t_max + (uint64_t)t) * (uint64_t)L;
     float part = 0.f;
-    for (int i = tid; i < FB_FRAME; i += 256) {
-        float v = src[i];
-        if (dither != 0.f) v += dither * dither_gauss(((uint64_t)b * (uint64_t)t_max + (uint64_t)t) * FB_FRAME + (uint64_t)i, dither_seed);
-        frame[i] = v; part += v;
+    if (g.snip_edges) {
+        src += (long long)t * g.frame_shift;
+#pragma unroll
+        for (int j = 0; j < PER_THREAD; ++j) {
+            const int i = tid + j * THREADS;
+            if (i < L) {
+                float v = src[i];
+                if (dither != 0.f) v = __fmaf_rn(dither, dither_gauss(key + (uint64_t)i, dither_seed), v);
+                frame[i] = v; part += v;
+            }
+        }
+    } else {
+        const long long start = (long long)t * g.frame_shift + g.frame_shift / 2 - L / 2, n = n_len[b];
+#pragma unroll
+        for (int j = 0; j < PER_THREAD; ++j) {
+            const int i = tid + j * THREADS;
+            if (i < L) {
+                float v = src[reflect_index(start + i, n)];
+                if (dither != 0.f) v = __fmaf_rn(dither, dither_gauss(key + (uint64_t)i, dither_seed), v);
+                frame[i] = v; part += v;
+            }
+        }
     }
     part = warp_sum(part);
     if ((tid & 31) == 0) red[tid >> 5] = part;
     __syncthreads();
-    float mean = 0.f;
+    float sum = 0.f, neg_inv_len = 0.f;
+    if (g.remove_dc) {
 #pragma unroll
-    for (int w = 0; w < 8; ++w) mean += red[w];
-    mean *= (1.0f / FB_FRAME);
+        for (int w = 0; w < WARPS; ++w) sum += red[w];
+        neg_inv_len = -(1.0f / (float)L);
+    }
     // DC removal, pre-emphasis (x[i] -= c*x[i-1], x[0] -= c*x[0]), window, zero-pad, bit-reversed placement
-    for (int i = tid; i < FB_NFFT; i += 256) {
-        float v = 0.f;
-        if (i < FB_FRAME) {
-            const float cur = frame[i] - mean;
-            const float prev = (i > 0 ? frame[i - 1] : frame[0]) - mean;
-            v = (cur - preemph * prev) * tb.window[i];
+#pragma unroll
+    for (int j = 0; j < PER_THREAD; ++j) {
+        const int i = tid + j * THREADS;
+        if (i < N) {
+            float v = 0.f;
+            if (i < L) {
+                const float cur = __fmaf_rn(sum, neg_inv_len, frame[i]);
+                const float prev = __fmaf_rn(sum, neg_inv_len, i > 0 ? frame[i - 1] : frame[0]);
+                v = __fmul_rn(__fmaf_rn(-preemph, prev, cur), tb.window[i]);
+            }
+            const int r = __brev((unsigned)i) >> (32 - LOG2N);
+            buf[r] = make_float2(v, 0.f);
         }
-        const int r = __brev((unsigned)i) >> (32 - 9);
-        buf[r] = make_float2(v, 0.f);
     }
     __syncthreads();
-    // 9 radix-2 stages, 256 butterflies each (one per thread)
+    // LOG2N radix-2 stages of N/2 butterflies, one per thread
 #pragma unroll
-    for (int s = 1; s <= 9; ++s) {
-        const int half = 1 << (s - 1);
-        const int grp = tid >> (s - 1), pos = tid & (half - 1);
-        const int i0 = grp * (half << 1) + pos, i1 = i0 + half;
-        const float2 w = tb.twiddle[pos << (9 - s)];
-        const float2 a = buf[i0], c = buf[i1];
-        const float2 wc = make_float2(c.x * w.x - c.y * w.y, c.x * w.y + c.y * w.x);
-        buf[i0] = make_float2(a.x + wc.x, a.y + wc.y);
-        buf[i1] = make_float2(a.x - wc.x, a.y - wc.y);
+    for (int s = 1; s <= LOG2N; ++s) {
+        if (NB == THREADS || tid < NB) {
+            const int half = 1 << (s - 1);
+            const int grp = tid >> (s - 1), pos = tid & (half - 1);
+            const int i0 = grp * (half << 1) + pos, i1 = i0 + half;
+            const float2 w = tb.twiddle[pos << (LOG2N - s)];
+            const float2 a = buf[i0], c = buf[i1];
+            const float2 wc = make_float2(__fmaf_rn(c.x, w.x, -__fmul_rn(c.y, w.y)), __fmaf_rn(c.x, w.y, __fmul_rn(c.y, w.x)));
+            buf[i0] = make_float2(__fadd_rn(a.x, wc.x), __fadd_rn(a.y, wc.y));
+            buf[i1] = make_float2(__fsub_rn(a.x, wc.x), __fsub_rn(a.y, wc.y));
+        }
         __syncthreads();
     }
-    power[tid] = buf[tid].x * buf[tid].x + buf[tid].y * buf[tid].y;
+    if (NB == THREADS || tid < NB) power[tid] = __fmaf_rn(buf[tid].x, buf[tid].x, __fmul_rn(buf[tid].y, buf[tid].y));
     __syncthreads();
     if (tid < n_mel) {
         float e = 0.f;
-        const float* w = tb.mel_w + (long long)tid * FB_BINS;
-        for (int k = tb.mel_lo[tid]; k < tb.mel_hi[tid]; ++k) e += w[k] * power[k];
+        const float* w = tb.mel_w + (long long)tid * NB;
+        for (int k = tb.mel_lo[tid]; k < tb.mel_hi[tid]; ++k) e = __fmaf_rn(w[k], power[k], e);
         feats[(long long)b * ld_b + (long long)t * n_mel + tid] = logf(fmaxf(e, 1.1920928955078125e-07f));
     }
 }
 
 // ------------------------------------------------------------------------------------ splice / CMN / CMVN / SpecAugment
-PK_DEVICE float spliced_value(const float* __restrict__ fb, int n_frames, int n_mel, int lctx, int t, int col) {
-    // frame t of the padded batch: rows >= n_frames replicate the last valid SPLICED frame
-    const int tt = min(t, n_frames - 1);
+// output row t of the padded batch: splice(feats)[::stride] (n_out = ceil(n_frames / stride) rows), rows >= n_out replicating the
+// last one; the spliced row of fbank frame tt stacks frames tt-lctx .. tt+rctx, clamped to the utterance.  STRIDED = false is
+// stride 1 without the extra index arithmetic, which costs the splice kernels about 13 % (they are instruction-bound)
+template <bool STRIDED>
+PK_DEVICE float spliced_value(const float* __restrict__ fb, int n_frames, int n_out, int n_mel, int lctx, int stride, int t, int col) {
+    const int tt = STRIDED ? min(t, n_out - 1) * stride : min(t, n_frames - 1);
     const int k = col / n_mel, c = col - k * n_mel;
     int src = tt + k - lctx;
     src = max(0, min(n_frames - 1, src));
     return fb[(long long)src * n_mel + c];
 }
+template <bool STRIDED>
 __global__ void splice_colsum_kernel(const float* __restrict__ feats, long long ld_b, const int* __restrict__ n_frames, int n_mel,
-                                     int lctx, int D, int t_max, float* __restrict__ sums) {
+                                     int lctx, int stride, int D, int t_max, float* __restrict__ sums) {
     const int b = blockIdx.y, col = threadIdx.x;
     if (col >= D || n_frames[b] <= 0) return;
     const int t0 = blockIdx.x * 64, t1 = min(t_max, t0 + 64);
     const float* fb = feats + (long long)b * ld_b;
+    const int nf = n_frames[b], n_out = STRIDED ? (nf + stride - 1) / stride : nf;
     float s = 0.f;
-    for (int t = t0; t < t1; ++t) s += spliced_value(fb, n_frames[b], n_mel, lctx, t, col);
+    for (int t = t0; t < t1; ++t) s += spliced_value<STRIDED>(fb, nf, n_out, n_mel, lctx, stride, t, col);
     atomicAdd(&sums[(long long)b * D + col], s);
 }
-template <typename T>
+template <typename T, bool STRIDED>
 __global__ void splice_finalize_kernel(const float* __restrict__ feats, long long ld_b, const int* __restrict__ n_frames, int n_mel,
-                                       int lctx, int D, int t_max, const float* __restrict__ sums, int cmn,
+                                       int lctx, int stride, int D, int t_max, const float* __restrict__ sums, int cmn,
                                        const float* __restrict__ offset, const float* __restrict__ scale, int f0, int fs, int t0m,
                                        int ts, T* __restrict__ out) {
     const int b = blockIdx.y;
     const long long total = (long long)t_max * D;
     const float* fb = feats + (long long)b * ld_b;
-    const int nf = n_frames[b];
+    const int nf = n_frames[b], n_out = STRIDED ? (nf + stride - 1) / stride : nf;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(i / D), col = (int)(i - (long long)t * D);
-        float v = nf > 0 ? spliced_value(fb, nf, n_mel, lctx, t, col) : 0.f;
+        float v = nf > 0 ? spliced_value<STRIDED>(fb, nf, n_out, n_mel, lctx, stride, t, col) : 0.f;
         if (cmn) v -= sums[(long long)b * D + col] / (float)t_max;
         if (offset) { v += offset[col]; v *= scale[col]; }
         if ((fs > 0 && col >= f0 && col < f0 + fs) || (ts > 0 && t >= t0m && t < t0m + ts)) v = 0.f;
@@ -508,7 +565,7 @@ __global__ void splice_finalize_kernel(const float* __restrict__ feats, long lon
 using namespace pk;
 
 /* Workspace layout of pk_frontend_fwd: resampled f64 [B, n_max] | partial f64 [B, parts] | wave f32 [B, n_max] |
- * feats f32 [B, t_max, n_mel] | sums f32 [B, D] | err int */
+ * feats f32 [B, t_max, n_mel] | sums f32 [B, D] | err int.  t_max here counts fbank frames, before the splice's stride. */
 static const int kAugParts = 64;
 extern "C" long long pk_frontend_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D) {
     long long b = 0;
@@ -604,22 +661,60 @@ extern "C" long long pk_frontend_noise_rir_workspace_bytes(int B, int n_max, int
     return align256(pk_frontend_workspace_bytes(B, n_max, t_max, n_mel, D)) + noise_rir_extra_bytes(B, n_max, rir_max_len, nullptr);
 }
 
-// the launch sequence of both front-end entry points; nr == nullptr is pk_frontend_fwd (gain and quantisation in one pass)
+// Kaldi fbank frame geometry: FFT size 2^log2_nfft in [2^7, 2^11], 1 <= frame_len <= N, frame_shift >= 1
+static bool fbank_geom_ok(int frame_len, int frame_shift, int log2_nfft) {
+    return log2_nfft >= FB_LOG2_MIN && log2_nfft <= FB_LOG2_MAX && frame_len >= 1 && frame_len <= (1 << log2_nfft) && frame_shift >= 1;
+}
+
+template <int LOG2N>
+static void fbank_launch_n(const float* wave, long long ld_wave, const int* n_len, const int* n_frames, int B, int t_max,
+                           const FbankTables& tb, const FrameGeom& g, int n_mel, float preemph, float* feats, float dither,
+                           uint32_t dither_seed, cudaStream_t st) {
+    fbank_kernel<LOG2N><<<dim3(t_max, B), fbank_threads(LOG2N), 0, st>>>(wave, ld_wave, n_len, n_frames, tb, g, n_mel, preemph, feats,
+                                                                         (long long)t_max * n_mel, t_max, dither, dither_seed);
+}
+
+// feats [B, t_max, n_mel] <- fbank of wave; the geometry has been checked by fbank_geom_ok
+static int fbank_launch(const float* wave, long long ld_wave, const int* n_len, const int* n_frames, int B, int t_max, const float* window,
+                        const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift,
+                        int log2_nfft, int snip_edges, int remove_dc, int n_mel, float preemph, float* feats, float dither,
+                        uint32_t dither_seed, cudaStream_t st) {
+    const FbankTables tb{window, reinterpret_cast<const float2*>(twiddle), mel_w, mel_lo, mel_hi};
+    const FrameGeom g{frame_len, frame_shift, snip_edges ? 1 : 0, remove_dc ? 1 : 0};
+    switch (log2_nfft) {
+        case 7: fbank_launch_n<7>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        case 8: fbank_launch_n<8>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        case 9: fbank_launch_n<9>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        case 10: fbank_launch_n<10>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        case 11: fbank_launch_n<11>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        default: PK_CHECK_ARG(false, "FFT size outside [128, 2048]");
+    }
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
+// the launch sequence of both front-end entry points; nr == nullptr is pk_frontend_fwd (gain and quantisation in one pass).
+// t_max is the number of output rows; the fbank runs over t_max * stride frames, which bounds every n_frames[b].
 static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                            const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx, int rctx,
-                           const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi,
-                           float preemph, int cmn, const float* offset, const float* scale, int f0, int fs, int t0, int ts, void* out,
-                           int out_dtype, short* wave_i16_out, void* workspace, long long workspace_bytes, int* err_flag, float dither,
+                           int stride, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi,
+                           int frame_len, int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, int cmn,
+                           const float* offset, const float* scale, int f0, int fs, int t0, int ts, void* out, int out_dtype,
+                           short* wave_i16_out, void* workspace, long long workspace_bytes, int* err_flag, float dither,
                            unsigned int dither_seed, void* stream, const NoiseRirArgs* nr) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int D = n_mel * (lctx + 1 + rctx);
-    PK_CHECK_ARG(B > 0 && n_max >= FB_FRAME && t_max > 0 && n_mel > 0 && n_mel <= 256 && D <= 1024, "bad frontend dims");
-    PK_CHECK_ARG(workspace_bytes >= pk_frontend_workspace_bytes(B, n_max, t_max, n_mel, D), "frontend workspace too small");
+    PK_CHECK_ARG(B > 0 && n_max > 0 && t_max > 0 && n_mel > 0 && n_mel <= 256 && D <= 1024, "bad frontend dims");
+    PK_CHECK_ARG(fbank_geom_ok(frame_len, frame_shift, log2_nfft), "bad fbank geometry (FFT size 128..2048, 1 <= frame_len <= FFT size)");
+    PK_CHECK_ARG(!snip_edges || n_max >= frame_len, "n_max shorter than one frame");
+    PK_CHECK_ARG(stride >= 1 && (long long)t_max * stride <= 0x7fffffffLL, "bad splice stride");
+    const int t_fb = t_max * stride;
+    PK_CHECK_ARG(workspace_bytes >= pk_frontend_workspace_bytes(B, n_max, t_fb, n_mel, D), "frontend workspace too small");
     unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
     double* resampled = reinterpret_cast<double*>(w); w += (long long)B * n_max * 8;
     double* partial = reinterpret_cast<double*>(w);   w += (long long)B * kAugParts * 8;
     float* wave = reinterpret_cast<float*>(w);        w += (long long)B * n_max * 4;
-    float* feats = reinterpret_cast<float*>(w);       w += (long long)B * t_max * n_mel * 4;
+    float* feats = reinterpret_cast<float*>(w);       w += (long long)B * t_fb * n_mel * 4;
     float* sums = reinterpret_cast<float*>(w);
     dim3 ga(kAugParts, B);
     aug_resample_kernel<<<ga, AUG_THREADS, 0, st>>>(pcm, ld_pcm, n_samples, rate, new_len, resampled, n_max, partial, kAugParts);
@@ -630,7 +725,7 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
         PK_CHECK_LAUNCH(); count_launch();
     } else {
         PK_CHECK_ARG(nr->rir_max_len >= 1 && nr->rir_max_len <= kRirMaxLen, "rir_max_len must be in [1, 65536]");
-        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_max, n_mel, D));
+        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_mel, D));
         ConvGeom g;
         PK_CHECK_ARG(workspace_bytes >= base + noise_rir_extra_bytes(B, n_max, nr->rir_max_len, &g), "frontend workspace too small");
         unsigned char* x = reinterpret_cast<unsigned char*>(workspace) + base;
@@ -654,44 +749,61 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
                                                            new_len, wave, wave_i16_out, n_max, err_flag);
         PK_CHECK_LAUNCH(); count_launch();
     }
-    FbankTables tb{window, reinterpret_cast<const float2*>(twiddle), mel_w, mel_lo, mel_hi};
-    fbank_kernel<<<dim3(t_max, B), 256, 0, st>>>(wave, n_max, n_frames, tb, n_mel, preemph, feats, (long long)t_max * n_mel, t_max, dither,
-                                                 dither_seed);
-    PK_CHECK_LAUNCH(); count_launch();
+    if (fbank_launch(wave, n_max, new_len, n_frames, B, t_fb, window, twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift, log2_nfft,
+                     snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed, st))
+        return -1;
+    const long long ld_fb = (long long)t_fb * n_mel;
     if (cmn) {
         PK_CHECK_CUDA(cudaMemsetAsync(sums, 0, sizeof(float) * B * D, st));
-        splice_colsum_kernel<<<dim3((t_max + 63) / 64, B), ((D + 31) / 32) * 32, 0, st>>>(feats, (long long)t_max * n_mel, n_frames, n_mel, lctx,
-                                                                                        D, t_max, sums);
+        const dim3 grid((t_max + 63) / 64, B);
+        const int threads = ((D + 31) / 32) * 32;
+        if (stride == 1)
+            splice_colsum_kernel<false><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums);
+        else
+            splice_colsum_kernel<true><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums);
         PK_CHECK_LAUNCH(); count_launch();
     }
-    const int gx = (int)(((long long)t_max * D + 255) / 256);
-    if (out_dtype == PK_BF16)
-        splice_finalize_kernel<__nv_bfloat16><<<dim3(gx, B), 256, 0, st>>>(feats, (long long)t_max * n_mel, n_frames, n_mel, lctx, D, t_max,
-                                                                          sums, cmn, offset, scale, f0, fs, t0, ts,
-                                                                          reinterpret_cast<__nv_bfloat16*>(out));
-    else
-        splice_finalize_kernel<float><<<dim3(gx, B), 256, 0, st>>>(feats, (long long)t_max * n_mel, n_frames, n_mel, lctx, D, t_max, sums, cmn,
-                                                                  offset, scale, f0, fs, t0, ts, reinterpret_cast<float*>(out));
+    const dim3 grid((int)(((long long)t_max * D + 255) / 256), B);
+    if (out_dtype == PK_BF16) {
+        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+        if (stride == 1)
+            splice_finalize_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums,
+                                                                               cmn, offset, scale, f0, fs, t0, ts, o);
+        else
+            splice_finalize_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums,
+                                                                              cmn, offset, scale, f0, fs, t0, ts, o);
+    } else {
+        float* o = reinterpret_cast<float*>(out);
+        if (stride == 1)
+            splice_finalize_kernel<float, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums, cmn,
+                                                                       offset, scale, f0, fs, t0, ts, o);
+        else
+            splice_finalize_kernel<float, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums, cmn,
+                                                                      offset, scale, f0, fs, t0, ts, o);
+    }
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }
 
 extern "C" int pk_frontend_fwd(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                                const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
-                               int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
-                               const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
-                               int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
-                               long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream) {
-    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, window, twiddle,
-                           mel_w, mel_lo, mel_hi, preemph, cmn, offset, scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace,
-                           workspace_bytes, err_flag, dither, dither_seed, stream, nullptr);
+                               int rctx, int stride, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
+                               const int* mel_hi, int frame_len, int frame_shift, int log2_nfft, int snip_edges, int remove_dc,
+                               float preemph, int cmn, const float* offset, const float* scale, int f0, int fs, int t0, int ts, void* out,
+                               int out_dtype, short* wave_i16_out, void* workspace, long long workspace_bytes, int* err_flag,
+                               float dither, unsigned int dither_seed, void* stream) {
+    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, stride, window,
+                           twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift, log2_nfft, snip_edges, remove_dc, preemph, cmn, offset,
+                           scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace, workspace_bytes, err_flag, dither, dither_seed,
+                           stream, nullptr);
 }
 
 extern "C" int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                                          const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
-                                         int rctx, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo,
-                                         const int* mel_hi, float preemph, int cmn, const float* offset, const float* scale, int f0,
-                                         int fs, int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                                         int rctx, int stride, const float* window, const float* twiddle, const float* mel_w,
+                                         const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift, int log2_nfft,
+                                         int snip_edges, int remove_dc, float preemph, int cmn, const float* offset, const float* scale,
+                                         int f0, int fs, int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
                                          long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
                                          const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,
                                          const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
@@ -699,19 +811,22 @@ extern "C" int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, con
     PK_CHECK_ARG(!noise || (noise_idx && noise_off && snr && noise_rms_db), "noise bank without its per-utterance draws");
     PK_CHECK_ARG(!rir || (rir_off && rir_len && rir_idx), "RIR bank without its offsets, lengths or per-utterance draws");
     const NoiseRirArgs nr{noise, noise_idx, noise_off, snr, noise_rms_db, rir, rir_off, rir_len, rir_idx, rir_max_len};
-    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, window, twiddle,
-                           mel_w, mel_lo, mel_hi, preemph, cmn, offset, scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace,
-                           workspace_bytes, err_flag, dither, dither_seed, stream, &nr);
+    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, stride, window,
+                           twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift, log2_nfft, snip_edges, remove_dc, preemph, cmn, offset,
+                           scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace, workspace_bytes, err_flag, dither, dither_seed,
+                           stream, &nr);
 }
 
 /* feats-only entry (fbank of already-augmented int16-scaled samples), used by parity tests and by
  * utils/compute_global_cmvn-style tooling: wave f32 [B, ld_wave] -> feats f32 [B, t_max, n_mel]. */
-extern "C" int pk_fbank(const float* wave, long long ld_wave, const int* n_frames, int B, int t_max, int n_mel, const float* window,
-                        const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, float preemph, float* feats,
-                        float dither, unsigned int dither_seed, void* stream) {
-    FbankTables tb{window, reinterpret_cast<const float2*>(twiddle), mel_w, mel_lo, mel_hi};
-    fbank_kernel<<<dim3(t_max, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(wave, ld_wave, n_frames, tb, n_mel, preemph, feats,
-                                                                                  (long long)t_max * n_mel, t_max, dither, dither_seed);
-    PK_CHECK_LAUNCH(); count_launch();
-    return 0;
+extern "C" int pk_fbank(const float* wave, long long ld_wave, const int* n_samples, const int* n_frames, int B, int t_max, int n_mel,
+                        const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len,
+                        int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, float* feats, float dither,
+                        unsigned int dither_seed, void* stream) {
+    PK_CHECK_ARG(B > 0 && t_max > 0 && n_mel > 0 && n_mel <= 256, "bad fbank dims");
+    PK_CHECK_ARG(fbank_geom_ok(frame_len, frame_shift, log2_nfft), "bad fbank geometry (FFT size 128..2048, 1 <= frame_len <= FFT size)");
+    PK_CHECK_ARG(snip_edges || n_samples, "snip_edges = 0 needs the sample counts");
+    return fbank_launch(wave, ld_wave, n_samples, n_frames, B, t_max, window, twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift,
+                        log2_nfft, snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed,
+                        reinterpret_cast<cudaStream_t>(stream));
 }

@@ -97,10 +97,19 @@ def put_thread(q, generator, *gen_args):
             break
 
 
+def feature_options(args):
+    """the fbank options of ``--feat_config`` (Kaldi's defaults with ``--feats_dim`` bins without one); ``--sample_rate`` must be the
+    config's sample frequency, as Kaldi's ComputeFeatures requires of the waveform's rate"""
+    opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
+    if float(args.sample_rate) != opts.sample_frequency:
+        raise ValueError("--sample_rate %s differs from the feature config's --sample-frequency=%g" % (args.sample_rate, opts.sample_frequency))
+    return opts
+
+
 def otf_utt_generator(data_triplets, rir, noise, args):
     """raw-PCM batches for one worker; mirrors the control flow of loader/otf_utt_loader.py:165-299"""
-    if args.stride != 1:
-        raise NotImplementedError("pika_b200 loader: --stride 1 only (the recipes never subsample in the loader)")
+    geometry = feature_options(args).geometry()
+    stride = args.stride
     batch_size = args.batch_size
     speed_rate = [float(r) for r in args.speed_rate.split(',')]
     gain_lo, gain_hi = [-float(g) for g in args.gain_range.split(',')]
@@ -113,7 +122,7 @@ def otf_utt_generator(data_triplets, rir, noise, args):
             assert uttid == uttid1
             spr = speed_rate[randint(0, len(speed_rate) - 1)]
             target_db = np.random.uniform(gain_lo, gain_hi)
-            new_len, frames = Frontend.lengths([audio_np.shape[0]], [spr])
+            new_len, frames = Frontend.lengths([audio_np.shape[0]], [spr], **geometry)
             draws = draw_noise_rir(new_len[0], noise, rir, snr_mu_sigma)
             ali = np.array(ali)
             if args.reverse_labels:
@@ -122,11 +131,11 @@ def otf_utt_generator(data_triplets, rir, noise, args):
                 ali = np.concatenate(([args.SOS], ali))
             if args.EOS >= 0:
                 ali = np.concatenate((ali, [args.EOS]))
-            utt_len = frames[0]
+            utt_len = frames[0] // stride + int(frames[0] % stride != 0)           # rows after the stride (:243-247)
             if utt_len > 0 and utt_len <= args.max_len and ali.shape[0] * utt_len // 3 <= args.TU_limit:
                 pcm.append(audio_np)
                 tgt.append(ali.astype(np.int32))
-                meta.append((audio_np.shape[0], spr, target_db, new_len[0], utt_len) + draws)
+                meta.append((audio_np.shape[0], spr, target_db, new_len[0], frames[0], utt_len) + draws)
             batch_idx += 1
             if batch_idx == batch_size:
                 yield assemble(pcm, tgt, meta, args, rir)
@@ -136,8 +145,9 @@ def otf_utt_generator(data_triplets, rir, noise, args):
 
 def assemble(pcm, tgt, meta, args, rir=None):
     """padded raw batch (or the reference's empty-batch tuple, loader/otf_utt_loader.py:283-287).  meta rows:
-    (n_samples, rate, target_db, new_len, n_frames[, snr, noise_idx, noise_off, rir_idx]); the noise keys (noise_idx, noise_off,
-    snr) and the RIR keys (rir_idx, and the host-side rir_max_len) are added only when those draws were made."""
+    (n_samples, rate, target_db, new_len, n_frames, utt_len[, snr, noise_idx, noise_off, rir_idx]) with n_frames the fbank frames and
+    utt_len the rows after the stride; t_max and lens count rows.  The noise keys (noise_idx, noise_off, snr) and the RIR keys
+    (rir_idx, and the host-side rir_max_len) are added only when those draws were made."""
     if not pcm:
         return None, None, torch.IntTensor([0]), torch.IntTensor([0])
     B = len(pcm)
@@ -155,15 +165,15 @@ def assemble(pcm, tgt, meta, args, rir=None):
                target_db=torch.tensor([m[2] for m in meta], dtype=torch.float32),
                new_len=torch.tensor([m[3] for m in meta], dtype=torch.int32),
                n_frames=torch.tensor([m[4] for m in meta], dtype=torch.int32),
-               t_max=max(m[4] for m in meta))
-    if len(meta[0]) > 5 and meta[0][5] is not None:
-        raw.update(noise_idx=torch.tensor([m[6] for m in meta], dtype=torch.int32),
-                   noise_off=torch.tensor([m[7] for m in meta], dtype=torch.int64),
-                   snr=torch.tensor([m[5] for m in meta], dtype=torch.float64))
-    if len(meta[0]) > 5 and meta[0][8] is not None:
-        raw.update(rir_idx=torch.tensor([m[8] for m in meta], dtype=torch.int32),
-                   rir_max_len=int(max(rir.lengths[m[8]] for m in meta)))
-    lens = raw["n_frames"].clone()
+               t_max=max(m[5] for m in meta))
+    if len(meta[0]) > 6 and meta[0][6] is not None:
+        raw.update(noise_idx=torch.tensor([m[7] for m in meta], dtype=torch.int32),
+                   noise_off=torch.tensor([m[8] for m in meta], dtype=torch.int64),
+                   snr=torch.tensor([m[6] for m in meta], dtype=torch.float64))
+    if len(meta[0]) > 6 and meta[0][9] is not None:
+        raw.update(rir_idx=torch.tensor([m[9] for m in meta], dtype=torch.int32),
+                   rir_max_len=int(max(rir.lengths[m[9]] for m in meta)))
+    lens = torch.tensor([m[5] for m in meta], dtype=torch.int32)
     ali_lens = torch.tensor([len(t) for t in tgt], dtype=torch.int32)
     return raw, target, lens, ali_lens
 
@@ -172,12 +182,12 @@ _frontends = {}
 
 
 def _frontend_for(args, device):
-    key = (args.feat_config, args.lctx, args.rctx, str(device))
+    key = (args.feat_config, args.feats_dim, args.sample_rate, args.lctx, args.rctx, args.stride, str(device))
     if key not in _frontends:
-        opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
+        opts = feature_options(args)
         if getattr(args, "no_dither", False):          # explicit opt-out (parity runs); otherwise the feature config decides
             opts.dither = 0.0
-        _frontends[key] = Frontend(opts, args.lctx, args.rctx, device)
+        _frontends[key] = Frontend(opts, args.lctx, args.rctx, device, stride=args.stride)
     return _frontends[key]
 
 
@@ -200,6 +210,7 @@ def dataloader(data_lst, rir, noise, args):
         data_lst: list of mrk and seq of input audios, and label ark
         rir, noise: ``AudioBank`` (loader/audio_bank.py) for on-the-fly reverberation / noise, or empty lists for none
     """
+    feature_options(args)                      # a config the front end cannot run fails here, before any worker starts
     data_triplets = kaldi_io.read_lst(data_lst)
     num_per_worker = (len(data_triplets) + args.num_workers - 1) // args.num_workers
     lst = [data_triplets[i:i + num_per_worker] for i in range(0, len(data_triplets), num_per_worker)]

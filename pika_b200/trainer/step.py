@@ -30,8 +30,8 @@ class TrainStep:
         self.num_done = 0
 
     def features(self, batch):
-        """batch: dict of device tensors (pcm int16 [B,n], n_samples, rate, target_db, new_len, n_frames) + t_max, and the
-        noise / reverberation draws when the loader made them (loader/otf_utt_loader.py: assemble)"""
+        """batch: dict of device tensors (pcm int16 [B,n], n_samples, rate, target_db, new_len, n_frames) + t_max (rows after the
+        front end's stride), and the noise / reverberation draws when the loader made them (loader/otf_utt_loader.py: assemble)"""
         a = self.args
         sa = (0, 0, 0, 0)
         if self.spec is not None:
@@ -48,7 +48,7 @@ class TrainStep:
         a = self.args
         self.opt.flat.zero_grad()                                         # optimizer.zero_grad()
         feats = self.features(batch)
-        len_batch = encoder_out_lens(batch["n_frames"], a.model_lctx, a.model_rctx, a.model_stride)
+        len_batch = encoder_out_lens(self.frontend.out_lens(batch["n_frames"]), a.model_lctx, a.model_rctx, a.model_stride)
         t_out = encoder_out_max(int(batch["t_max"]), a.model_lctx, a.model_rctx, a.model_stride)
         costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out)
         engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1

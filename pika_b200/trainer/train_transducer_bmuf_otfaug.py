@@ -16,7 +16,7 @@ import sys
 
 import torch
 
-from ..frontend import FbankOptions, Frontend
+from ..frontend import Frontend
 from ..loader.audio_bank import AudioBank
 from ..loader import kaldi_io
 from ..utils.logger import Logger
@@ -60,7 +60,7 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
                 with torch.no_grad():
                     feats = step.features(batch)
                     from .step import encoder_out_lens, encoder_out_max
-                    tl = encoder_out_lens(batch["n_frames"], args.model_lctx, args.model_rctx, args.model_stride)
+                    tl = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
                     t_out = encoder_out_max(int(batch["t_max"]), args.model_lctx, args.model_rctx, args.model_stride)
                     costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
             loss = float(costs.sum().item())
@@ -186,10 +186,10 @@ def main(argv=None):
                                                                                 args.rnn_type, num_param / 1000 / 1000))
     log_f.write('*' * 60 + '\n')
     log_f.flush()
-    opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
+    opts = loader_module.feature_options(args)
     # opts.dither is honoured (egs/fbank.conf: dither=1): counter-based Gaussian dither in the fbank kernel; set dither=0 in the
     # feature config for bit-reproducible features (Kaldi's own RNG stream is not reproduced, DESIGN.md)
-    args.frontend = Frontend(opts, args.lctx, args.rctx, dev)
+    args.frontend = Frontend(opts, args.lctx, args.rctx, dev, stride=args.stride)
     args.frontend.noise = args.noise or None
     args.frontend.rir = args.rir or None
     args.offset = args.scale = None

@@ -18,7 +18,7 @@ import torch
 
 from ..decoder.beam_transducer import GlobalScorer
 from ..decoder.transducer_decoder import TransducerDecoder
-from ..frontend import FbankOptions, Frontend
+from ..frontend import Frontend
 from ..loader.audio_bank import AudioBank
 from ..loader import kaldi_io
 from ..utils.logger import Logger
@@ -58,7 +58,7 @@ def run_one_epoch(epoch, log_f, model, args, bmuf_trainer):
             target = target_cpu.long().to(dev)
             ali_lens = ali_lens_cpu.to(dev)
             feats = step.features(batch)                                      # CMN / CMVN, no SpecAugment yet (:109-115)
-            len_batch = encoder_out_lens(batch["n_frames"], args.model_lctx, args.model_rctx, args.model_stride)
+            len_batch = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
             model.eval()                                                      # N-best generation (:117-123)
             ret, _ = decoder.decode_batch(feats, len_batch.cpu(), [int(t) + int(u) + 3 for t, u in zip(len_batch.cpu(), ali_lens_cpu)])
             model.train()
@@ -137,8 +137,8 @@ def main(argv=None):
     model.to(dev)
     flat = FlatParams(model)
     bmuf_trainer = BmufTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr, flat=flat)
-    opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
-    args.frontend = Frontend(opts, args.lctx, args.rctx, dev)
+    opts = loader_module.feature_options(args)
+    args.frontend = Frontend(opts, args.lctx, args.rctx, dev, stride=args.stride)
     args.frontend.noise = args.noise or None
     args.frontend.rir = args.rir or None
     args.offset = args.scale = None

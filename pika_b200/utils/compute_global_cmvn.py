@@ -37,6 +37,8 @@ def main(argv=None):
         sys.exit("pika_b200.utils.compute_global_cmvn: the front end runs on the GPU only")
     dev = torch.device("cuda", 0)
     opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feat_dim)
+    if float(args.sample_rate) != opts.sample_frequency:
+        raise ValueError("--sample_rate %s differs from the feature config's --sample-frequency=%g" % (args.sample_rate, opts.sample_frequency))
     assert opts.num_mel_bins == args.feat_dim, "--feat_dim must match num-mel-bins of the feature config"
     fe = Frontend(opts, 0, 0, dev)
     speed_rate = [0.9, 1.0, 1.1]
@@ -48,7 +50,7 @@ def main(argv=None):
             return
         B = len(pcms)
         ns = [len(p) for p in pcms]
-        new_len, frames = Frontend.lengths(ns, rates)
+        new_len, frames = Frontend.lengths(ns, rates, **opts.geometry())
         n_max, t_max = max(max(ns), max(new_len)), max(frames)
         if t_max == 0:
             return
