@@ -363,6 +363,35 @@ int pk_frontend_fwd_noise_rir(const short* pcm, long long ld_pcm, const int* n_s
                               const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
                               const int* rir_idx, int rir_max_len);
 
+/* Kaldi MFCC (feat/feature-mfcc.cc MfccComputer::Compute) in place of fbank: the same frames, window, FFT and mel banks, then per frame
+ * c = dct . log(max(mel, FLT_EPSILON)), and
+ *   dct          [n_mel, num_ceps] f32: the first num_ceps rows of the orthonormal DCT-II of size n_mel, each times its lifter
+ *                coefficient 1 + Q/2 sin(pi k / Q) (Q = --cepstral-lifter, none when 0), stored transposed; 1 <= num_ceps <= n_mel
+ *   use_energy   c0 <- log(max(E, FLT_EPSILON)), raised to log(energy_floor) when energy_floor > 0; E is the sum of squares of the
+ *                window after dither and DC removal (raw_energy) or of the windowed, pre-emphasised frame (otherwise)
+ *   htk_compat   c0 (or the energy) moves to the last column; without use_energy it is multiplied by sqrt(2)
+ * Features are num_ceps wide: the splice, CMN/CMVN and SpecAugment stages and the workspace queries take num_ceps where the fbank
+ * entry points take n_mel (D = num_ceps * (lctx + 1 + rctx)).
+ * pk_mfcc: arguments up to `stream` are those of pk_fbank; feats [B, t_max, num_ceps].
+ * pk_frontend_fwd_mfcc: arguments up to `rir_max_len` are those of pk_frontend_fwd_noise_rir, whose banks may both be null (then the
+ * sequence of pk_frontend_fwd runs, and pk_frontend_workspace_bytes suffices). */
+int pk_mfcc(const float* wave, long long ld_wave, const int* n_samples, const int* n_frames, int B, int t_max, int n_mel,
+            const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len,
+            int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, float* feats, float dither,
+            unsigned int dither_seed, void* stream, const float* dct, int num_ceps, int use_energy, int raw_energy,
+            float energy_floor, int htk_compat);
+int pk_frontend_fwd_mfcc(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                         const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
+                         int rctx, int stride, const float* window, const float* twiddle, const float* mel_w,
+                         const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift, int log2_nfft, int snip_edges,
+                         int remove_dc, float preemph, int cmn, const float* offset, const float* scale, int f0, int fs,
+                         int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                         long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
+                         const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,
+                         const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
+                         const int* rir_idx, int rir_max_len, const float* dct, int num_ceps, int use_energy,
+                         int raw_energy, float energy_floor, int htk_compat);
+
 /* scipy.signal.fftconvolve(x, h, "same") in float64 for ragged batches: x [B, ld_x] (lengths n_len), h [B, ld_h] (lengths
  * m_len, 1 <= m_len <= m_max <= 65536) -> y [B, ld_y], n_len[b] samples each (y may alias x).  Workspace:
  * pk_conv_same_f64_workspace_bytes (< 0 on bad dims). */

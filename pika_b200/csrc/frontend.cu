@@ -404,6 +404,12 @@ struct FrameGeom {          // Kaldi FrameExtractionOptions, in samples
     int frame_len, frame_shift, snip_edges, remove_dc;
 };
 
+struct MfccParams {         // Kaldi MfccOptions past the mel banks (feat/feature-mfcc.cc); unused by the fbank instances
+    const float* dct;       // [n_mel][num_ceps]: DCT-II rows times the lifter, transposed so that a frame's coefficients read coalesced
+    int num_ceps, use_energy, raw_energy, htk_compat;
+    float energy_floor;     // floor of the energy when > 0 (linear, as --energy-floor)
+};
+
 // N/2 butterflies per stage, one per thread; at least 256 threads so that every mel bin (n_mel <= 256) has one
 constexpr int fbank_threads(int log2n) { return (1 << (log2n - 1)) < 256 ? 256 : (1 << (log2n - 1)); }
 
@@ -427,12 +433,17 @@ PK_DEVICE long long reflect_index(long long s, long long n) {
 // explicit roundings: DC removal fused into the subtraction of the window's sum times -1/frame_len, pre-emphasis as
 // fma(-c, prev, cur), the complex products and |X|^2 with the first product fused -- the same operations, in the same order, at
 // every FFT size.
-template <int LOG2N>
+//
+// MFCC = true swaps the epilogue for Kaldi's MfccComputer::Compute: the log mel energies go to shared memory and each of the first
+// num_ceps threads forms one cepstral coefficient, then the frame's log energy replaces c0 (use_energy) and HTK ordering moves c0 last.
+// The energy is summed per thread in the pre-emphasis loop, after dither and DC removal (raw_energy, Kaldi's ProcessWindow) or of the
+// windowed frame (otherwise).  The fbank instances (MFCC = false) compile to the code they had before the epilogue was added.
+template <int LOG2N, bool MFCC>
 __global__ void __launch_bounds__(fbank_threads(LOG2N), 2048 / fbank_threads(LOG2N)) fbank_kernel(const float* __restrict__ wave, long long ld_wave,
                                                                      const int* __restrict__ n_len, const int* __restrict__ n_frames,
                                                                      FbankTables tb, FrameGeom g, int n_mel, float preemph,
                                                                      float* __restrict__ feats, long long ld_b, int t_max, float dither,
-                                                                     uint32_t dither_seed) {
+                                                                     uint32_t dither_seed, MfccParams mp) {
     constexpr int N = 1 << LOG2N, NB = N / 2, THREADS = fbank_threads(LOG2N), WARPS = THREADS / 32;
     constexpr int PER_THREAD = (N + THREADS - 1) / THREADS;
     const int t = blockIdx.x, b = blockIdx.y;
@@ -478,6 +489,7 @@ __global__ void __launch_bounds__(fbank_threads(LOG2N), 2048 / fbank_threads(LOG
         neg_inv_len = -(1.0f / (float)L);
     }
     // DC removal, pre-emphasis (x[i] -= c*x[i-1], x[0] -= c*x[0]), window, zero-pad, bit-reversed placement
+    float energy = 0.f;                                 // MFCC: this thread's part of the frame's sum of squares
 #pragma unroll
     for (int j = 0; j < PER_THREAD; ++j) {
         const int i = tid + j * THREADS;
@@ -487,10 +499,19 @@ __global__ void __launch_bounds__(fbank_threads(LOG2N), 2048 / fbank_threads(LOG
                 const float cur = __fmaf_rn(sum, neg_inv_len, frame[i]);
                 const float prev = __fmaf_rn(sum, neg_inv_len, i > 0 ? frame[i - 1] : frame[0]);
                 v = __fmul_rn(__fmaf_rn(-preemph, prev, cur), tb.window[i]);
+                if constexpr (MFCC) {
+                    const float x = mp.raw_energy ? cur : v;
+                    energy = __fmaf_rn(x, x, energy);
+                }
             }
             const int r = __brev((unsigned)i) >> (32 - LOG2N);
             buf[r] = make_float2(v, 0.f);
         }
+    }
+    __shared__ float ered[MFCC ? WARPS : 1];
+    if constexpr (MFCC) {
+        energy = warp_sum(energy);
+        if ((tid & 31) == 0) ered[tid >> 5] = energy;   // read after the FFT's barriers
     }
     __syncthreads();
     // LOG2N radix-2 stages of N/2 butterflies, one per thread
@@ -510,11 +531,36 @@ __global__ void __launch_bounds__(fbank_threads(LOG2N), 2048 / fbank_threads(LOG
     }
     if (NB == THREADS || tid < NB) power[tid] = __fmaf_rn(buf[tid].x, buf[tid].x, __fmul_rn(buf[tid].y, buf[tid].y));
     __syncthreads();
+    __shared__ float logmel[MFCC ? 256 : 1];
     if (tid < n_mel) {
         float e = 0.f;
         const float* w = tb.mel_w + (long long)tid * NB;
         for (int k = tb.mel_lo[tid]; k < tb.mel_hi[tid]; ++k) e = __fmaf_rn(w[k], power[k], e);
-        feats[(long long)b * ld_b + (long long)t * n_mel + tid] = logf(fmaxf(e, 1.1920928955078125e-07f));
+        if constexpr (MFCC)
+            logmel[tid] = logf(fmaxf(e, 1.1920928955078125e-07f));
+        else
+            feats[(long long)b * ld_b + (long long)t * n_mel + tid] = logf(fmaxf(e, 1.1920928955078125e-07f));
+    }
+    if constexpr (MFCC) {
+        __syncthreads();
+        const int nc = mp.num_ceps;
+        if (tid < nc) {
+            float c = 0.f;
+            for (int j = 0; j < n_mel; ++j) c = __fmaf_rn(mp.dct[j * nc + tid], logmel[j], c);
+            if (tid == 0) {
+                if (mp.use_energy) {
+                    float e = 0.f;
+#pragma unroll
+                    for (int w = 0; w < WARPS; ++w) e += ered[w];
+                    c = logf(fmaxf(e, 1.1920928955078125e-07f));
+                    if (mp.energy_floor > 0.f) c = fmaxf(c, logf(mp.energy_floor));
+                } else if (mp.htk_compat) {
+                    c = __fmul_rn(c, 1.41421356237309505f);
+                }
+            }
+            const int col = mp.htk_compat ? (tid == 0 ? nc - 1 : tid - 1) : tid;
+            feats[(long long)b * ld_b + (long long)t * nc + col] = c;
+        }
     }
 }
 
@@ -666,55 +712,70 @@ static bool fbank_geom_ok(int frame_len, int frame_shift, int log2_nfft) {
     return log2_nfft >= FB_LOG2_MIN && log2_nfft <= FB_LOG2_MAX && frame_len >= 1 && frame_len <= (1 << log2_nfft) && frame_shift >= 1;
 }
 
+// mp == nullptr: fbank, feats [B, t_max, n_mel]; otherwise MFCC, feats [B, t_max, num_ceps]
 template <int LOG2N>
 static void fbank_launch_n(const float* wave, long long ld_wave, const int* n_len, const int* n_frames, int B, int t_max,
                            const FbankTables& tb, const FrameGeom& g, int n_mel, float preemph, float* feats, float dither,
-                           uint32_t dither_seed, cudaStream_t st) {
-    fbank_kernel<LOG2N><<<dim3(t_max, B), fbank_threads(LOG2N), 0, st>>>(wave, ld_wave, n_len, n_frames, tb, g, n_mel, preemph, feats,
-                                                                         (long long)t_max * n_mel, t_max, dither, dither_seed);
+                           uint32_t dither_seed, const MfccParams* mp, cudaStream_t st) {
+    const dim3 grid(t_max, B);
+    if (!mp)
+        fbank_kernel<LOG2N, false><<<grid, fbank_threads(LOG2N), 0, st>>>(wave, ld_wave, n_len, n_frames, tb, g, n_mel, preemph, feats,
+                                                                          (long long)t_max * n_mel, t_max, dither, dither_seed,
+                                                                          MfccParams{});
+    else
+        fbank_kernel<LOG2N, true><<<grid, fbank_threads(LOG2N), 0, st>>>(wave, ld_wave, n_len, n_frames, tb, g, n_mel, preemph, feats,
+                                                                         (long long)t_max * mp->num_ceps, t_max, dither, dither_seed, *mp);
 }
 
-// feats [B, t_max, n_mel] <- fbank of wave; the geometry has been checked by fbank_geom_ok
+// feats <- fbank (mp == nullptr) or MFCC of wave; the geometry has been checked by fbank_geom_ok, the MFCC arguments by mfcc_ok
 static int fbank_launch(const float* wave, long long ld_wave, const int* n_len, const int* n_frames, int B, int t_max, const float* window,
                         const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift,
                         int log2_nfft, int snip_edges, int remove_dc, int n_mel, float preemph, float* feats, float dither,
-                        uint32_t dither_seed, cudaStream_t st) {
+                        uint32_t dither_seed, cudaStream_t st, const MfccParams* mp = nullptr) {
     const FbankTables tb{window, reinterpret_cast<const float2*>(twiddle), mel_w, mel_lo, mel_hi};
     const FrameGeom g{frame_len, frame_shift, snip_edges ? 1 : 0, remove_dc ? 1 : 0};
     switch (log2_nfft) {
-        case 7: fbank_launch_n<7>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
-        case 8: fbank_launch_n<8>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
-        case 9: fbank_launch_n<9>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
-        case 10: fbank_launch_n<10>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
-        case 11: fbank_launch_n<11>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, st); break;
+        case 7: fbank_launch_n<7>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, mp, st); break;
+        case 8: fbank_launch_n<8>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, mp, st); break;
+        case 9: fbank_launch_n<9>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, mp, st); break;
+        case 10: fbank_launch_n<10>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, mp, st); break;
+        case 11: fbank_launch_n<11>(wave, ld_wave, n_len, n_frames, B, t_max, tb, g, n_mel, preemph, feats, dither, dither_seed, mp, st); break;
         default: PK_CHECK_ARG(false, "FFT size outside [128, 2048]");
     }
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }
 
-// the launch sequence of both front-end entry points; nr == nullptr is pk_frontend_fwd (gain and quantisation in one pass).
-// t_max is the number of output rows; the fbank runs over t_max * stride frames, which bounds every n_frames[b].
+// the MFCC epilogue's arguments: 1 <= num_ceps <= n_mel (Kaldi: "num-ceps cannot be larger than num-mel-bins"), a DCT table
+static bool mfcc_ok(const MfccParams& mp, int n_mel) {
+    return mp.dct && mp.num_ceps >= 1 && mp.num_ceps <= n_mel;
+}
+
+// the launch sequence of every front-end entry point; nr == nullptr is pk_frontend_fwd (gain and quantisation in one pass), mp == nullptr
+// fbank features (n_mel per frame), otherwise MFCC (num_ceps per frame).  t_max is the number of output rows; the fbank runs over
+// t_max * stride frames, which bounds every n_frames[b].
 static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
                            const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx, int rctx,
                            int stride, const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi,
                            int frame_len, int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, int cmn,
                            const float* offset, const float* scale, int f0, int fs, int t0, int ts, void* out, int out_dtype,
                            short* wave_i16_out, void* workspace, long long workspace_bytes, int* err_flag, float dither,
-                           unsigned int dither_seed, void* stream, const NoiseRirArgs* nr) {
+                           unsigned int dither_seed, void* stream, const NoiseRirArgs* nr, const MfccParams* mp = nullptr) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const int D = n_mel * (lctx + 1 + rctx);
+    PK_CHECK_ARG(!mp || mfcc_ok(*mp, n_mel), "bad MFCC arguments (1 <= num_ceps <= n_mel and a DCT table)");
+    const int n_feat = mp ? mp->num_ceps : n_mel;     // per-frame width of the features the splice reads
+    const int D = n_feat * (lctx + 1 + rctx);
     PK_CHECK_ARG(B > 0 && n_max > 0 && t_max > 0 && n_mel > 0 && n_mel <= 256 && D <= 1024, "bad frontend dims");
     PK_CHECK_ARG(fbank_geom_ok(frame_len, frame_shift, log2_nfft), "bad fbank geometry (FFT size 128..2048, 1 <= frame_len <= FFT size)");
     PK_CHECK_ARG(!snip_edges || n_max >= frame_len, "n_max shorter than one frame");
     PK_CHECK_ARG(stride >= 1 && (long long)t_max * stride <= 0x7fffffffLL, "bad splice stride");
     const int t_fb = t_max * stride;
-    PK_CHECK_ARG(workspace_bytes >= pk_frontend_workspace_bytes(B, n_max, t_fb, n_mel, D), "frontend workspace too small");
+    PK_CHECK_ARG(workspace_bytes >= pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D), "frontend workspace too small");
     unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
     double* resampled = reinterpret_cast<double*>(w); w += (long long)B * n_max * 8;
     double* partial = reinterpret_cast<double*>(w);   w += (long long)B * kAugParts * 8;
     float* wave = reinterpret_cast<float*>(w);        w += (long long)B * n_max * 4;
-    float* feats = reinterpret_cast<float*>(w);       w += (long long)B * t_fb * n_mel * 4;
+    float* feats = reinterpret_cast<float*>(w);       w += (long long)B * t_fb * n_feat * 4;
     float* sums = reinterpret_cast<float*>(w);
     dim3 ga(kAugParts, B);
     aug_resample_kernel<<<ga, AUG_THREADS, 0, st>>>(pcm, ld_pcm, n_samples, rate, new_len, resampled, n_max, partial, kAugParts);
@@ -725,7 +786,7 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
         PK_CHECK_LAUNCH(); count_launch();
     } else {
         PK_CHECK_ARG(nr->rir_max_len >= 1 && nr->rir_max_len <= kRirMaxLen, "rir_max_len must be in [1, 65536]");
-        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_mel, D));
+        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D));
         ConvGeom g;
         PK_CHECK_ARG(workspace_bytes >= base + noise_rir_extra_bytes(B, n_max, nr->rir_max_len, &g), "frontend workspace too small");
         unsigned char* x = reinterpret_cast<unsigned char*>(workspace) + base;
@@ -750,35 +811,35 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
         PK_CHECK_LAUNCH(); count_launch();
     }
     if (fbank_launch(wave, n_max, new_len, n_frames, B, t_fb, window, twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift, log2_nfft,
-                     snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed, st))
+                     snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed, st, mp))
         return -1;
-    const long long ld_fb = (long long)t_fb * n_mel;
+    const long long ld_fb = (long long)t_fb * n_feat;
     if (cmn) {
         PK_CHECK_CUDA(cudaMemsetAsync(sums, 0, sizeof(float) * B * D, st));
         const dim3 grid((t_max + 63) / 64, B);
         const int threads = ((D + 31) / 32) * 32;
         if (stride == 1)
-            splice_colsum_kernel<false><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums);
+            splice_colsum_kernel<false><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums);
         else
-            splice_colsum_kernel<true><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums);
+            splice_colsum_kernel<true><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums);
         PK_CHECK_LAUNCH(); count_launch();
     }
     const dim3 grid((int)(((long long)t_max * D + 255) / 256), B);
     if (out_dtype == PK_BF16) {
         __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
         if (stride == 1)
-            splice_finalize_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums,
+            splice_finalize_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums,
                                                                                cmn, offset, scale, f0, fs, t0, ts, o);
         else
-            splice_finalize_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums,
+            splice_finalize_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums,
                                                                               cmn, offset, scale, f0, fs, t0, ts, o);
     } else {
         float* o = reinterpret_cast<float*>(out);
         if (stride == 1)
-            splice_finalize_kernel<float, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums, cmn,
+            splice_finalize_kernel<float, false><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums, cmn,
                                                                        offset, scale, f0, fs, t0, ts, o);
         else
-            splice_finalize_kernel<float, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_mel, lctx, stride, D, t_max, sums, cmn,
+            splice_finalize_kernel<float, true><<<grid, 256, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums, cmn,
                                                                       offset, scale, f0, fs, t0, ts, o);
     }
     PK_CHECK_LAUNCH(); count_launch();
@@ -829,4 +890,43 @@ extern "C" int pk_fbank(const float* wave, long long ld_wave, const int* n_sampl
     return fbank_launch(wave, ld_wave, n_samples, n_frames, B, t_max, window, twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift,
                         log2_nfft, snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed,
                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+/* MFCC counterpart of pk_fbank: wave f32 [B, ld_wave] -> feats f32 [B, t_max, num_ceps] */
+extern "C" int pk_mfcc(const float* wave, long long ld_wave, const int* n_samples, const int* n_frames, int B, int t_max, int n_mel,
+                       const float* window, const float* twiddle, const float* mel_w, const int* mel_lo, const int* mel_hi, int frame_len,
+                       int frame_shift, int log2_nfft, int snip_edges, int remove_dc, float preemph, float* feats, float dither,
+                       unsigned int dither_seed, void* stream, const float* dct, int num_ceps, int use_energy, int raw_energy,
+                       float energy_floor, int htk_compat) {
+    const MfccParams mp{dct, num_ceps, use_energy ? 1 : 0, raw_energy ? 1 : 0, htk_compat ? 1 : 0, energy_floor};
+    PK_CHECK_ARG(B > 0 && t_max > 0 && n_mel > 0 && n_mel <= 256, "bad fbank dims");
+    PK_CHECK_ARG(mfcc_ok(mp, n_mel), "bad MFCC arguments (1 <= num_ceps <= n_mel and a DCT table)");
+    PK_CHECK_ARG(fbank_geom_ok(frame_len, frame_shift, log2_nfft), "bad fbank geometry (FFT size 128..2048, 1 <= frame_len <= FFT size)");
+    PK_CHECK_ARG(snip_edges || n_samples, "snip_edges = 0 needs the sample counts");
+    return fbank_launch(wave, ld_wave, n_samples, n_frames, B, t_max, window, twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift,
+                        log2_nfft, snip_edges, remove_dc, n_mel, preemph, feats, dither, dither_seed,
+                        reinterpret_cast<cudaStream_t>(stream), &mp);
+}
+
+/* the whole front end with MFCC features: the arguments of pk_frontend_fwd_noise_rir (null banks = no noise / no RIR), then the
+ * MFCC epilogue's */
+extern "C" int pk_frontend_fwd_mfcc(const short* pcm, long long ld_pcm, const int* n_samples, const float* rate, const int* new_len,
+                                    const float* target_db, const int* n_frames, int B, int n_max, int t_max, int n_mel, int lctx,
+                                    int rctx, int stride, const float* window, const float* twiddle, const float* mel_w,
+                                    const int* mel_lo, const int* mel_hi, int frame_len, int frame_shift, int log2_nfft,
+                                    int snip_edges, int remove_dc, float preemph, int cmn, const float* offset, const float* scale,
+                                    int f0, int fs, int t0, int ts, void* out, int out_dtype, short* wave_i16_out, void* workspace,
+                                    long long workspace_bytes, int* err_flag, float dither, unsigned int dither_seed, void* stream,
+                                    const short* noise, const int* noise_idx, const long long* noise_off, const double* snr,
+                                    const double* noise_rms_db, const short* rir, const long long* rir_off, const int* rir_len,
+                                    const int* rir_idx, int rir_max_len, const float* dct, int num_ceps, int use_energy,
+                                    int raw_energy, float energy_floor, int htk_compat) {
+    PK_CHECK_ARG(!noise || (noise_idx && noise_off && snr && noise_rms_db), "noise bank without its per-utterance draws");
+    PK_CHECK_ARG(!rir || (rir_off && rir_len && rir_idx), "RIR bank without its offsets, lengths or per-utterance draws");
+    const NoiseRirArgs nr{noise, noise_idx, noise_off, snr, noise_rms_db, rir, rir_off, rir_len, rir_idx, rir_max_len};
+    const MfccParams mp{dct, num_ceps, use_energy ? 1 : 0, raw_energy ? 1 : 0, htk_compat ? 1 : 0, energy_floor};
+    return frontend_launch(pcm, ld_pcm, n_samples, rate, new_len, target_db, n_frames, B, n_max, t_max, n_mel, lctx, rctx, stride, window,
+                           twiddle, mel_w, mel_lo, mel_hi, frame_len, frame_shift, log2_nfft, snip_edges, remove_dc, preemph, cmn, offset,
+                           scale, f0, fs, t0, ts, out, out_dtype, wave_i16_out, workspace, workspace_bytes, err_flag, dither, dither_seed,
+                           stream, (noise || rir) ? &nr : nullptr, &mp);
 }

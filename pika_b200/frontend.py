@@ -2,7 +2,7 @@
 
 Replaces the CPU chain of loader/otf_utt_loader.py:218-250 (AudioSegment augmentation -> PyKaldi
 Fbank -> splice) plus trainer/train_transducer_bmuf_otfaug.py:86-93 (CMN/CMVN, SpecAugment).
-Feature options are Kaldi's, read from a Kaldi-style config file such as egs/fbank.conf.
+Feature options are Kaldi's fbank or MFCC options, read from a Kaldi-style config file such as egs/fbank.conf.
 """
 import math
 
@@ -65,16 +65,20 @@ class FbankOptions:
         """keyword arguments of ``Frontend.lengths`` for these options"""
         return dict(frame_len=self.frame_len, frame_shift=self.frame_shift_samples, snip_edges=self.snip_edges)
 
+    # Kaldi option names of the options above, and the Kaldi options refused (ValueError) rather than ignored
+    NAMES = {"window-type": "window_type", "sample-frequency": "sample_frequency", "dither": "dither",
+             "low-freq": "low_freq", "high-freq": "high_freq", "num-mel-bins": "num_mel_bins",
+             "preemphasis-coefficient": "preemphasis_coefficient", "frame-length": "frame_length",
+             "frame-shift": "frame_shift", "snip-edges": "snip_edges", "remove-dc-offset": "remove_dc_offset",
+             "blackman-coeff": "blackman_coeff", "round-to-power-of-two": "round_to_power_of_two"}
+    REFUSED = UNSUPPORTED
+    KIND = "fbank"
+
     @classmethod
     def from_config(cls, path):
         """Kaldi option file: one ``--name=value`` per line, ``#`` comments (ParseOptions.read_config_file,
         loader/otf_utt_loader.py:195-200)."""
         kw = {}
-        names = {"window-type": "window_type", "sample-frequency": "sample_frequency", "dither": "dither",
-                 "low-freq": "low_freq", "high-freq": "high_freq", "num-mel-bins": "num_mel_bins",
-                 "preemphasis-coefficient": "preemphasis_coefficient", "frame-length": "frame_length",
-                 "frame-shift": "frame_shift", "snip-edges": "snip_edges", "remove-dc-offset": "remove_dc_offset",
-                 "blackman-coeff": "blackman_coeff", "round-to-power-of-two": "round_to_power_of_two"}
         with open(path) as f:
             for line in f:
                 line = line.split("#")[0].strip()
@@ -84,12 +88,31 @@ class FbankOptions:
                     raise ValueError("bad config line: %r" % line)
                 k, v = line[2:].split("=", 1)
                 k = k.strip()
-                if k in UNSUPPORTED:
-                    raise ValueError("fbank option --%s is not supported by the GPU front end" % k)
-                if k not in names:
-                    raise ValueError("unsupported fbank option --%s" % k)
-                kw[names[k]] = v.strip()
+                if k in cls.REFUSED:
+                    raise ValueError("%s option --%s is not supported by the GPU front end" % (cls.KIND, k))
+                if k not in cls.NAMES:
+                    raise ValueError("unsupported %s option --%s" % (cls.KIND, k))
+                kw[cls.NAMES[k]] = v.strip()
         return cls(**kw)
+
+
+class MfccOptions(FbankOptions):
+    """Kaldi MfccOptions (feat/feature-mfcc.h): FbankOptions' frame and mel options with their defaults (23 mel bins, dither 1), plus
+    num-ceps 13, use-energy true, energy-floor 0, raw-energy true, cepstral-lifter 22 and htk-compat false.  Kaldi's MFCC has no
+    --use-log-fbank or --use-power (it always takes the log of the power spectrum's mel energies); a config that sets one is refused."""
+
+    NAMES = dict(FbankOptions.NAMES, **{"num-ceps": "num_ceps", "use-energy": "use_energy", "energy-floor": "energy_floor",
+                                        "raw-energy": "raw_energy", "cepstral-lifter": "cepstral_lifter", "htk-compat": "htk_compat"})
+    REFUSED = ("use-log-fbank", "use-power", "vtln-warp", "vtln-low", "vtln-high", "allow-downsample", "allow-upsample")
+    KIND = "MFCC"
+
+    def __init__(self, num_ceps=13, use_energy=True, energy_floor=0.0, raw_energy=True, cepstral_lifter=22.0, htk_compat=False, **fbank):
+        super().__init__(**fbank)
+        self.num_ceps, self.use_energy, self.energy_floor = int(num_ceps), _bool(use_energy), float(energy_floor)
+        self.raw_energy, self.cepstral_lifter, self.htk_compat = _bool(raw_energy), float(cepstral_lifter), _bool(htk_compat)
+        if not 1 <= self.num_ceps <= self.num_mel_bins:
+            raise ValueError("--num-ceps=%d: num-ceps cannot be larger than num-mel-bins (%d) and must be at least 1"
+                             % (self.num_ceps, self.num_mel_bins))
 
 
 def noise_rir_kwargs(raw):
@@ -151,21 +174,49 @@ def fbank_tables(opts):
     return window_function(opts), tw, w.astype(np.float32), lo, hi_i
 
 
+def dct_matrix(num_ceps, n):
+    """Kaldi ComputeDctMatrix (matrix/matrix-functions.cc): the orthonormal DCT-II of size n, row 0 scaled by sqrt(1/n) and the others
+    by sqrt(2/n), first num_ceps rows: [num_ceps, n] float64"""
+    k = np.arange(num_ceps, dtype=np.float64)[:, None]
+    m = np.sqrt(2.0 / n) * np.cos(np.pi / n * (np.arange(n, dtype=np.float64)[None, :] + 0.5) * k)
+    m[0] = np.sqrt(1.0 / n)
+    return m
+
+
+def lifter_coeffs(num_ceps, q):
+    """Kaldi ComputeLifterCoeffs: 1 + 0.5 Q sin(pi i / Q), all ones when Q = 0 (no liftering): [num_ceps] float64"""
+    if q == 0.0:
+        return np.ones(num_ceps)
+    return 1.0 + 0.5 * q * np.sin(np.pi * np.arange(num_ceps, dtype=np.float64) / q)
+
+
+def mfcc_tables(opts):
+    """host table of the MFCC epilogue: [n_mel, num_ceps] float32, the DCT rows times the lifter, transposed.  Folding the lifter into
+    the DCT (in float64, one rounding to float32) changes only the rounding against Kaldi's separate multiply by the lifter."""
+    d = dct_matrix(opts.num_ceps, opts.num_mel_bins) * lifter_coeffs(opts.num_ceps, opts.cepstral_lifter)[:, None]
+    return np.ascontiguousarray(d.T).astype(np.float32)
+
+
 class Frontend:
     """Device-resident tables + workspace; ``__call__`` runs one padded batch.  ``stride`` keeps every stride-th spliced frame
-    (loader/otf_utt_loader.py:243-250): an utterance of n fbank frames yields ceil(n / stride) rows."""
+    (loader/otf_utt_loader.py:243-250): an utterance of n fbank frames yields ceil(n / stride) rows.  ``opts`` is an FbankOptions
+    (log mel energies, n_feat = num_mel_bins per frame) or an MfccOptions (cepstra, n_feat = num_ceps per frame); n_mel is the
+    number of mel bins either way."""
 
     def __init__(self, opts, lctx=1, rctx=1, device="cuda", stride=1):
         if int(stride) < 1:
             raise ValueError("stride must be >= 1, got %r" % stride)
         self.opts, self.lctx, self.rctx, self.device, self.stride = opts, lctx, rctx, device, int(stride)
         self.n_mel = opts.num_mel_bins
-        self.D = self.n_mel * (lctx + 1 + rctx)
+        self.is_mfcc = isinstance(opts, MfccOptions)
+        self.n_feat = opts.num_ceps if self.is_mfcc else self.n_mel
+        self.D = self.n_feat * (lctx + 1 + rctx)
         if self.D > 1024:
             raise ValueError("spliced dimension %d above 1024" % self.D)
         win, tw, w, lo, hi_i = fbank_tables(opts)
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
         self.window, self.twiddle, self.mel_w, self.mel_lo, self.mel_hi = t(win), t(tw), t(w), t(lo), t(hi_i)
+        self.dct = t(mfcc_tables(opts)) if self.is_mfcc else None
         self.err = torch.zeros(1, dtype=torch.int32, device=device)
         self._ws = None
         self.noise = self.rir = None           # AudioBank defaults for on-the-fly noise / reverberation (loader/audio_bank.py)
@@ -174,6 +225,10 @@ class Frontend:
     def _geometry_args(self):
         o = self.opts
         return (o.frame_len, o.frame_shift_samples, o.log2_nfft, int(o.snip_edges), int(o.remove_dc_offset), o.preemphasis_coefficient)
+
+    def _mfcc_args(self):
+        o = self.opts
+        return (K._P(self.dct), o.num_ceps, int(o.use_energy), int(o.raw_energy), o.energy_floor, int(o.htk_compat))
 
     def out_lens(self, n_frames):
         """rows per utterance after the stride: ceil(n_frames / stride), for an int, a list or a tensor"""
@@ -199,7 +254,7 @@ class Frontend:
                  offset=None, scale=None, specaug=(0, 0, 0, 0), want_wave=False, noise=None, noise_idx=None, noise_off=None,
                  snr=None, rir=None, rir_idx=None, rir_max_len=None):
         """pcm int16 [B, n_max] (device); n_samples/new_len/n_frames int32 [B], rate/target_db f32 [B] (device);
-        -> feats [B, t_max, D] (out_dtype) [, augmented int16 wave].  n_frames counts fbank frames (``lengths``), t_max output
+        -> feats [B, t_max, D] (out_dtype) [, augmented int16 wave], D = n_feat * (lctx + 1 + rctx).  n_frames counts fbank frames (``lengths``), t_max output
         rows: at least the longest ``out_lens(n_frames)``.
 
         On-the-fly noise (loader/audio.py:467-513 add_noise) runs when ``noise_idx`` is given: noise_idx int32 [B] segment of
@@ -210,11 +265,11 @@ class Frontend:
         aug = noise_idx is not None or rir_idx is not None
         if aug:
             rir_max_len = self._rir_max_len(rir, rir_idx, rir_max_len)
-            need = int(lib.pk_frontend_noise_rir_workspace_bytes(B, n_max, t_max * self.stride, self.n_mel, self.D, rir_max_len))
+            need = int(lib.pk_frontend_noise_rir_workspace_bytes(B, n_max, t_max * self.stride, self.n_feat, self.D, rir_max_len))
             if need < 0:
                 raise ValueError("rir_max_len %d outside [1, 65536]" % rir_max_len)
         else:
-            need = int(lib.pk_frontend_workspace_bytes(B, n_max, t_max * self.stride, self.n_mel, self.D))
+            need = int(lib.pk_frontend_workspace_bytes(B, n_max, t_max * self.stride, self.n_feat, self.D))
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         out = torch.empty(B, t_max, self.D, dtype=out_dtype, device=self.device)
@@ -227,7 +282,10 @@ class Frontend:
                 int(cmn), P(offset), P(scale), int(f0), int(fs), int(t0), int(ts), P(out), K._dt(out), P(wave),
                 P(self._ws), need, P(self.err), self.opts.dither, self._next_dither_seed(), K._stream())
         if not aug:
-            check(lib.pk_frontend_fwd(*args), "pk_frontend_fwd")
+            if self.is_mfcc:
+                check(lib.pk_frontend_fwd_mfcc(*args, *(None,) * 9, 1, *self._mfcc_args()), "pk_frontend_fwd_mfcc")
+            else:
+                check(lib.pk_frontend_fwd(*args), "pk_frontend_fwd")
             return (out, wave) if want_wave else out
         dev = lambda t, dt: torch.as_tensor(t).to(device=self.device, dtype=dt, non_blocking=True)  # noqa: E731
         nz = (None,) * 5
@@ -244,8 +302,11 @@ class Frontend:
             bank = rir if rir is not None else self.rir
             samples, offs, lens, _ = bank.device(self.device)
             rr = (samples, offs, lens, dev(rir_idx, torch.int32))
-        check(lib.pk_frontend_fwd_noise_rir(*args, *[P(t) for t in nz], *[P(t) for t in rr], int(rir_max_len)),
-              "pk_frontend_fwd_noise_rir")
+        banks = (*[P(t) for t in nz], *[P(t) for t in rr], int(rir_max_len))
+        if self.is_mfcc:
+            check(lib.pk_frontend_fwd_mfcc(*args, *banks, *self._mfcc_args()), "pk_frontend_fwd_mfcc")
+        else:
+            check(lib.pk_frontend_fwd_noise_rir(*args, *banks), "pk_frontend_fwd_noise_rir")
         return (out, wave) if want_wave else out
 
     def _rir_max_len(self, rir, rir_idx, rir_max_len):
@@ -274,4 +335,20 @@ class Frontend:
                            P(self.twiddle), P(self.mel_w), P(self.mel_lo), P(self.mel_hi), *self._geometry_args(), P(feats),
                            self.opts.dither if dither is None else dither,
                            (self._next_dither_seed() if seed is None else seed) & 0xFFFFFFFF, K._stream()), "pk_fbank")
+        return feats
+
+    def mfcc(self, wave_f32, n_frames, t_max, dither=None, seed=None, n_samples=None):
+        """the MFCC counterpart of ``fbank`` (MfccOptions only): wave f32 [B, n] of int16-scaled samples -> [B, t_max, num_ceps]
+        cepstra (rows >= n_frames[b] undefined)"""
+        if not self.is_mfcc:
+            raise ValueError("Frontend.mfcc needs MfccOptions")
+        if not self.opts.snip_edges and n_samples is None:
+            raise ValueError("Frontend.mfcc: snip_edges=false needs n_samples")
+        B = wave_f32.shape[0]
+        feats = torch.zeros(B, t_max, self.n_feat, dtype=torch.float32, device=self.device)
+        P = K._P
+        check(lib.pk_mfcc(P(wave_f32), wave_f32.stride(0), P(n_samples), P(n_frames), B, t_max, self.n_mel, P(self.window),
+                          P(self.twiddle), P(self.mel_w), P(self.mel_lo), P(self.mel_hi), *self._geometry_args(), P(feats),
+                          self.opts.dither if dither is None else dither,
+                          (self._next_dither_seed() if seed is None else seed) & 0xFFFFFFFF, K._stream(), *self._mfcc_args()), "pk_mfcc")
         return feats

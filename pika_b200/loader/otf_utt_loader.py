@@ -26,7 +26,7 @@ from threading import Thread
 import numpy as np
 import torch
 
-from ..frontend import FbankOptions, Frontend, noise_rir_kwargs
+from ..frontend import FbankOptions, Frontend, MfccOptions, noise_rir_kwargs
 from . import kaldi_io
 
 
@@ -46,6 +46,8 @@ def register(parser):
     parser.add_argument('--batch_first', action='store_true', help='1st dim is batch or frame')
     parser.add_argument('--reverse_labels', action='store_true', help='reverse labels for training, eg for LAS')
     parser.add_argument('--feat_config', type=str, default=None, help='feature extraction config file')
+    parser.add_argument('--feat_type', type=str, default='fbank', choices=('fbank', 'mfcc'),
+                        help='Kaldi feature type that --feat_config describes (pika_b200 extension)')
     parser.add_argument('--stride', type=int, default=1, help='strides for subsampling input')
     parser.add_argument('--batch_size', type=int, default=1024, help='batch size')
     parser.add_argument('--SOS', type=int, default=-1, help='start of seq id, valid when beyond 0')
@@ -98,9 +100,16 @@ def put_thread(q, generator, *gen_args):
 
 
 def feature_options(args):
-    """the fbank options of ``--feat_config`` (Kaldi's defaults with ``--feats_dim`` bins without one); ``--sample_rate`` must be the
-    config's sample frequency, as Kaldi's ComputeFeatures requires of the waveform's rate"""
-    opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
+    """the feature options of ``--feat_config``, read as ``--feat_type``'s Kaldi options (FbankOptions or MfccOptions; the reference
+    switches between the two by editing loader/otf_utt_loader.py:196-202).  Without a config: Kaldi's defaults with ``--feats_dim``
+    mel bins (fbank) or cepstra (MFCC).  An MFCC config must have ``--feats_dim`` cepstra.  ``--sample_rate`` must be the config's
+    sample frequency, as Kaldi's ComputeFeatures requires of the waveform's rate"""
+    if getattr(args, "feat_type", "fbank") == "mfcc":
+        opts = MfccOptions.from_config(args.feat_config) if args.feat_config else MfccOptions(num_ceps=args.feats_dim)
+        if opts.num_ceps != args.feats_dim:
+            raise ValueError("--feats_dim %d differs from the MFCC config's --num-ceps=%d" % (args.feats_dim, opts.num_ceps))
+    else:
+        opts = FbankOptions.from_config(args.feat_config) if args.feat_config else FbankOptions(num_mel_bins=args.feats_dim)
     if float(args.sample_rate) != opts.sample_frequency:
         raise ValueError("--sample_rate %s differs from the feature config's --sample-frequency=%g" % (args.sample_rate, opts.sample_frequency))
     return opts
@@ -182,7 +191,8 @@ _frontends = {}
 
 
 def _frontend_for(args, device):
-    key = (args.feat_config, args.feats_dim, args.sample_rate, args.lctx, args.rctx, args.stride, str(device))
+    key = (getattr(args, "feat_type", "fbank"), args.feat_config, args.feats_dim, args.sample_rate, args.lctx, args.rctx, args.stride,
+           str(device))
     if key not in _frontends:
         opts = feature_options(args)
         if getattr(args, "no_dither", False):          # explicit opt-out (parity runs); otherwise the feature config decides
