@@ -146,6 +146,65 @@ int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const int* label
                                  long long workspace_bytes, const float* row_lse, int n_parts, const void* h, int H,
                                  void* h_c, int* row_map, int* row_count, void* stream);
 
+/* The lattice pass alone, on log-prob tables the caller built (the simple and the pruned RNN-T losses below).
+ *   lpb_skew, lpl_skew [B][T+U1-1][U1] f32: node (b, t, u) at ((b*(T+U1-1) + t+u)*U1 + u); lpb = log P(blank | t, u), lpl =
+ *           log P(y_{u+1} | t, u) (read for u < U_b only).  -inf marks a node no path may use.  Every node t < T_b, u <= U_b is read.
+ *   costs [B] = -log P(y | x) (+inf when no path has a finite score); gb, gl [B][T][U1] f32 = d cost / d lpb, d cost / d lpl (<= 0,
+ *           times grad_scale[b] when grad_scale is not NULL; 0 at padded nodes).  -(gb + gl) is the node occupancy.
+ *   workspace >= the size pk_rnnt_lattice_workspace writes to *bytes (the f64 alpha / beta). */
+int pk_rnnt_lattice_workspace(int B, int T, int U1, long long* bytes);
+int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew, const float* lpl_skew,
+                    const float* grad_scale, float* costs, float* gb, float* gl, void* workspace, long long workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Pruned RNN-T loss (pika_b200/csrc/rnnt_pruned.cu, rnnt_loss.cu; DESIGN.md "Pruned RNN-T").
+ * Simple joiner z[t,u] = am[t] + lm[u]; its normaliser N[t,u] = log(E_t . P_u) + max(am_t) + max(lm_u) with E = exp(am - rowmax),
+ * P = exp(lm - rowmax), E.P^T a batched pk_gemm_bf16 product.  E.P below 2^-100 is clamped there (N stays finite; the clamped
+ * node's normaliser is then constant in the gradient).
+ *
+ * pk_rnnt_simple_prep: src f32 rows (b, i < n_in) of [nb*n_in, ld_src] (V valid columns) -> hi (, lo: NULL or the bf16 residual)
+ *   [nb*n_out, ld_out] bf16 = exp(src - rowmax), zero columns [V, ld_out) and zero rows i in [n_in, n_out); rmax [nb*n_in].
+ * pk_rnnt_simple_tables: S [B*T, ld_s] f32 = E.P^T -> lpb_skew / lpl_skew (layout of pk_rnnt_lattice).
+ * pk_rnnt_simple_w: gb, gl of that lattice -> W [B*T, ld_w] bf16 hi (, lo) = scale[b] * (-(gb + gl)) / S at the valid unclamped
+ *   nodes, 0 elsewhere (including the columns [U1, ld_w)).  scale may be NULL (1).
+ * pk_rnnt_simple_grad: axis 0 -> d am rows (b, t) [B*T, ldv]: exp(am - rmax) (.) G + scale * (sum_u gb at column 0, gl[t,u] at column
+ *   y_{u+1}); axis 1 -> d lm rows (b, u) [B*U1, ldv]: the same with the sums over t.  G = W.P (axis 0) or W^T.E (axis 1), f32, row
+ *   (b, i) at b*n_g + i, pitch ld_g.  One CTA per row; the blank / label terms are added by one thread in a fixed order.
+ *   out_dtype PK_F32 | PK_BF16; columns [V, ldv) are written 0.  ldv <= 51200.
+ * pk_rnnt_prune_bounds: occupancy gamma = -(ga + gb) (gb may be NULL) [B][T][U1] f32 -> bounds [B][T] int32 (DESIGN.md "Pruned RNN-T":
+ *   window argmax in f64 with the smallest start on ties, clamp, running max, reverse pass; padded frames copy the last frame).
+ *   An utterance with U_b > T_b (R-1) has no path inside the windows: its bounds are all -1 (the pruned loss is then +inf).
+ * pk_joint_gate_pruned_fwd: h [B*T*R, H] row (b, t, r) = tanh(ex1[b,t] + py1[b,u]) * sigmoid(exg[b,t] + pyg[b,u]),
+ *   u = min(max(bounds[b,t], 0) + r, U1 - 1).  ex [B*T, 2H], py [B*U1, 2H] as pk_joint_gate_fwd.
+ * pk_joint_gate_pruned_bwd: dh [B*T*R, H] -> dex [B*T, 2H] (sum over r in order), dpy [B*U1, 2H] (sum over the frames whose window
+ *   holds u, in frame order: one contiguous range because bounds are non-decreasing).  dh must be zero on the masked rows (u > U_b
+ *   or t >= T_b), as pk_rnnt_pruned_loss writes it; rows whose u was clamped are not read.
+ * pk_rnnt_pruned_loss: logits [B*T*R, ldv] (row (b, t, r) = node (t, bounds[b,t] + r)) -> costs [B], dlogits (may alias logits; NULL =
+ *   costs only; masked rows and the padding columns written 0), dlogits_colsum [ldv] (NULL or the fc2 bias gradient, fixed-order
+ *   sum).  Nodes outside the windows are -inf.  row_lse: NULL or the producing GEMM's [n_parts][B*T*R][2] partials.
+ *   workspace >= the size pk_rnnt_pruned_loss_workspace writes to *bytes. */
+int pk_rnnt_simple_prep(const float* src, int ld_src, int V, int nb, int n_in, int n_out, void* hi, void* lo, int ld_out, float* rmax,
+                        void* stream);
+int pk_rnnt_simple_tables(const float* am, const float* lm, int ldv, const float* am_max, const float* lm_max, const float* S, int ld_s,
+                          const int* labels, int ld_labels, const int* frame_lens, const int* label_lens, int B, int T, int U1,
+                          float* lpb_skew, float* lpl_skew, void* stream);
+int pk_rnnt_simple_w(const float* gb, const float* gl, const float* S, int ld_s, const int* frame_lens, const int* label_lens,
+                     const float* scale, int B, int T, int U1, void* w_hi, void* w_lo, int ld_w, void* stream);
+int pk_rnnt_simple_grad(const float* src, int ldv, int V, const float* rmax, const float* G, int ld_g, int n_g, int axis, const float* gb,
+                        const float* gl, const int* labels, int ld_labels, const int* frame_lens, const int* label_lens, const float* scale,
+                        int B, int T, int U1, void* out, int out_dtype, void* stream);
+int pk_rnnt_prune_bounds(const float* ga, const float* gb, const int* frame_lens, const int* label_lens, int B, int T, int U1, int R,
+                         int* bounds, void* stream);
+int pk_joint_gate_pruned_fwd(const void* ex, const void* py, const int* bounds, void* h, int dtype, int B, int T, int U1, int R, int H,
+                             void* stream);
+int pk_joint_gate_pruned_bwd(const void* ex, const void* py, const int* bounds, const void* dh, void* dex, void* dpy, int dtype, int B,
+                             int T, int U1, int R, int H, void* stream);
+int pk_rnnt_pruned_loss_workspace(int B, int T, int U1, int R, int ldv, long long* bytes);
+int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, const int* bounds,
+                        int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale, float* costs, void* dlogits,
+                        float* dlogits_colsum, void* workspace, long long workspace_bytes, const float* row_lse, int n_parts,
+                        void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Memory-bound layers around the GEMMs (pika_b200/csrc/elementwise.cu).  `dtype` is the
  * activation type (PK_BF16 production, PK_F32 fp32-class parity mode); statistics are f32.

@@ -55,6 +55,18 @@ PK_DEVICE float ex2_approx(float x) {            // 2^x on the MUFU, flush-to-ze
 PK_DEVICE float bf16lo(uint32_t v) { return __uint_as_float(v << 16); }
 PK_DEVICE float bf16hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
 
+// activation pair of the gated joint (dense and pruned): precise libm in the fp32-class mode, MUFU.TANH in production (bf16)
+template <typename T> PK_DEVICE float jt_tanh(float x);
+template <> PK_DEVICE float jt_tanh<float>(float x) { return tanhf(x); }
+template <> PK_DEVICE float jt_tanh<__nv_bfloat16>(float x) {
+    float y;
+    asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+template <typename T> PK_DEVICE float jt_sigmoid(float x);
+template <> PK_DEVICE float jt_sigmoid<float>(float x) { return 1.f / (1.f + expf(-x)); }
+template <> PK_DEVICE float jt_sigmoid<__nv_bfloat16>(float x) { return fmaf(jt_tanh<__nv_bfloat16>(0.5f * x), 0.5f, 0.5f); }
+
 // Counter-based dropout RNG: a 64-bit element index and a seed -> 32 uniform bits.
 // (murmur3-style finaliser; forward and backward regenerate the same mask.)
 PK_DEVICE uint32_t hash_u32(uint64_t idx, uint32_t seed) {

@@ -800,17 +800,7 @@ __global__ void __launch_bounds__(256) log_softmax_kernel(const T* __restrict__ 
 // h[b,t,u,c] = tanh(e1[b,t,c] + p1[b,u,c]) * sigmoid(eg[b,t,c] + pg[b,u,c])
 // ex = [B*T, 2H] (cols [0,H) = fc1 part, [H,2H) = gate part), py = [B*U1, 2H]; biases already folded into ex.
 PK_DEVICE float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
-// activation pair of the gated joint: precise libm in the fp32-class mode, MUFU.TANH in production (bf16)
-template <typename T> PK_DEVICE float jt_tanh(float x);
-template <> PK_DEVICE float jt_tanh<float>(float x) { return tanhf(x); }
-template <> PK_DEVICE float jt_tanh<__nv_bfloat16>(float x) {
-    float y;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-template <typename T> PK_DEVICE float jt_sigmoid(float x);
-template <> PK_DEVICE float jt_sigmoid<float>(float x) { return 1.f / (1.f + expf(-x)); }
-template <> PK_DEVICE float jt_sigmoid<__nv_bfloat16>(float x) { return fmaf(jt_tanh<__nv_bfloat16>(0.5f * x), 0.5f, 0.5f); }
+// the activation pair jt_tanh / jt_sigmoid lives in common.cuh (shared with the pruned joint, rnnt_pruned.cu)
 
 template <typename T>
 __global__ void __launch_bounds__(128) joint_gate_fwd_kernel(const T* __restrict__ ex, const T* __restrict__ py, T* __restrict__ h,

@@ -15,6 +15,7 @@
 //                           dlogits = -softmax * (gb + gl) + [v==blank] gb + [v==label] gl
 //                           (in place if dlogits aliases logits).
 // Algorithmic HBM traffic: 3 * B*T*(U+1)*V * sizeof(elem)  (+ O(nodes) fp32).
+#include <algorithm>
 #include <cstdlib>
 
 #include "../../include/pika_b200.h"
@@ -452,13 +453,15 @@ __global__ void __launch_bounds__(SCAN_THREADS) grad_rows_map_kernel(const float
 // and its joint activations h[r] are copied to h_c[row_map[r]].  The CTA blocks and the column sums are those of the dense form.
 constexpr int GRAD_THREADS = 256;
 template <typename T> struct GradCfg { static constexpr int MAXG = 32 / Vec16<T>::N; };   // 16-byte groups per thread: V <= 8192 for bf16 and f32
-template <typename T, int GRAD_RU, int MINB, bool COMPACT>
+// ROWY (the pruned loss): row r is not node (b, t, u = r % U1) but a gathered one; its label column is row_y[r] (-1: none).
+template <typename T, int GRAD_RU, int MINB, bool COMPACT, bool ROWY = false>
 __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* logits, const int* __restrict__ labels,
                                                                     const int* __restrict__ label_lens, RnntDims d,
                                                                     const float* __restrict__ lse_in, const float* __restrict__ gb_in,
                                                                     const float* __restrict__ gl_in, T* dlogits, float* __restrict__ colsum,
                                                                     long long rows_per_cta, const int* __restrict__ row_map,
-                                                                    const T* __restrict__ h, T* __restrict__ h_c, int H) {
+                                                                    const T* __restrict__ h, T* __restrict__ h_c, int H,
+                                                                    const int* __restrict__ row_y = nullptr) {
     constexpr int VN = Vec16<T>::N;
     constexpr int GRAD_MAXG = GradCfg<T>::MAXG;
     extern __shared__ float gsm[];                          // per-row scalars of this CTA's block: gb, gl, lse*log2e, label (, map)
@@ -477,9 +480,13 @@ __global__ void __launch_bounds__(GRAD_THREADS, MINB) rnnt_grad_kernel(const T* 
         s_gb[i] = gb_in[row];
         s_gl[i] = gl_in[row];
         s_l2[i] = lse_in[row] * kLog2e;
-        const int u = (int)(row % d.U1);
-        const int b = (int)(row / ((long long)d.T * d.U1));
-        s_y[i] = (u < label_lens[b]) ? labels[(size_t)b * d.ld_labels + u] : -1;
+        if (ROWY) {
+            s_y[i] = row_y[row];
+        } else {
+            const int u = (int)(row % d.U1);
+            const int b = (int)(row / ((long long)d.T * d.U1));
+            s_y[i] = (u < label_lens[b]) ? labels[(size_t)b * d.ld_labels + u] : -1;
+        }
         if (COMPACT) s_map[i] = row_map[row];
     }
     __syncthreads();
@@ -602,6 +609,108 @@ __global__ void __launch_bounds__(256) colsum_partials_kernel(const float* __res
     }
 }
 
+// ------------------------------------------------------------------------------------ pruned loss (pk_rnnt_pruned_loss)
+// Row (b, t, r) of the [B*T*R, ldv] logits is node (t, u = s_t + r); it is masked (no log-prob, zero gradient) when t >= T_b or
+// u > U_b.  Pass 1: the row log-sum-exp, one warp per row (streamed) or merged from the producing GEMM's partials.
+template <typename T>
+__global__ void __launch_bounds__(256) pruned_row_lse_kernel(const T* __restrict__ logits, const int* __restrict__ frame_lens,
+                                                             const int* __restrict__ label_lens, const int* __restrict__ bounds, int Tt,
+                                                             int R, int V, int ldv, long long rows, const float2* __restrict__ parts,
+                                                             int n_parts, float* __restrict__ lse_out) {
+    constexpr int VN = Vec16<T>::N;
+    const int lane = threadIdx.x & 31;
+    const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows; row += n_warps) {
+        const long long bt = row / R;
+        const int r = (int)(row - bt * R), t = (int)(bt % Tt), b = (int)(bt / Tt);
+        if (t >= frame_lens[b] || bounds[bt] < 0 || bounds[bt] + r > label_lens[b]) continue;     // masked row (warp-uniform)
+        float lse;
+        if (parts != nullptr) {
+            float m = -INFINITY, sum = 0.f;
+            for (int i = 0; i < n_parts; ++i) m = fmaxf(m, parts[(size_t)i * rows + row].x);
+            for (int i = 0; i < n_parts; ++i) { const float2 ps = parts[(size_t)i * rows + row]; sum += ps.y * exp2f(ps.x - m); }
+            lse = (m + log2f(sum)) * kLn2;
+        } else {
+            const T* rp = logits + row * (long long)ldv;
+            float m = -INFINITY, sum = 0.f;
+            const int nfull = V / VN;
+            for (int i = lane; i < nfull; i += 32) {
+                float f[VN];
+                Vec16<T>::unpack(ld_plain(reinterpret_cast<const uint4*>(rp) + i), f);
+#pragma unroll
+                for (int e = 0; e < VN; ++e) {
+                    const float x = f[e] * kLog2e;
+                    if (x > m) { sum *= exp2f(m - x); m = x; }
+                    sum += exp2f(x - m);
+                }
+            }
+            for (int v = nfull * VN + lane; v < V; v += 32) {
+                const float x = to_f32<T>(rp[v]) * kLog2e;
+                if (x > m) { sum *= exp2f(m - x); m = x; }
+                sum += exp2f(x - m);
+            }
+            const float mw = warp_max(m);
+            sum = (m == -INFINITY) ? 0.f : sum * exp2f(m - mw);
+            sum = warp_sum(sum);
+            lse = (mw + log2f(sum)) * kLn2;
+        }
+        if (lane == 0) lse_out[row] = lse;
+    }
+}
+
+// Pass 2: the lattice tables.  One thread per valid node (b, t, u): inside the frame's window it reads its row's blank / label logit,
+// outside it is -inf (no path through it).
+template <typename T>
+__global__ void __launch_bounds__(256) pruned_tables_kernel(const T* __restrict__ logits, const int* __restrict__ labels,
+                                                            const int* __restrict__ frame_lens, const int* __restrict__ label_lens,
+                                                            const int* __restrict__ bounds, RnntDims d, int R,
+                                                            const float* __restrict__ lse, float* __restrict__ lpb_skew,
+                                                            float* __restrict__ lpl_skew) {
+    const long long n = (long long)d.B * d.T * d.U1;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int u = (int)(i % d.U1);
+        const long long bt = i / d.U1;
+        const int t = (int)(bt % d.T), b = (int)(bt / d.T);
+        const int Un = label_lens[b];
+        if (t >= frame_lens[b] || u > Un) continue;
+        const int r = u - bounds[bt];
+        const size_t sk = skew_index(d, b, t, u);
+        float pb = -INFINITY, pl = -INFINITY;
+        if (bounds[bt] >= 0 && r >= 0 && r < R) {
+            const long long row = bt * R + r;
+            const T* rp = logits + row * (long long)d.ldv;
+            pb = to_f32<T>(rp[0]) - lse[row];
+            if (u < Un) pl = to_f32<T>(rp[labels[(size_t)b * d.ld_labels + u]]) - lse[row];
+        }
+        lpb_skew[sk] = pb;
+        if (u < Un) lpl_skew[sk] = pl;
+    }
+}
+
+// Pass 4 (after the lattice): per-row gradient coefficients for rnnt_grad_kernel<ROWY>: the occupancies of the row's node and its
+// label column; masked rows get zeros (the gradient kernel writes a zero row without reading the logits).
+__global__ void __launch_bounds__(256) pruned_rows_kernel(const int* __restrict__ labels, const int* __restrict__ frame_lens,
+                                                          const int* __restrict__ label_lens, const int* __restrict__ bounds, RnntDims d,
+                                                          int R, const float* __restrict__ gb, const float* __restrict__ gl,
+                                                          float* __restrict__ gb_row, float* __restrict__ gl_row, int* __restrict__ y_row) {
+    const long long rows = (long long)d.B * d.T * R;
+    for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < rows; row += (long long)gridDim.x * blockDim.x) {
+        const long long bt = row / R;
+        const int r = (int)(row - bt * R), t = (int)(bt % d.T), b = (int)(bt / d.T);
+        const int Un = label_lens[b], u = bounds[bt] + r;
+        float vb = 0.f, vl = 0.f;
+        int y = -1;
+        if (t < frame_lens[b] && bounds[bt] >= 0 && u <= Un) {
+            const long long node = bt * d.U1 + u;
+            vb = gb[node];
+            if (u < Un) { vl = gl[node]; y = labels[(size_t)b * d.ld_labels + u]; }
+        }
+        gb_row[row] = vb;
+        gl_row[row] = vl;
+        y_row[row] = y;
+    }
+}
+
 }  // namespace pk
 
 extern "C" long long pk_rnnt_loss_workspace_bytes(int B, int T, int U1) {
@@ -624,6 +733,27 @@ extern "C" long long pk_rnnt_loss_colsum_workspace_bytes(int B, int T, int U1, i
     int ggrid; long long rpc;
     rnnt_grad_grid((long long)B * T * U1, &rpc, &ggrid);
     return (long long)ggrid * ldv * 4;
+}
+
+static int launch_lattice(const int* frame_lens, const int* label_lens, const pk::RnntDims& d, const float* lpb, const float* lpl,
+                          double* alpha, double* beta, const float* grad_scale, float* costs, float* gb, float* gl, cudaStream_t stream) {
+    using namespace pk;
+    const int U1 = d.U1;
+    const int lat_smem = 2 * 2 * (U1 + 2) * 8;
+    int G = ((U1 + 31) / 32) * 32;
+    if (G > LAT_MAX_G) G = LAT_MAX_G;
+    const int cpt = (U1 + G - 1) / G;
+    PK_CHECK_ARG(cpt <= LAT_MAX_CPT, "U too large for the lattice kernel (U+1 <= 2048)");
+    static bool configured = false;                  // the two ping-pong diagonals exceed the default 48 KB from U+1 = 1534 on
+    if (!configured) {
+        PK_CHECK_CUDA(cudaFuncSetAttribute(rnnt_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           2 * 2 * (LAT_MAX_G * LAT_MAX_CPT + 2) * (int)sizeof(lat_t)));
+        configured = true;
+    }
+    rnnt_lattice_kernel<<<d.B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
+                                                       costs, gb, gl);
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
 }
 
 static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, const int* frame_lens,
@@ -669,20 +799,10 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
         rnnt_rowstats_kernel<float><<<grid, 256, 0, stream>>>(reinterpret_cast<const float*>(logits), labels, frame_lens,
                                                               label_lens, d, lse, lpb, lpl);
     PK_CHECK_LAUNCH(); count_launch();
-    const int lat_smem = 2 * 2 * (U1 + 2) * 8;
-    int G = ((U1 + 31) / 32) * 32;
-    if (G > LAT_MAX_G) G = LAT_MAX_G;
-    const int cpt = (U1 + G - 1) / G;
-    PK_CHECK_ARG(cpt <= LAT_MAX_CPT, "U too large for the lattice kernel (U+1 <= 2048)");
-    static bool configured = false;                  // the two ping-pong diagonals exceed the default 48 KB from U+1 = 1534 on
-    if (!configured) {
-        PK_CHECK_CUDA(cudaFuncSetAttribute(rnnt_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           2 * 2 * (LAT_MAX_G * LAT_MAX_CPT + 2) * (int)sizeof(lat_t)));
-        configured = true;
+    {
+        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
+        if (rc) return rc;
     }
-    rnnt_lattice_kernel<<<B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
-                                                     costs, gb, gl);
-    PK_CHECK_LAUNCH(); count_launch();
     if (dlogits != nullptr) {
         PK_CHECK_ARG(ldv <= 8192, "V too large for the gradient kernel (V <= 8192)");
         int ggrid; long long rpc;
@@ -755,4 +875,111 @@ extern "C" int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const
     PK_CHECK_ARG((reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(h_c) & 15) == 0, "h / h_c not 16B aligned");
     return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dz_c,
                           dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, row_map, row_count, h, H, h_c, stream);
+}
+
+static long long lattice_ws_bytes(int B, int T, int U1) { return 2 * (long long)B * ((long long)T + U1 - 1) * U1 * 8; }
+extern "C" int pk_rnnt_lattice_workspace(int B, int T, int U1, long long* bytes) {
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && bytes != nullptr, "bad dims or null pointer");
+    *bytes = lattice_ws_bytes(B, T, U1);
+    return 0;
+}
+
+extern "C" int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
+                               const float* lpl_skew, const float* grad_scale, float* costs, float* gb, float* gl, void* workspace,
+                               long long workspace_bytes, void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0, "bad dims");
+    PK_CHECK_ARG(lpb_skew && lpl_skew && costs && gb && gl && workspace, "null pointer");
+    PK_CHECK_ARG(workspace_bytes >= lattice_ws_bytes(B, T, U1), "workspace too small");
+    RnntDims d{B, T, U1, 2, 2, 1, T + U1 - 1};
+    const size_t skew = (size_t)B * d.ND * U1;
+    double* alpha = reinterpret_cast<double*>(workspace);
+    return launch_lattice(frame_lens, label_lens, d, lpb_skew, lpl_skew, alpha, alpha + skew, grad_scale, costs, gb, gl,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+// workspace of pk_rnnt_pruned_loss: alpha, beta (f64 skew), lpb, lpl (f32 skew), gb, gl (f32 nodes), lse, gb_row, gl_row, y_row
+// (per pruned row), then the gradient pass's per-CTA column-sum partials
+static long long pruned_ws_parts(int B, int T, int U1, int R, int ldv, long long* colsum_off) {
+    const long long skew = (long long)B * ((long long)T + U1 - 1) * U1, nodes = (long long)B * T * U1, rows = (long long)B * T * R;
+    const long long base = 2 * skew * 8 + 2 * skew * 4 + 2 * nodes * 4 + 4 * rows * 4;
+    const long long off = (base + 255) / 256 * 256;
+    int ggrid; long long rpc;
+    rnnt_grad_grid(rows, &rpc, &ggrid);
+    if (colsum_off) *colsum_off = off;
+    return off + (long long)ggrid * ldv * 4;
+}
+extern "C" int pk_rnnt_pruned_loss_workspace(int B, int T, int U1, int R, int ldv, long long* bytes) {
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && R >= 1 && ldv > 0 && bytes != nullptr, "bad dims or null pointer");
+    *bytes = pruned_ws_parts(B, T, U1, R, ldv, nullptr);
+    return 0;
+}
+
+extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                                   const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
+                                   float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
+                                   const float* row_lse, int n_parts, void* stream_v) {
+    using namespace pk;
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    PK_CHECK_ARG(dtype == PK_F32 || dtype == PK_BF16, "bad dtype");
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && R >= 1 && V > 1, "bad dims");
+    const int vn = dtype == PK_F32 ? 4 : 8;
+    PK_CHECK_ARG(ldv >= V && ldv % vn == 0, "ldv must be >= V and a multiple of 16 bytes");
+    PK_CHECK_ARG((reinterpret_cast<uintptr_t>(logits) & 15) == 0, "logits not 16B aligned");
+    PK_CHECK_ARG(dlogits == nullptr || (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0, "dlogits not 16B aligned");
+    PK_CHECK_ARG(row_lse == nullptr || n_parts >= 1, "n_parts must be >= 1");
+    long long cs_off;
+    PK_CHECK_ARG(workspace_bytes >= pruned_ws_parts(B, T, U1, R, ldv, &cs_off), "workspace too small");
+    RnntDims d{B, T, U1, V, ldv, ld_labels, T + U1 - 1};
+    const size_t skew = (size_t)B * d.ND * U1, nodes = (size_t)B * T * U1;
+    const long long rows = (long long)B * T * R;
+    double* alpha = reinterpret_cast<double*>(workspace); double* beta = alpha + skew;
+    float* lpb = reinterpret_cast<float*>(beta + skew); float* lpl = lpb + skew;
+    float* gb = lpl + skew; float* gl = gb + nodes;
+    float* lse = gl + nodes; float* gb_row = lse + rows; float* gl_row = gb_row + rows;
+    int* y_row = reinterpret_cast<int*>(gl_row + rows);
+    const int wgrid = (int)std::min<long long>((rows + 7) / 8, (long long)num_sms() * 32);
+    const long long nn = (long long)B * T * U1;
+    const int ngrid = (int)std::min<long long>((nn + 255) / 256, (long long)num_sms() * 8);
+    if (dtype == PK_BF16) {
+        using TT = __nv_bfloat16;
+        pruned_row_lse_kernel<TT><<<wgrid, 256, 0, stream>>>((const TT*)logits, frame_lens, label_lens, bounds, T, R, V, ldv, rows,
+                                                            (const float2*)row_lse, n_parts, lse);
+        PK_CHECK_LAUNCH(); count_launch();
+        pruned_tables_kernel<TT><<<ngrid, 256, 0, stream>>>((const TT*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb, lpl);
+    } else {
+        pruned_row_lse_kernel<float><<<wgrid, 256, 0, stream>>>((const float*)logits, frame_lens, label_lens, bounds, T, R, V, ldv, rows,
+                                                               (const float2*)row_lse, n_parts, lse);
+        PK_CHECK_LAUNCH(); count_launch();
+        pruned_tables_kernel<float><<<ngrid, 256, 0, stream>>>((const float*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb, lpl);
+    }
+    PK_CHECK_LAUNCH(); count_launch();
+    {
+        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
+        if (rc) return rc;
+    }
+    if (dlogits == nullptr) return 0;
+    PK_CHECK_ARG(ldv <= 8192, "V too large for the gradient kernel (V <= 8192)");
+    const int rgrid = (int)std::min<long long>((rows + 255) / 256, (long long)num_sms() * 8);
+    pruned_rows_kernel<<<rgrid, 256, 0, stream>>>(labels, frame_lens, label_lens, bounds, d, R, gb, gl, gb_row, gl_row, y_row);
+    PK_CHECK_LAUNCH(); count_launch();
+    int ggrid; long long rpc;
+    rnnt_grad_grid(rows, &rpc, &ggrid);
+    float* cs_part = dlogits_colsum ? reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(workspace) + cs_off) : nullptr;
+    RnntDims dr{B, T, R, V, ldv, ld_labels, 0};          // the gradient kernel's rows are the B*T*R pruned rows
+    const size_t gsmem = (size_t)rpc * 16;
+    if (dtype == PK_BF16)
+        rnnt_grad_kernel<__nv_bfloat16, 2, 3, false, true><<<ggrid, GRAD_THREADS, gsmem, stream>>>(
+            (const __nv_bfloat16*)logits, labels, label_lens, dr, lse, gb_row, gl_row, (__nv_bfloat16*)dlogits, cs_part, rpc, nullptr,
+            nullptr, nullptr, 0, y_row);
+    else
+        rnnt_grad_kernel<float, 2, 2, false, true><<<ggrid, GRAD_THREADS, gsmem, stream>>>(
+            (const float*)logits, labels, label_lens, dr, lse, gb_row, gl_row, (float*)dlogits, cs_part, rpc, nullptr, nullptr, nullptr, 0,
+            y_row);
+    PK_CHECK_LAUNCH(); count_launch();
+    if (dlogits_colsum) {
+        colsum_partials_kernel<<<(ldv + 31) / 32, 256, 0, stream>>>(cs_part, ggrid, ldv, dlogits_colsum);
+        PK_CHECK_LAUNCH(); count_launch();
+    }
+    return 0;
 }

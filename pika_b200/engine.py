@@ -829,22 +829,29 @@ def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None,
     dpy = _new((B * U1, 2 * H), like=dlogits)
     K.joint_gate_bwd(st["ex"], st["py"], dh, dex, dpy, B, T, U1, H, dh_map=row_map)
     del dh
+    return _gate_input_grads(dex, dpy, st, model, need_enc, need_pred)
+
+
+def _gate_input_grads(dex, dpy, st, model, need_enc, need_pred):
+    """gate-input gradients dex [B*T, 2H], dpy [B*U1, 2H] -> (d_enc, d_pred); the fc1 / fc_gate gradients written in place"""
+    B, T, U1, H = st["dims"][:4]
+    fc1, fcg = model.fc1, model.fc_gate
     dex_parts, dpy_parts = stage_act(dex), stage_act(dpy)
     g1, gg = grad_of(fc1.weight), grad_of(fcg.weight)
     for (dparts, xparts, lo) in ((dex_parts, st["enc_parts"], 0), (dpy_parts, st["pred_parts"], H)):
         gemm_parts([[p[:, :H] for p in dparts]], [xparts], g1[:, lo:lo + H], a_mn=True, b_mn=True)
         gemm_parts([[p[:, H:] for p in dparts]], [xparts], gg[:, lo:lo + H], a_mn=True, b_mn=True)
-    dbx = torch.empty(2 * H, dtype=torch.float32, device=dlogits.device)
+    dbx = torch.empty(2 * H, dtype=torch.float32, device=dex.device)
     K.colsum(dex, dbx)
     grad_of(fc1.bias).copy_(dbx[:H])
     grad_of(fcg.bias).copy_(dbx[H:])
     d_enc = d_pred = None
     if need_enc:
-        d_enc = _new((B * T, H), like=dlogits)
+        d_enc = _new((B * T, H), like=dex)
         gemm_parts([dex_parts], [[p[:, :H] for p in st["wx"]]], d_enc, b_mn=True)
         d_enc = d_enc.view(B, T, H)
     if need_pred:
-        d_pred = _new((B * U1, H), like=dlogits)
+        d_pred = _new((B * U1, H), like=dex)
         gemm_parts([dpy_parts], [[p[:, H:] for p in st["wx"]]], d_pred, b_mn=True)
         d_pred = d_pred.view(B, U1, H)
     return d_enc, d_pred
@@ -871,7 +878,8 @@ _UNIT_LOSS_GRAD = False
 def assume_unit_loss_grad(flag):
     """The training step calls ``costs.sum().backward()`` (trainer/train_transducer_bmuf_otfaug.py:97-103), i.e. the upstream
     gradient of every cost is exactly 1.  TrainStep declares that here so JointLossFn.backward does no re-scaling work;
-    any other caller gets the general (scaled) backward."""
+    any other caller gets the general (scaled) backward.  For the pruned loss (transducer_loss_pruned) the declaration is that the
+    upstream gradients are exactly the simple / pruned scales it was called with."""
     global _UNIT_LOSS_GRAD
     _UNIT_LOSS_GRAD = bool(flag)
 
@@ -1154,3 +1162,226 @@ def transducer_loss(model, x, y, frame_lens, label_lens, x_len=None, t_out=None)
     pred = prednet_forward_act(model, y)
     return JointLossFn.apply(enc, pred, model, y.int().contiguous(), frame_lens.int().contiguous(), label_lens.int().contiguous(),
                              torch.is_grad_enabled())
+
+
+# ------------------------------------------------------------------------------------------------
+# pruned RNN-T loss (DESIGN.md "Pruned RNN-T"): a simple joiner am[t] + lm[u] gives a full lattice cheaply, its occupancies choose a
+# window of R label positions per frame, and the gated joint + fc2 run on those B*T*R rows only.
+def _scaled_grads_backward(ctx, dcosts, params, who):
+    """Shared backward of the two pruned-loss Functions: their gradients were formed in forward for an upstream gradient equal to
+    ``ctx.scale`` per utterance.  TrainStep declares exactly that (assume_unit_loss_grad); any other caller's uniform upstream
+    gradient is re-scaled here, and per-utterance weights raise, as in JointLossFn."""
+    if not ctx.need_grad:
+        raise RuntimeError("%s: forward ran with grad mode off; there is nothing to back-propagate" % who)
+    d_enc, d_pred = ctx.saved_tensors
+    if not _UNIT_LOSS_GRAD:
+        w = dcosts.detach().float()
+        if not bool((w == w[0]).all()):
+            raise RuntimeError("%s: per-utterance loss weights are not supported (its parameter gradients were formed for a uniform "
+                               "upstream gradient)" % who)
+        f = float(w[0])
+        if f != ctx.scale:
+            if ctx.scale == 0.0:
+                raise RuntimeError("%s: forward ran with scale 0, so no gradient was formed; pass the scale the loss is weighted by" % who)
+            r = f / ctx.scale
+            for p in params:
+                p.grad.mul_(r)
+            d_enc = d_enc * r
+            d_pred = d_pred * r
+    return d_enc, d_pred
+
+
+def _proj_backward(d, x_parts, lin, V):
+    """d [rows, ldv] (act dtype, padding columns 0) = d(loss)/d(x W^T + b) of a projection to V -> dx [rows, H]; dW, db written"""
+    d_parts = stage_act(d)
+    d_v = [p[:, :V] for p in d_parts]
+    w_parts = stage_weight(lin.weight)
+    dx = _new((d.shape[0], lin.weight.shape[1]), like=d)
+    gemm_parts([d_v], [w_parts], dx, b_mn=True)
+    gemm_parts([d_v], [x_parts], grad_of(lin.weight), a_mn=True, b_mn=True)
+    db = torch.empty(d.shape[1], dtype=torch.float32, device=d.device)
+    K.colsum(d, db)
+    grad_of(lin.bias).copy_(db[:V])
+    return dx
+
+
+def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.0, need_grad=True):
+    """The simple joiner's RNN-T loss from its two projections am [B*T, ldv], lm [B*U1, ldv] (f32, V valid columns) -> (costs [B],
+    bounds [B,T] int32 for windows of R, dam, dlm) with dam [B*T, ldv], dlm [B*U1, ldv] (activation dtype, padding columns 0) the
+    gradients of sum_b scale * cost_b, or None when ``need_grad`` is False.  R = 0: no bounds (None)."""
+    ldv = am.shape[1]
+    U1p = (U1 + 7) // 8 * 8
+    dev = am.device
+    split = _PRECISION == "fp32"
+
+    def parts(rows, cols):
+        return [torch.empty(rows, cols, dtype=torch.bfloat16, device=dev) for _ in range(2 if split else 1)]
+    E, P = parts(B * T, ldv), parts(B * U1p, ldv)
+    am_max = K.rnnt_simple_prep(am, V, B, T, T, E[0], E[1] if split else None)
+    lm_max = K.rnnt_simple_prep(lm, V, B, U1, U1p, P[0], P[1] if split else None)
+    E3 = [e.view(B, T, ldv) for e in E]
+    P3 = [p.view(B, U1p, ldv) for p in P]
+    S = torch.empty(B, T, U1p, dtype=torch.float32, device=dev)
+    with _Tap("simple_loss"):
+        gemm_parts([E3], [P3], S)                                   # S[t,u] = E[t] . P[u]
+        lpb, lpl = K.rnnt_simple_tables(am, lm, am_max, lm_max, S.view(B * T, U1p), labels, frame_lens, label_lens, B, T, U1)
+        costs, gb, gl = K.rnnt_lattice(lpb, lpl, frame_lens, label_lens, B, T, U1)
+    del lpb, lpl
+    bounds = None
+    if R:
+        with _Tap("prune_bounds"):
+            bounds = K.rnnt_prune_bounds(gb, gl, frame_lens, label_lens, R)
+    if not need_grad:
+        return costs, bounds, None, None
+    scale_t = torch.full((B,), float(scale), dtype=torch.float32, device=dev)
+    W = parts(B * T, U1p)
+    K.rnnt_simple_w(gb, gl, S.view(B * T, U1p), frame_lens, label_lens, scale_t, W[0], W[1] if split else None)
+    W3 = [w.view(B, T, U1p) for w in W]
+    WP = torch.empty(B, T, ldv, dtype=torch.float32, device=dev)
+    WtE = torch.empty(B, U1p, ldv, dtype=torch.float32, device=dev)
+    gemm_parts([W3], [P3], WP, b_mn=True)                           # (W P)[t]   = sum_u W[t,u] P[u]
+    gemm_parts([W3], [E3], WtE, a_mn=True, b_mn=True)               # (W^T E)[u] = sum_t W[t,u] E[t]
+    del W, W3, E, E3, P, P3, S
+    dam = _new((B * T, ldv), like=am)
+    dlm = _new((B * U1, ldv), like=am)
+    K.rnnt_simple_grad(am, V, am_max, WP.view(B * T, ldv), T, 0, gb, gl, labels, frame_lens, label_lens, scale_t, dam)
+    K.rnnt_simple_grad(lm, V, lm_max, WtE.view(B * U1p, ldv), U1p, 1, gb, gl, labels, frame_lens, label_lens, scale_t, dlm)
+    return costs, bounds, dam, dlm
+
+
+class SimpleLossFn(torch.autograd.Function):
+    """Simple-joiner RNN-T loss and the pruning bounds: enc [B,T,H], pred [B,U1,H] -> (costs [B], bounds [B,T] int32).
+    am = simple_am_proj(enc), lm = simple_lm_proj(pred) in f32; z[t,u] = am[t] + lm[u] is never formed: the normaliser is
+    log(E.P^T) + the row maxes (pk_rnnt_simple_*), the lattice runs on the resulting tables (pk_rnnt_lattice) and its occupancies give the
+    bounds (pk_rnnt_prune_bounds).  The gradients (for an upstream gradient of ``scale`` per utterance) are formed here in forward:
+    dam = E (.) (W P) and dlm = P (.) (W^T E) plus the blank / label terms, W = scale * occupancy / (E.P^T)."""
+
+    @staticmethod
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, R, scale, need_grad):
+        B, T, H = enc.shape
+        U1 = pred.shape[1]
+        am_p, lm_p = model.simple_am_proj, model.simple_lm_proj
+        V = am_p.weight.shape[0]
+        ldv = _ldv(V)
+        enc_parts = stage_act(enc.reshape(B * T, H))
+        pred_parts = stage_act(pred.reshape(B * U1, H))
+        am = torch.zeros(B * T, ldv, dtype=torch.float32, device=enc.device)
+        lm = torch.zeros(B * U1, ldv, dtype=torch.float32, device=enc.device)
+        gemm_parts([enc_parts], [stage_weight(am_p.weight)], am[:, :V], bias=am_p.bias.detach())
+        gemm_parts([pred_parts], [stage_weight(lm_p.weight)], lm[:, :V], bias=lm_p.bias.detach())
+        costs, bounds, dam, dlm = simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale, need_grad)
+        del am, lm
+        ctx.mark_non_differentiable(bounds)
+        ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
+        if need_grad:
+            d_enc = _proj_backward(dam, enc_parts, am_p, V).view(B, T, H)
+            d_pred = _proj_backward(dlm, pred_parts, lm_p, V).view(B, U1, H)
+            ctx.save_for_backward(d_enc, d_pred)
+        return costs, bounds
+
+    @staticmethod
+    def backward(ctx, dcosts, _dbounds):
+        m = ctx.model
+        d_enc, d_pred = _scaled_grads_backward(ctx, dcosts, (m.simple_am_proj.weight, m.simple_am_proj.bias, m.simple_lm_proj.weight,
+                                                             m.simple_lm_proj.bias), "SimpleLossFn")
+        return d_enc, d_pred, None, None, None, None, None, None, None
+
+
+class PrunedJointLossFn(torch.autograd.Function):
+    """Pruned joint + RNN-T loss: row (b, t, r) of the joint is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd),
+    fc2 runs on the B*T*R rows (with the row log-sum-exp epilogue in bf16), the loss and its gradient come from pk_rnnt_pruned_loss
+    (in place over the logits), and the joint backward runs at once, as in JointLossFn.  Gradients are formed for an upstream
+    gradient of ``scale`` per utterance."""
+
+    @staticmethod
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, bounds, R, scale, need_grad):
+        B, T, H = enc.shape
+        U1 = pred.shape[1]
+        fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
+        V = fc2.weight.shape[0]
+        ldv = _ldv(V)
+        dev = enc.device
+        wx = stage_weight([fc1.weight, fcg.weight])
+        enc_parts = stage_act(enc.reshape(B * T, H))
+        pred_parts = stage_act(pred.reshape(B * U1, H))
+        ex = _new((B * T, 2 * H), like=enc)
+        py = _new((B * U1, 2 * H), like=enc)
+        gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=_cat_bias([fc1.bias, fcg.bias]))
+        gemm_parts([pred_parts], [[p[:, H:] for p in wx]], py)
+        rows = B * T * R
+        h = _new((rows, H), like=enc)
+        K.joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H)
+        w2 = stage_weight(fc2.weight)
+        logits = _new((rows, ldv), like=enc, zero=(ldv != V))
+        h_parts = stage_act(h)
+        del h
+        row_lse = None
+        if _FUSED_LSE and logits.dtype == torch.bfloat16 and V % 8 == 0:
+            row_lse = torch.empty(K.row_lse_parts(rows, V, 256), rows, 2, dtype=torch.float32, device=dev)
+        with _Tap("fc2_fwd"):
+            gemm_parts([h_parts], [w2], logits[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
+                       **({"block_n": 256} if row_lse is not None else {}))
+        ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
+        if not need_grad:
+            return K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=row_lse)
+        scale_t = torch.full((B,), float(scale), dtype=torch.float32, device=dev)
+        db2 = torch.empty(ldv, dtype=torch.float32, device=dev)
+        with _Tap("rnnt_loss"):
+            costs = K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=scale_t, dlogits=logits,
+                                       colsum=db2, row_lse=row_lse)
+        del row_lse
+        dl_v = [p[:, :V] for p in stage_act(logits)]
+        dh = _new((rows, H), like=enc)
+        gemm_parts([dl_v], [w2], dh, b_mn=True)
+        gemm_parts([dl_v], [h_parts], grad_of(fc2.weight), a_mn=True, b_mn=True)
+        grad_of(fc2.bias).copy_(db2[:V])
+        del dl_v, logits, h_parts
+        dex = _new((B * T, 2 * H), like=enc)
+        dpy = _new((B * U1, 2 * H), like=enc)
+        K.joint_gate_pruned_bwd(ex, py, bounds, dh, dex, dpy, B, T, U1, R, H)
+        del dh
+        st = dict(enc_parts=enc_parts, pred_parts=pred_parts, wx=wx, dims=(B, T, U1, H, V, ldv))
+        d_enc, d_pred = _gate_input_grads(dex, dpy, st, model, True, True)
+        ctx.save_for_backward(d_enc, d_pred)
+        return costs
+
+    @staticmethod
+    def backward(ctx, dcosts):
+        m = ctx.model
+        d_enc, d_pred = _scaled_grads_backward(ctx, dcosts, (m.fc1.weight, m.fc1.bias, m.fc_gate.weight, m.fc_gate.bias, m.fc2.weight,
+                                                             m.fc2.bias), "PrunedJointLossFn")
+        return d_enc, d_pred, None, None, None, None, None, None, None, None
+
+
+def check_prune_feasible(frame_lens, label_lens, prune_range):
+    """Raise ValueError naming every utterance with U > T (R - 1): no path through the lattice fits in windows of R label positions
+    (each frame advances a window by at most R - 1).  Reads the lengths on the host."""
+    R = int(prune_range)
+    if R < 2:
+        raise ValueError("prune_range must be >= 2 (got %d)" % R)
+    fl = torch.as_tensor(frame_lens).long().cpu()
+    ll = torch.as_tensor(label_lens).long().cpu()
+    bad = torch.nonzero(ll > fl * (R - 1)).flatten().tolist()
+    if bad:
+        raise ValueError("pruned RNN-T loss: utterance(s) %s have more labels than frames x (prune_range - 1) = %s; no alignment fits "
+                         "in windows of %d label positions (raise --prune_range or drop them)"
+                         % (bad, ["U=%d > T=%d x %d" % (int(ll[i]), int(fl[i]), R - 1) for i in bad], R))
+
+
+def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, simple_scale, pruned_scale, x_len=None, t_out=None):
+    """Pruned RNN-T training path -> (simple_costs [B], pruned_costs [B]).  The gradients wired to every parameter are those of
+    sum_b (simple_scale * simple_b + pruned_scale * pruned_b); back-propagate exactly that sum (TrainStep does).  Refuses, before any
+    work, an utterance that has no path inside the windows.  With grad mode off only the costs are computed.  ``model`` needs the
+    simple projections (Net with prune_range > 0)."""
+    check_prune_feasible(frame_lens, label_lens, prune_range)
+    if not hasattr(model, "simple_am_proj"):
+        raise ValueError("the pruned RNN-T loss needs the simple joiner: build Net with prune_range > 0")
+    R = int(prune_range)
+    fl, ll = frame_lens.int().contiguous(), label_lens.int().contiguous()
+    labels = y.int().contiguous()
+    need = torch.is_grad_enabled()
+    enc = model_encoder_forward_act(model, x, x_len, t_out)
+    pred = prednet_forward_act(model, y)
+    simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need)
+    pruned_costs = PrunedJointLossFn.apply(enc, pred, model, labels, fl, ll, bounds, R, float(pruned_scale), need)
+    return simple_costs, pruned_costs

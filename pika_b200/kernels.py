@@ -2,6 +2,8 @@
 
 torch is used here only for device memory, streams and shape bookkeeping.
 """
+import ctypes
+
 import torch
 
 from . import _lib
@@ -481,3 +483,97 @@ def conv_same_f64(x, n_len, h, m_len, y=None):
     check(lib.pk_conv_same_f64(_P(x), x.stride(0), _P(n_len), _P(h), h.stride(0), _P(m_len), B, n, m, _P(y), y.stride(0), _P(ws), need,
                                _stream()), "pk_conv_same_f64")
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# pruned RNN-T loss (include/pika_b200.h, "Pruned RNN-T loss")
+
+
+def _ws_query(fn, name, *dims):
+    """a workspace size returned through a long long* out-parameter"""
+    out = ctypes.c_longlong(0)
+    check(fn(*dims, ctypes.addressof(out)), name)
+    return int(out.value)
+
+
+def rnnt_lattice(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1, grad_scale=None):
+    """log-prob tables in the lattice's skewed layout [B, T+U1-1, U1] -> (costs [B], gb [B,T,U1], gl [B,T,U1])"""
+    dev = lpb_skew.device
+    ws_bytes = _ws_query(lib.pk_rnnt_lattice_workspace, "pk_rnnt_lattice_workspace", B, T, U1)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    costs = torch.empty(B, dtype=torch.float32, device=dev)
+    gb = torch.empty(B, T, U1, dtype=torch.float32, device=dev)
+    gl = torch.empty_like(gb)
+    check(lib.pk_rnnt_lattice(_P(frame_lens), _P(label_lens), B, T, U1, _P(lpb_skew), _P(lpl_skew), _P(grad_scale), _P(costs), _P(gb),
+                              _P(gl), _P(ws), ws_bytes, _stream()), "pk_rnnt_lattice")
+    return costs, gb, gl
+
+
+def rnnt_simple_prep(src, V, nb, n_in, n_out, hi, lo=None):
+    """src f32 [nb*n_in, ld] -> hi (, lo) bf16 [nb*n_out, ld_out] = exp(src - rowmax) with zero padding; returns rowmax [nb*n_in]"""
+    assert src.dtype == torch.float32 and src.stride(-1) == 1 and hi.dtype == torch.bfloat16 and hi.is_contiguous()
+    rmax = torch.empty(nb * n_in, dtype=torch.float32, device=src.device)
+    check(lib.pk_rnnt_simple_prep(_P(src), src.stride(0), V, nb, n_in, n_out, _P(hi), _P(lo), hi.shape[-1], _P(rmax), _stream()),
+          "pk_rnnt_simple_prep")
+    return rmax
+
+
+def rnnt_simple_tables(am, lm, am_max, lm_max, S, labels, frame_lens, label_lens, B, T, U1):
+    """-> (lpb_skew, lpl_skew) [B, T+U1-1, U1] f32 of the simple joiner"""
+    dev = am.device
+    lpb = torch.empty(B, T + U1 - 1, U1, dtype=torch.float32, device=dev)
+    lpl = torch.empty_like(lpb)
+    check(lib.pk_rnnt_simple_tables(_P(am), _P(lm), am.stride(0), _P(am_max), _P(lm_max), _P(S), S.shape[-1], _P(labels),
+                                    max(labels.stride(0), 1), _P(frame_lens), _P(label_lens), B, T, U1, _P(lpb), _P(lpl), _stream()),
+          "pk_rnnt_simple_tables")
+    return lpb, lpl
+
+
+def rnnt_simple_w(gb, gl, S, frame_lens, label_lens, scale, w_hi, w_lo=None):
+    B, T, U1 = gb.shape
+    check(lib.pk_rnnt_simple_w(_P(gb), _P(gl), _P(S), S.shape[-1], _P(frame_lens), _P(label_lens), _P(scale), B, T, U1, _P(w_hi), _P(w_lo),
+                               w_hi.shape[-1], _stream()), "pk_rnnt_simple_w")
+
+
+def rnnt_simple_grad(src, V, rmax, G, n_g, axis, gb, gl, labels, frame_lens, label_lens, scale, out):
+    """out [rows, ldv] (f32 | bf16): d am (axis 0, rows over t) or d lm (axis 1, rows over u) of the simple loss"""
+    B, T, U1 = gb.shape
+    assert out.is_contiguous() and out.shape[-1] == src.stride(0) and G.stride(-1) == 1
+    check(lib.pk_rnnt_simple_grad(_P(src), src.stride(0), V, _P(rmax), _P(G), G.shape[-1], n_g, axis, _P(gb), _P(gl), _P(labels),
+                                  max(labels.stride(0), 1), _P(frame_lens), _P(label_lens), _P(scale), B, T, U1, _P(out), _dt(out),
+                                  _stream()), "pk_rnnt_simple_grad")
+
+
+def rnnt_prune_bounds(ga, gb, frame_lens, label_lens, R):
+    """occupancy -(ga + gb) [B,T,U1] (gb may be None) -> bounds [B,T] int32"""
+    B, T, U1 = ga.shape
+    bounds = torch.empty(B, T, dtype=torch.int32, device=ga.device)
+    check(lib.pk_rnnt_prune_bounds(_P(ga), _P(gb), _P(frame_lens), _P(label_lens), B, T, U1, R, _P(bounds), _stream()),
+          "pk_rnnt_prune_bounds")
+    return bounds
+
+
+def joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H):
+    check(lib.pk_joint_gate_pruned_fwd(_P(ex), _P(py), _P(bounds), _P(h), _dt(ex), B, T, U1, R, H, _stream()), "pk_joint_gate_pruned_fwd")
+
+
+def joint_gate_pruned_bwd(ex, py, bounds, dh, dex, dpy, B, T, U1, R, H):
+    check(lib.pk_joint_gate_pruned_bwd(_P(ex), _P(py), _P(bounds), _P(dh), _P(dex), _P(dpy), _dt(ex), B, T, U1, R, H, _stream()),
+          "pk_joint_gate_pruned_bwd")
+
+
+def rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=None, dlogits=None, colsum=None, row_lse=None):
+    """logits [B*T*R, ldv] (row (b,t,r) = node (t, bounds[b,t] + r)) -> costs [B]; dlogits (may alias logits) and colsum [ldv] filled
+    when given"""
+    B, T = bounds.shape
+    rows, ldv = logits.shape
+    assert rows == B * T * R and logits.is_contiguous() and labels.dtype == torch.int32 and bounds.dtype == torch.int32
+    ws_bytes = _ws_query(lib.pk_rnnt_pruned_loss_workspace, "pk_rnnt_pruned_loss_workspace", B, T, U1, R, ldv)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=logits.device)
+    costs = torch.empty(B, dtype=torch.float32, device=logits.device)
+    if row_lse is not None:
+        assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (rows, 2)
+    check(lib.pk_rnnt_pruned_loss(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), _P(bounds), B, T, U1, R, V, ldv,
+                                  max(labels.stride(0), 1), _P(grad_scale), _P(costs), _P(dlogits), _P(colsum), _P(ws), ws_bytes,
+                                  _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _stream()), "pk_rnnt_pruned_loss")
+    return costs

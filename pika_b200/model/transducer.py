@@ -13,6 +13,13 @@ from .rnnt_conv_transformer_lm import Net as decoder_transformer
 from .rnnt_tdnn_transformer import Net as encoder_tdnn
 
 
+def add_simple_joiner(net, hid_dim, output_dim):
+    """simple_am_proj / simple_lm_proj: the two linear maps of the simple joiner am[t] + lm[u] (encoder and prediction-net outputs to
+    the vocabulary).  Also used to extend a dense checkpoint for pruned training."""
+    net.simple_am_proj = nn.Linear(hid_dim, output_dim)
+    net.simple_lm_proj = nn.Linear(hid_dim, output_dim)
+
+
 class Net(nn.Module):
     def __init__(self, opt, input_dim, output_dim):
         super().__init__()
@@ -40,6 +47,10 @@ class Net(nn.Module):
         self.fc1 = nn.Linear(2 * self.hid_dim, self.hid_dim)
         self.fc_gate = nn.Linear(2 * self.hid_dim, self.hid_dim)
         self.fc2 = nn.Linear(self.hid_dim, output_dim)
+        if getattr(opt, "prune_range", 0) > 0:
+            # the pruned RNN-T loss's simple joiner (engine.transducer_loss_pruned), created after every module of the reference so
+            # that a seeded Net still draws the reference's weights for those; forward and decoding never use it
+            add_simple_joiner(self, self.hid_dim, output_dim)
 
     def forward(self, x, y, x_len=None, softmax=True):
         """x [B,T,D] f32, y [B,U] int64 -> [B,T',U+1,V] log-probs (or logits if softmax=False).  With the LSTM encoder, x_len

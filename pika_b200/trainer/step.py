@@ -23,6 +23,17 @@ def encoder_out_max(t_max, lctx, rctx, stride):
     return l // stride + (l % stride != 0)
 
 
+def prune_loss_scales(args, i):
+    """(simple_scale, pruned_scale) of the pruned RNN-T objective at global batch index i: (--simple_loss_scale, 1), or during the
+    --prune_warmup_batches W warm-up 1 - (1 - simple_loss_scale) f and 0.1 + 0.9 f with f = min(i / W, 1)"""
+    W = int(getattr(args, "prune_warmup_batches", 0))
+    ss = float(getattr(args, "simple_loss_scale", 0.5))
+    if W <= 0:
+        return ss, 1.0
+    f = min(i / W, 1.0)
+    return 1.0 - (1.0 - ss) * f, 0.1 + 0.9 * f
+
+
 class TrainStep:
     def __init__(self, model, args, frontend, bmuf, optimizer, offset=None, scale=None, spec_augmentor=None):
         self.model, self.args, self.frontend, self.bmuf, self.opt = model, args, frontend, bmuf, optimizer
@@ -50,10 +61,19 @@ class TrainStep:
         feats = self.features(batch)
         len_batch = encoder_out_lens(self.frontend.out_lens(batch["n_frames"]), a.model_lctx, a.model_rctx, a.model_stride)
         t_out = encoder_out_max(int(batch["t_max"]), a.model_lctx, a.model_rctx, a.model_stride)
-        costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out)
+        self.simple_costs = None
+        if getattr(a, "prune_range", 0) > 0:
+            ss, ps = prune_loss_scales(a, a.epoch * a.num_batches_per_epoch + self.num_done)
+            simple, costs = engine.transducer_loss_pruned(self.model, feats, batch["target"], len_batch, batch["ali_lens"], a.prune_range,
+                                                          ss, ps, x_len=len_batch, t_out=t_out)
+            self.simple_costs = simple
+            loss = (simple * ss + costs * ps).sum()                       # upstream gradients: exactly the scales passed above
+        else:
+            costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out)
+            loss = costs.sum()
         engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1
         try:
-            costs.sum().backward()
+            loss.backward()
         finally:
             engine.assume_unit_loss_grad(False)
         self.opt.step()                                                   # clip_grad_norm_(inf) + SGD(nesterov)

@@ -41,7 +41,8 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
         optimizer.reset(lr)
     else:
         optimizer = SgdNesterovClip(bmuf_trainer.flat, lr, args.momentum, args.grad_clip)
-    loss_logger = Logger(args.log, args.log_per_n_frames, ['Loss'])
+    pruned = getattr(args, 'prune_range', 0) > 0
+    loss_logger = Logger(args.log, args.log_per_n_frames, ['Loss', 'Simple'] if pruned else ['Loss'])
     spec = SpecAugment(args.max_freq_span, args.max_time_span) if args.spec_augment else None
     model.train(training)
     step = TrainStep(model, args, args.frontend, bmuf_trainer, optimizer, offset=args.offset, scale=args.scale, spec_augmentor=spec)
@@ -56,23 +57,29 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
                     costs = step(batch)
                 except FloatingPointError:
                     return float('nan')                       # BMUF returned STOP (:113-114)
+                simple = step.simple_costs
             else:
                 with torch.no_grad():
                     feats = step.features(batch)
                     from .step import encoder_out_lens, encoder_out_max
                     tl = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
                     t_out = encoder_out_max(int(batch["t_max"]), args.model_lctx, args.model_rctx, args.model_stride)
-                    costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
+                    if pruned:
+                        simple, costs = engine.transducer_loss_pruned(model, feats, batch["target"], tl, batch["ali_lens"],
+                                                                      args.prune_range, args.simple_loss_scale, 1.0, x_len=tl, t_out=t_out)
+                    else:
+                        costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
             loss = float(costs.sum().item())
+            simple_loss = float(simple.sum().item()) if pruned else 0.0
         else:                                                 # empty batch (:100-101)
-            loss = 0.0
+            loss = simple_loss = 0.0
             if training:
                 try:
                     step.skip()                               # still counts, still syncs (:112-123)
                 except FloatingPointError:
                     return float('nan')
         labels = int(ali_lens_cpu.sum().item())
-        loss_logger.update_and_log(labels, [loss])
+        loss_logger.update_and_log(labels, [loss, simple_loss] if pruned else [loss])
     if training and bmuf_trainer.update_and_sync() != 1:
         return float('nan')
     tot_loss, tot_num = loss_logger.summarize_and_log()
@@ -135,6 +142,15 @@ def build_parser():
     parser.add_argument('--max_freq_span', type=int, default=15)
     parser.add_argument('--max_time_span', type=int, default=35)
     parser.add_argument('--precision', choices=['bf16', 'fp32'], default='bf16', help='pika_b200: compute mode')
+    parser.add_argument('--prune_range', type=int, default=0,
+                        help='pruned RNN-T loss: train the joint over this many label positions per frame, chosen by a simple joiner '
+                             '(DESIGN.md "Pruned RNN-T"); 0 = the full joint (default), otherwise >= 2.  The logged Loss is then the '
+                             'pruned cost and Simple the simple joiner\'s')
+    parser.add_argument('--simple_loss_scale', type=float, default=0.5,
+                        help='weight of the simple joiner\'s loss in the pruned objective (the pruned loss has weight 1)')
+    parser.add_argument('--prune_warmup_batches', type=int, default=0,
+                        help='ramp the pruned loss weight from 0.1 to 1 and the simple loss weight from 1 to --simple_loss_scale '
+                             'linearly over this many batches; 0 = off')
     return parser
 
 
@@ -168,6 +184,11 @@ def main(argv=None):
         model = nnet_module.Net(args, args.input_dim, args.output_dim)
     else:
         model = torch.load(args.init_model, map_location=lambda storage, loc: storage, weights_only=False)
+        if args.prune_range > 0 and not hasattr(model, 'simple_am_proj'):
+            from ..model.transducer import add_simple_joiner
+            add_simple_joiner(model, model.fc2.weight.shape[1], model.fc2.weight.shape[0])   # drawn after the seed above
+    if args.prune_range == 1 or args.prune_range < 0:
+        parser.error('--prune_range must be 0 (off) or >= 2')
     model.to(dev)
     flat = FlatParams(model)
     if args.block_sync == 'bmuf_adam':
