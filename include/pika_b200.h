@@ -171,6 +171,17 @@ int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, 
  *   y_{u+1}); axis 1 -> d lm rows (b, u) [B*U1, ldv]: the same with the sums over t.  G = W.P (axis 0) or W^T.E (axis 1), f32, row
  *   (b, i) at b*n_g + i, pitch ld_g.  One CTA per row; the blank / label terms are added by one thread in a fixed order.
  *   out_dtype PK_F32 | PK_BF16; columns [V, ldv) are written 0.  ldv <= 51200.
+ * Smoothing (DESIGN.md "Pruned RNN-T"; lam_l = lm_only_scale, lam_a = am_only_scale, both >= 0 with lam_l + lam_a < 1, mu = 1 - both):
+ * pk_rnnt_simple_smooth_stats: am [B*T, ldv], lm [B*U1, ldv] f32 (V valid columns) and their row maxes from pk_rnnt_simple_prep ->
+ *   Nl [B*U1] = logsumexp_v lm[u], logq [ldv] = log(mean of softmax(lm[b, u]) over the batch's valid rows u <= U_b + 1e-10) (0 on
+ *   the columns [V, ldv)), Na [B*T] = logsumexp_v (am[t] + logq).  Rows past T_b / U_b are written 0 and enter no sum; the unigram's
+ *   column partials are summed per 64-row chunk, then in chunk order (no atomics).  workspace >= the size
+ *   pk_rnnt_simple_smooth_stats_workspace writes to *bytes.
+ * pk_rnnt_simple_tables_smooth: as pk_rnnt_simple_tables with lp = mu (z[k] - N) + lam_l (lm[u,k] - Nl[u]) + lam_a (am[t,k] + logq[k]
+ *   - Na[t]) for k = 0 and k = y_{u+1}.
+ * pk_rnnt_simple_grad_smooth: as pk_rnnt_simple_grad (G formed from W with the scale mu * scale[b]) with the blank / label terms
+ *   weighted by scale[b] (mu + lam) and the row term scale[b] lam Gamma softmax(src [+ logq]), Gamma the row's summed occupancy;
+ *   lam = lam_a with logq and lse = Na on axis 0, lam_l with lse = Nl on axis 1 (logq is not read there).
  * pk_rnnt_prune_bounds: occupancy gamma = -(ga + gb) (gb may be NULL) [B][T][U1] f32 -> bounds [B][T] int32 (DESIGN.md "Pruned RNN-T":
  *   window argmax in f64 with the smallest start on ties, clamp, running max, reverse pass; padded frames copy the last frame).
  *   An utterance with U_b > T_b (R-1) has no path inside the windows: its bounds are all -1 (the pruned loss is then +inf).
@@ -193,6 +204,18 @@ int pk_rnnt_simple_w(const float* gb, const float* gl, const float* S, int ld_s,
 int pk_rnnt_simple_grad(const float* src, int ldv, int V, const float* rmax, const float* G, int ld_g, int n_g, int axis, const float* gb,
                         const float* gl, const int* labels, int ld_labels, const int* frame_lens, const int* label_lens, const float* scale,
                         int B, int T, int U1, void* out, int out_dtype, void* stream);
+int pk_rnnt_simple_smooth_stats_workspace(int B, int U1, int ldv, long long* bytes);
+int pk_rnnt_simple_smooth_stats(const float* am, const float* lm, int ldv, int V, const float* am_max, const float* lm_max,
+                                const int* frame_lens, const int* label_lens, int B, int T, int U1, float* Nl, float* logq, float* Na,
+                                void* workspace, long long workspace_bytes, void* stream);
+int pk_rnnt_simple_tables_smooth(const float* am, const float* lm, int ldv, const float* am_max, const float* lm_max, const float* S,
+                                 int ld_s, const int* labels, int ld_labels, const int* frame_lens, const int* label_lens, int B, int T,
+                                 int U1, const float* Nl, const float* logq, const float* Na, float lm_only_scale, float am_only_scale,
+                                 float* lpb_skew, float* lpl_skew, void* stream);
+int pk_rnnt_simple_grad_smooth(const float* src, int ldv, int V, const float* rmax, const float* G, int ld_g, int n_g, int axis,
+                               const float* gb, const float* gl, const int* labels, int ld_labels, const int* frame_lens,
+                               const int* label_lens, const float* scale, const float* logq, const float* lse, float lm_only_scale,
+                               float am_only_scale, int B, int T, int U1, void* out, int out_dtype, void* stream);
 int pk_rnnt_prune_bounds(const float* ga, const float* gb, const int* frame_lens, const int* label_lens, int B, int T, int U1, int R,
                          int* bounds, void* stream);
 int pk_joint_gate_pruned_fwd(const void* ex, const void* py, const int* bounds, void* h, int dtype, int B, int T, int U1, int R, int H,

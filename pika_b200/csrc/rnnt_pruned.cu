@@ -9,6 +9,7 @@
 //     pk_rnnt_simple_w       W = scale * gamma / S, gamma = -(gb + gl): the operand of the two gradient GEMMs W.P and W^T.E
 //     pk_rnnt_simple_grad    dam = E (.) (W P) + blank / label terms, dlm = P (.) (W^T E) + blank / label terms; one CTA per row,
 //                            the terms added by one thread in a fixed order (no atomics)
+//     pk_rnnt_simple_smooth_stats, _tables_smooth, _grad_smooth   the same with LM-only / AM-only log-probs mixed into the lattice
 //   pk_rnnt_prune_bounds     the simple occupancies -> the first label position s[b, t] of each frame's window of R positions
 //   pk_joint_gate_pruned_fwd / _bwd   the factored gate h = tanh(ex1 + py1) * sigmoid(exg + pyg) on the B*T*R rows (t, s_t + r)
 // The pruned loss itself (tables from the [B*T*R, ldv] logits, lattice, gradient) is pk_rnnt_pruned_loss in rnnt_loss.cu, next to
@@ -68,13 +69,84 @@ __global__ void __launch_bounds__(256) simple_prep_kernel(const float* __restric
 
 PK_DEVICE size_t skew_at(int ND, int U1, int b, int t, int u) { return ((size_t)b * ND + (t + u)) * U1 + u; }
 
-// one thread per node (b, t, u) of the valid lattice: N = log(max(S, floor)) + the two maxes; lpb = z[0] - N, lpl = z[y_{u+1}] - N
+PK_DEVICE float block_reduce_sum(float v, float* s_red) {   // blockDim.x == 256; the partials are added in warp order
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float r = s_red[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) r += s_red[i];
+    __syncthreads();
+    return r;
+}
+
+// ------------------------------------------------------------------------------------ smoothing statistics
+// The LM-only / AM-only terms' normalisers and the batch unigram q (DESIGN.md "Pruned RNN-T").  Rows outside the valid lengths are
+// written 0 and never read; they enter no sum.
+constexpr int kSmoothRowChunk = 64;            // lm rows per column-partial CTA of the unigram
+
+// one CTA per row i < n_rows of utterance b (rows with i > last valid are written 0):
+//   out = rmax + log sum_{v<V} exp(src + (lq ? lq : 0) - rmax).  With lq = log q <= 0, rmax (the row max of src) still bounds the
+//   exponents, and the term at the row's argmax is >= q_min = 1e-10, so the sum cannot underflow to 0.
+__global__ void __launch_bounds__(256) smooth_lse_kernel(const float* __restrict__ src, int ldv, int V, const float* __restrict__ rmax,
+                                                         const float* __restrict__ lq, const int* __restrict__ lens, int len_off,
+                                                         int n_rows, float* __restrict__ out) {
+    __shared__ float s_red[8];
+    const int b = blockIdx.x / n_rows, i = blockIdx.x - b * n_rows;
+    if (i >= lens[b] + len_off) {
+        if (threadIdx.x == 0) out[blockIdx.x] = 0.f;
+        return;
+    }
+    const float* x = src + (long long)blockIdx.x * ldv;
+    const float m = rmax[blockIdx.x];
+    float s = 0.f;
+    for (int c = threadIdx.x; c < V; c += 256) s += expf(x[c] + (lq ? lq[c] : 0.f) - m);
+    s = block_reduce_sum(s, s_red);
+    if (threadIdx.x == 0) out[blockIdx.x] = m + logf(s);
+}
+
+// grid (ceil(ldv / 256), n_chunks): column partials part[chunk][c] = sum over the valid rows of chunk (rows chunk*64 .. +63 of the
+// flattened [B*U1] lm, ascending) of exp(lm - Nl); columns >= V are 0
+__global__ void __launch_bounds__(256) smooth_q_part_kernel(const float* __restrict__ lm, int ldv, int V, const float* __restrict__ Nl,
+                                                            const int* __restrict__ label_lens, int B, int U1, float* __restrict__ part) {
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    if (c >= ldv) return;
+    const long long r0 = (long long)blockIdx.y * kSmoothRowChunk, n = (long long)B * U1;
+    float s = 0.f;
+    if (c < V) {
+        for (long long r = r0; r < r0 + kSmoothRowChunk && r < n; ++r) {
+            const int b = (int)(r / U1), u = (int)(r - (long long)b * U1);
+            if (u <= label_lens[b]) s += expf(lm[r * ldv + c] - Nl[r]);
+        }
+    }
+    part[(long long)blockIdx.y * ldv + c] = s;
+}
+
+// log q[c] = log(sum of the chunk partials in chunk order / sum_b (U_b + 1) + 1e-10) for c < V; 0 on the padding columns
+__global__ void __launch_bounds__(256) smooth_q_finish_kernel(const float* __restrict__ part, int n_chunks, int ldv, int V,
+                                                              const int* __restrict__ label_lens, int B, float* __restrict__ logq) {
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    if (c >= ldv) return;
+    if (c >= V) { logq[c] = 0.f; return; }
+    long long rows = 0;
+    for (int b = 0; b < B; ++b) rows += label_lens[b] + 1;
+    float s = 0.f;
+    for (int k = 0; k < n_chunks; ++k) s += part[(long long)k * ldv + c];
+    logq[c] = logf(s / (float)rows + 1e-10f);
+}
+
+// one thread per node (b, t, u) of the valid lattice: N = log(max(S, floor)) + the two maxes; lpb = z[0] - N, lpl = z[y_{u+1}] - N.
+// SMOOTH: lp = mu (z[k] - N) + lam_l (lm[u,k] - Nl[u]) + lam_a (am[t,k] + log q[k] - Na[t]), mu = 1 - lam_l - lam_a.
+template <bool SMOOTH>
 __global__ void __launch_bounds__(256) simple_tables_kernel(const float* __restrict__ am, const float* __restrict__ lm, int ldv,
                                                             const float* __restrict__ am_max, const float* __restrict__ lm_max,
                                                             const float* __restrict__ S, int ld_s, const int* __restrict__ labels,
                                                             int ld_labels, const int* __restrict__ frame_lens,
                                                             const int* __restrict__ label_lens, int B, int T, int U1,
-                                                            float* __restrict__ lpb_skew, float* __restrict__ lpl_skew) {
+                                                            float* __restrict__ lpb_skew, float* __restrict__ lpl_skew,
+                                                            const float* __restrict__ Nl = nullptr, const float* __restrict__ logq = nullptr,
+                                                            const float* __restrict__ Na = nullptr, float mu = 1.f, float lam_l = 0.f,
+                                                            float lam_a = 0.f) {
     const long long n = (long long)B * T * U1;
     const int ND = T + U1 - 1;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -86,10 +158,20 @@ __global__ void __launch_bounds__(256) simple_tables_kernel(const float* __restr
         const long long ar = bt, lr = (long long)b * U1 + u;
         const float N = logf(fmaxf(S[bt * ld_s + u], kSimpleFloor)) + am_max[ar] + lm_max[lr];
         const size_t sk = skew_at(ND, U1, b, t, u);
-        lpb_skew[sk] = (am[ar * ldv] + lm[lr * ldv]) - N;
-        if (u < Un) {
-            const int y = labels[(size_t)b * ld_labels + u];
-            lpl_skew[sk] = (am[ar * ldv + y] + lm[lr * ldv + y]) - N;
+        if constexpr (SMOOTH) {
+            const float nl = Nl[lr], na = Na[ar];
+            lpb_skew[sk] = mu * ((am[ar * ldv] + lm[lr * ldv]) - N) + lam_l * (lm[lr * ldv] - nl) + lam_a * ((am[ar * ldv] + logq[0]) - na);
+            if (u < Un) {
+                const int y = labels[(size_t)b * ld_labels + u];
+                lpl_skew[sk] = mu * ((am[ar * ldv + y] + lm[lr * ldv + y]) - N) + lam_l * (lm[lr * ldv + y] - nl) +
+                               lam_a * ((am[ar * ldv + y] + logq[y]) - na);
+            }
+        } else {
+            lpb_skew[sk] = (am[ar * ldv] + lm[lr * ldv]) - N;
+            if (u < Un) {
+                const int y = labels[(size_t)b * ld_labels + u];
+                lpl_skew[sk] = (am[ar * ldv + y] + lm[lr * ldv + y]) - N;
+            }
         }
     }
 }
@@ -121,14 +203,19 @@ __global__ void __launch_bounds__(256) simple_w_kernel(const float* __restrict__
 // d[row] = exp(src[row] - rmax[row]) (.) G[row] over the V columns, then the blank term at column 0 and the label terms at their
 // columns, each summed by one thread in a fixed order.  axis 0: rows (b, t), the terms sum over u of node (t, u); axis 1: rows (b, u),
 // the terms sum over t.  G row of (b, i) is b * n_g + i.  One CTA per row, the row staged in shared memory (ldv floats).
-template <typename TO>
+// SMOOTH: the blank / label terms are weighted by (mu + lam), and the row gains scale * lam * Gamma * exp(src + lq - lse) with
+// Gamma = -(sum of the blank terms + sum of the label terms) accumulated by the same thread in the same order (lq: log q on axis 0,
+// NULL on axis 1; lse: Na or Nl).
+template <typename TO, bool SMOOTH>
 __global__ void __launch_bounds__(256) simple_grad_kernel(const float* __restrict__ src, int ldv, int V, const float* __restrict__ rmax,
                                                           const float* __restrict__ G, int ld_g, int n_g, int axis,
                                                           const float* __restrict__ gb, const float* __restrict__ gl,
                                                           const int* __restrict__ labels, int ld_labels, const int* __restrict__ frame_lens,
                                                           const int* __restrict__ label_lens, const float* __restrict__ scale, int T,
-                                                          int U1, TO* __restrict__ out) {
+                                                          int U1, TO* __restrict__ out, const float* __restrict__ lq = nullptr,
+                                                          const float* __restrict__ lse = nullptr, float mu = 1.f, float lam = 0.f) {
     extern __shared__ float s_row[];
+    __shared__ float s_gam;
     const int n_rows_b = axis == 0 ? T : U1;
     const int b = blockIdx.x / n_rows_b, i = blockIdx.x - b * n_rows_b;
     const long long row = blockIdx.x;
@@ -141,7 +228,28 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const float* __restric
         const int Tn = frame_lens[b], Un = label_lens[b];
         const float sc = scale ? scale[b] : 1.f;
         const long long node0 = (long long)b * T * U1;
-        if (axis == 0 && i < Tn) {
+        if constexpr (SMOOTH) {
+            const float k = sc * (mu + lam);
+            float blank = 0.f, lab = 0.f;
+            if (axis == 0 && i < Tn) {
+                for (int u = 0; u <= Un; ++u) blank += gb[node0 + (long long)i * U1 + u];
+                s_row[0] += k * blank;
+                for (int u = 0; u < Un; ++u) {
+                    const float g = gl[node0 + (long long)i * U1 + u];
+                    lab += g;
+                    s_row[labels[(size_t)b * ld_labels + u]] += k * g;
+                }
+            } else if (axis == 1 && i <= Un) {
+                for (int t = 0; t < Tn; ++t) {
+                    blank += gb[node0 + (long long)t * U1 + i];
+                    lab += gl[node0 + (long long)t * U1 + i];
+                }
+                if (i == Un) lab = 0.f;
+                s_row[0] += k * blank;
+                if (i < Un) s_row[labels[(size_t)b * ld_labels + i]] += k * lab;
+            }
+            s_gam = -(blank + lab) * sc * lam;
+        } else if (axis == 0 && i < Tn) {
             float blank = 0.f;
             for (int u = 0; u <= Un; ++u) blank += gb[node0 + (long long)i * U1 + u];
             s_row[0] += sc * blank;
@@ -158,6 +266,15 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const float* __restric
     }
     __syncthreads();
     TO* o = out + row * ldv;
+    if constexpr (SMOOTH) {
+        const float w = s_gam;                   // 0 on padded rows, whose lse is not defined
+        if (w != 0.f) {
+            const float l = lse[row];
+            for (int c = threadIdx.x; c < ldv; c += 256)
+                o[c] = from_f32<TO>(c < V ? s_row[c] + w * expf(x[c] + (lq ? lq[c] : 0.f) - l) : 0.f);
+            return;
+        }
+    }
     for (int c = threadIdx.x; c < ldv; c += 256) o[c] = from_f32<TO>(s_row[c]);
 }
 
@@ -306,8 +423,59 @@ extern "C" int pk_rnnt_simple_tables(const float* am, const float* lm, int ldv, 
     using namespace pk;
     PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && ld_s >= U1, "bad dims");
     const long long n = (long long)B * T * U1;
-    simple_tables_kernel<<<grid_of(n), 256, 0, STREAM(stream)>>>(am, lm, ldv, am_max, lm_max, S, ld_s, labels, ld_labels, frame_lens,
-                                                                  label_lens, B, T, U1, lpb_skew, lpl_skew);
+    simple_tables_kernel<false><<<grid_of(n), 256, 0, STREAM(stream)>>>(am, lm, ldv, am_max, lm_max, S, ld_s, labels, ld_labels, frame_lens,
+                                                                         label_lens, B, T, U1, lpb_skew, lpl_skew);
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
+static bool smooth_scales_ok(float lam_l, float lam_a) {
+    return lam_l >= 0.f && lam_a >= 0.f && (double)lam_l + (double)lam_a < 1.0;   // false for NaN too
+}
+
+extern "C" int pk_rnnt_simple_smooth_stats_workspace(int B, int U1, int ldv, long long* bytes) {
+    PK_CHECK_ARG(bytes, "null pointer");
+    PK_CHECK_ARG(B > 0 && U1 > 0 && ldv > 0, "bad dims");
+    const long long chunks = ((long long)B * U1 + pk::kSmoothRowChunk - 1) / pk::kSmoothRowChunk;
+    *bytes = chunks * ldv * 4;
+    return 0;
+}
+
+extern "C" int pk_rnnt_simple_smooth_stats(const float* am, const float* lm, int ldv, int V, const float* am_max, const float* lm_max,
+                                           const int* frame_lens, const int* label_lens, int B, int T, int U1, float* Nl, float* logq,
+                                           float* Na, void* workspace, long long workspace_bytes, void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(am && lm && am_max && lm_max && frame_lens && label_lens && Nl && logq && Na && workspace, "null pointer");
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && V > 0 && ldv >= V, "bad dims");
+    const int chunks = (int)(((long long)B * U1 + kSmoothRowChunk - 1) / kSmoothRowChunk);
+    PK_CHECK_ARG(chunks <= 65535, "B * U1 too large for the unigram's row chunks (B * U1 <= 4194240)");
+    PK_CHECK_ARG(workspace_bytes >= (long long)chunks * ldv * 4, "workspace too small (pk_rnnt_simple_smooth_stats_workspace)");
+    float* part = (float*)workspace;
+    const int col_blocks = (ldv + 255) / 256;
+    smooth_lse_kernel<<<B * U1, 256, 0, STREAM(stream)>>>(lm, ldv, V, lm_max, nullptr, label_lens, 1, U1, Nl);
+    PK_CHECK_LAUNCH(); count_launch();
+    smooth_q_part_kernel<<<dim3(col_blocks, chunks), 256, 0, STREAM(stream)>>>(lm, ldv, V, Nl, label_lens, B, U1, part);
+    PK_CHECK_LAUNCH(); count_launch();
+    smooth_q_finish_kernel<<<col_blocks, 256, 0, STREAM(stream)>>>(part, chunks, ldv, V, label_lens, B, logq);
+    PK_CHECK_LAUNCH(); count_launch();
+    smooth_lse_kernel<<<B * T, 256, 0, STREAM(stream)>>>(am, ldv, V, am_max, logq, frame_lens, 0, T, Na);
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
+extern "C" int pk_rnnt_simple_tables_smooth(const float* am, const float* lm, int ldv, const float* am_max, const float* lm_max,
+                                            const float* S, int ld_s, const int* labels, int ld_labels, const int* frame_lens,
+                                            const int* label_lens, int B, int T, int U1, const float* Nl, const float* logq, const float* Na,
+                                            float lm_only_scale, float am_only_scale, float* lpb_skew, float* lpl_skew, void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(Nl && logq && Na, "null pointer");
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && ld_s >= U1, "bad dims");
+    PK_CHECK_ARG(smooth_scales_ok(lm_only_scale, am_only_scale), "need lm_only_scale >= 0, am_only_scale >= 0, their sum < 1");
+    const float mu = 1.f - lm_only_scale - am_only_scale;
+    const long long n = (long long)B * T * U1;
+    simple_tables_kernel<true><<<grid_of(n), 256, 0, STREAM(stream)>>>(am, lm, ldv, am_max, lm_max, S, ld_s, labels, ld_labels, frame_lens,
+                                                                        label_lens, B, T, U1, lpb_skew, lpl_skew, Nl, logq, Na, mu,
+                                                                        lm_only_scale, am_only_scale);
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }
@@ -335,14 +503,46 @@ extern "C" int pk_rnnt_simple_grad(const float* src, int ldv, int V, const float
     const int rows = B * (axis == 0 ? T : U1);
     if (out_dtype == PK_BF16) {
         static bool cfg = false;
-        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
-        simple_grad_kernel<__nv_bfloat16><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
-                                                                               frame_lens, label_lens, scale, T, U1, (__nv_bfloat16*)out);
+        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<__nv_bfloat16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
+        simple_grad_kernel<__nv_bfloat16, false><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
+                                                                                      frame_lens, label_lens, scale, T, U1, (__nv_bfloat16*)out);
     } else {
         static bool cfg = false;
-        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
-        simple_grad_kernel<float><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
-                                                                       frame_lens, label_lens, scale, T, U1, (float*)out);
+        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
+        simple_grad_kernel<float, false><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
+                                                                              frame_lens, label_lens, scale, T, U1, (float*)out);
+    }
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
+extern "C" int pk_rnnt_simple_grad_smooth(const float* src, int ldv, int V, const float* rmax, const float* G, int ld_g, int n_g, int axis,
+                                          const float* gb, const float* gl, const int* labels, int ld_labels, const int* frame_lens,
+                                          const int* label_lens, const float* scale, const float* logq, const float* lse,
+                                          float lm_only_scale, float am_only_scale, int B, int T, int U1, void* out, int out_dtype,
+                                          void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(axis == 0 || axis == 1, "axis must be 0 (rows over t) or 1 (rows over u)");
+    PK_CHECK_ARG(out_dtype == PK_F32 || out_dtype == PK_BF16, "bad dtype");
+    PK_CHECK_ARG(lse && (axis == 1 || logq), "null pointer (lse; logq on axis 0)");
+    PK_CHECK_ARG(smooth_scales_ok(lm_only_scale, am_only_scale), "need lm_only_scale >= 0, am_only_scale >= 0, their sum < 1");
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && V > 0 && ldv >= V && ld_g >= ldv && n_g >= (axis == 0 ? T : U1), "bad dims");
+    const size_t smem = (size_t)ldv * 4;
+    PK_CHECK_ARG(smem <= 200 * 1024, "ldv too large for the shared-memory row (ldv <= 51200)");
+    const int rows = B * (axis == 0 ? T : U1);
+    const float mu = 1.f - lm_only_scale - am_only_scale, lam = axis == 0 ? am_only_scale : lm_only_scale;
+    const float* lq = axis == 0 ? logq : nullptr;
+    if (out_dtype == PK_BF16) {
+        static bool cfg = false;
+        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<__nv_bfloat16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
+        simple_grad_kernel<__nv_bfloat16, true><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
+                                                                                     frame_lens, label_lens, scale, T, U1, (__nv_bfloat16*)out,
+                                                                                     lq, lse, mu, lam);
+    } else {
+        static bool cfg = false;
+        if (!cfg) { PK_CHECK_CUDA(cudaFuncSetAttribute(simple_grad_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); cfg = true; }
+        simple_grad_kernel<float, true><<<rows, 256, smem, STREAM(stream)>>>(src, ldv, V, rmax, G, ld_g, n_g, axis, gb, gl, labels, ld_labels,
+                                                                             frame_lens, label_lens, scale, T, U1, (float*)out, lq, lse, mu, lam);
     }
     PK_CHECK_LAUNCH(); count_launch();
     return 0;

@@ -1205,10 +1205,23 @@ def _proj_backward(d, x_parts, lin, V):
     return dx
 
 
-def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.0, need_grad=True):
+def check_smoothing_scales(lm_only_scale, am_only_scale):
+    """-> (lm_only_scale, am_only_scale) as floats; ValueError unless both are >= 0 and their sum is < 1"""
+    lam_l, lam_a = float(lm_only_scale), float(am_only_scale)
+    if not (lam_l >= 0.0 and lam_a >= 0.0 and lam_l + lam_a < 1.0):
+        raise ValueError("simple-loss smoothing needs lm_only_scale >= 0, am_only_scale >= 0 and lm_only_scale + am_only_scale < 1 "
+                         "(got %r, %r)" % (lm_only_scale, am_only_scale))
+    return lam_l, lam_a
+
+
+def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.0, need_grad=True, lm_only_scale=0.0, am_only_scale=0.0):
     """The simple joiner's RNN-T loss from its two projections am [B*T, ldv], lm [B*U1, ldv] (f32, V valid columns) -> (costs [B],
     bounds [B,T] int32 for windows of R, dam, dlm) with dam [B*T, ldv], dlm [B*U1, ldv] (activation dtype, padding columns 0) the
-    gradients of sum_b scale * cost_b, or None when ``need_grad`` is False.  R = 0: no bounds (None)."""
+    gradients of sum_b scale * cost_b, or None when ``need_grad`` is False.  R = 0: no bounds (None).
+    ``lm_only_scale`` / ``am_only_scale`` (lam_l, lam_a): the lattice's log-probs become mu * full + lam_l * LM-only + lam_a * AM-only,
+    mu = 1 - lam_l - lam_a (DESIGN.md "Pruned RNN-T"); costs and bounds are then the smoothed ones.  Both 0: the unsmoothed kernels."""
+    lam_l, lam_a = check_smoothing_scales(lm_only_scale, am_only_scale)
+    smooth = lam_l > 0.0 or lam_a > 0.0
     ldv = am.shape[1]
     U1p = (U1 + 7) // 8 * 8
     dev = am.device
@@ -1224,7 +1237,12 @@ def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.
     S = torch.empty(B, T, U1p, dtype=torch.float32, device=dev)
     with _Tap("simple_loss"):
         gemm_parts([E3], [P3], S)                                   # S[t,u] = E[t] . P[u]
-        lpb, lpl = K.rnnt_simple_tables(am, lm, am_max, lm_max, S.view(B * T, U1p), labels, frame_lens, label_lens, B, T, U1)
+        if smooth:
+            Nl, logq, Na = K.rnnt_simple_smooth_stats(am, lm, V, am_max, lm_max, frame_lens, label_lens, B, T, U1)
+            lpb, lpl = K.rnnt_simple_tables_smooth(am, lm, am_max, lm_max, S.view(B * T, U1p), labels, frame_lens, label_lens, B, T, U1,
+                                                   Nl, logq, Na, lam_l, lam_a)
+        else:
+            lpb, lpl = K.rnnt_simple_tables(am, lm, am_max, lm_max, S.view(B * T, U1p), labels, frame_lens, label_lens, B, T, U1)
         costs, gb, gl = K.rnnt_lattice(lpb, lpl, frame_lens, label_lens, B, T, U1)
     del lpb, lpl
     bounds = None
@@ -1234,8 +1252,13 @@ def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.
     if not need_grad:
         return costs, bounds, None, None
     scale_t = torch.full((B,), float(scale), dtype=torch.float32, device=dev)
+    scale_w = scale_t
+    if smooth:                  # the full term's share of the gradient: W = mu * scale * gamma / S, mu in f32 as the kernels form it
+        f32 = lambda v: torch.tensor(v, dtype=torch.float32)                 # noqa: E731
+        mu = f32(1.0) - f32(lam_l) - f32(lam_a)
+        scale_w = torch.full((B,), float(f32(float(scale)) * mu), dtype=torch.float32, device=dev)
     W = parts(B * T, U1p)
-    K.rnnt_simple_w(gb, gl, S.view(B * T, U1p), frame_lens, label_lens, scale_t, W[0], W[1] if split else None)
+    K.rnnt_simple_w(gb, gl, S.view(B * T, U1p), frame_lens, label_lens, scale_w, W[0], W[1] if split else None)
     W3 = [w.view(B, T, U1p) for w in W]
     WP = torch.empty(B, T, ldv, dtype=torch.float32, device=dev)
     WtE = torch.empty(B, U1p, ldv, dtype=torch.float32, device=dev)
@@ -1244,8 +1267,14 @@ def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.
     del W, W3, E, E3, P, P3, S
     dam = _new((B * T, ldv), like=am)
     dlm = _new((B * U1, ldv), like=am)
-    K.rnnt_simple_grad(am, V, am_max, WP.view(B * T, ldv), T, 0, gb, gl, labels, frame_lens, label_lens, scale_t, dam)
-    K.rnnt_simple_grad(lm, V, lm_max, WtE.view(B * U1p, ldv), U1p, 1, gb, gl, labels, frame_lens, label_lens, scale_t, dlm)
+    if smooth:
+        K.rnnt_simple_grad_smooth(am, V, am_max, WP.view(B * T, ldv), T, 0, gb, gl, labels, frame_lens, label_lens, scale_t, logq, Na,
+                                  lam_l, lam_a, dam)
+        K.rnnt_simple_grad_smooth(lm, V, lm_max, WtE.view(B * U1p, ldv), U1p, 1, gb, gl, labels, frame_lens, label_lens, scale_t, logq, Nl,
+                                  lam_l, lam_a, dlm)
+    else:
+        K.rnnt_simple_grad(am, V, am_max, WP.view(B * T, ldv), T, 0, gb, gl, labels, frame_lens, label_lens, scale_t, dam)
+        K.rnnt_simple_grad(lm, V, lm_max, WtE.view(B * U1p, ldv), U1p, 1, gb, gl, labels, frame_lens, label_lens, scale_t, dlm)
     return costs, bounds, dam, dlm
 
 
@@ -1254,10 +1283,11 @@ class SimpleLossFn(torch.autograd.Function):
     am = simple_am_proj(enc), lm = simple_lm_proj(pred) in f32; z[t,u] = am[t] + lm[u] is never formed: the normaliser is
     log(E.P^T) + the row maxes (pk_rnnt_simple_*), the lattice runs on the resulting tables (pk_rnnt_lattice) and its occupancies give the
     bounds (pk_rnnt_prune_bounds).  The gradients (for an upstream gradient of ``scale`` per utterance) are formed here in forward:
-    dam = E (.) (W P) and dlm = P (.) (W^T E) plus the blank / label terms, W = scale * occupancy / (E.P^T)."""
+    dam = E (.) (W P) and dlm = P (.) (W^T E) plus the blank / label terms, W = scale * occupancy / (E.P^T).  ``lm_only_scale`` /
+    ``am_only_scale`` smooth the lattice as in simple_loss."""
 
     @staticmethod
-    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, R, scale, need_grad):
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, R, scale, need_grad, lm_only_scale=0.0, am_only_scale=0.0):
         B, T, H = enc.shape
         U1 = pred.shape[1]
         am_p, lm_p = model.simple_am_proj, model.simple_lm_proj
@@ -1269,7 +1299,8 @@ class SimpleLossFn(torch.autograd.Function):
         lm = torch.zeros(B * U1, ldv, dtype=torch.float32, device=enc.device)
         gemm_parts([enc_parts], [stage_weight(am_p.weight)], am[:, :V], bias=am_p.bias.detach())
         gemm_parts([pred_parts], [stage_weight(lm_p.weight)], lm[:, :V], bias=lm_p.bias.detach())
-        costs, bounds, dam, dlm = simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale, need_grad)
+        costs, bounds, dam, dlm = simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale, need_grad, lm_only_scale,
+                                              am_only_scale)
         del am, lm
         ctx.mark_non_differentiable(bounds)
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
@@ -1284,7 +1315,7 @@ class SimpleLossFn(torch.autograd.Function):
         m = ctx.model
         d_enc, d_pred = _scaled_grads_backward(ctx, dcosts, (m.simple_am_proj.weight, m.simple_am_proj.bias, m.simple_lm_proj.weight,
                                                              m.simple_lm_proj.bias), "SimpleLossFn")
-        return d_enc, d_pred, None, None, None, None, None, None, None
+        return d_enc, d_pred, None, None, None, None, None, None, None, None, None
 
 
 class PrunedJointLossFn(torch.autograd.Function):
@@ -1368,11 +1399,14 @@ def check_prune_feasible(frame_lens, label_lens, prune_range):
                          % (bad, ["U=%d > T=%d x %d" % (int(ll[i]), int(fl[i]), R - 1) for i in bad], R))
 
 
-def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, simple_scale, pruned_scale, x_len=None, t_out=None):
+def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, simple_scale, pruned_scale, x_len=None, t_out=None,
+                           lm_only_scale=0.0, am_only_scale=0.0):
     """Pruned RNN-T training path -> (simple_costs [B], pruned_costs [B]).  The gradients wired to every parameter are those of
     sum_b (simple_scale * simple_b + pruned_scale * pruned_b); back-propagate exactly that sum (TrainStep does).  Refuses, before any
     work, an utterance that has no path inside the windows.  With grad mode off only the costs are computed.  ``model`` needs the
-    simple projections (Net with prune_range > 0)."""
+    simple projections (Net with prune_range > 0).  ``lm_only_scale`` / ``am_only_scale`` smooth the simple loss (simple_loss); its
+    costs and the bounds are then the smoothed ones.  Out-of-range scales raise ValueError before any work."""
+    lam_l, lam_a = check_smoothing_scales(lm_only_scale, am_only_scale)
     check_prune_feasible(frame_lens, label_lens, prune_range)
     if not hasattr(model, "simple_am_proj"):
         raise ValueError("the pruned RNN-T loss needs the simple joiner: build Net with prune_range > 0")
@@ -1382,6 +1416,6 @@ def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, sim
     need = torch.is_grad_enabled()
     enc = model_encoder_forward_act(model, x, x_len, t_out)
     pred = prednet_forward_act(model, y)
-    simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need)
+    simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need, lam_l, lam_a)
     pruned_costs = PrunedJointLossFn.apply(enc, pred, model, labels, fl, ll, bounds, R, float(pruned_scale), need)
     return simple_costs, pruned_costs

@@ -544,6 +544,45 @@ def rnnt_simple_grad(src, V, rmax, G, n_g, axis, gb, gl, labels, frame_lens, lab
                                   _stream()), "pk_rnnt_simple_grad")
 
 
+def rnnt_simple_smooth_stats(am, lm, V, am_max, lm_max, frame_lens, label_lens, B, T, U1):
+    """the smoothing terms' statistics -> (Nl [B*U1], logq [ldv], Na [B*T]) f32; rows past the lengths are 0"""
+    assert am.dtype == lm.dtype == torch.float32 and am.is_contiguous() and lm.is_contiguous() and am.shape[1] == lm.shape[1]
+    ldv = am.shape[1]
+    dev = am.device
+    ws_bytes = _ws_query(lib.pk_rnnt_simple_smooth_stats_workspace, "pk_rnnt_simple_smooth_stats_workspace", B, U1, ldv)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    Nl = torch.empty(B * U1, dtype=torch.float32, device=dev)
+    logq = torch.empty(ldv, dtype=torch.float32, device=dev)
+    Na = torch.empty(B * T, dtype=torch.float32, device=dev)
+    check(lib.pk_rnnt_simple_smooth_stats(_P(am), _P(lm), ldv, V, _P(am_max), _P(lm_max), _P(frame_lens), _P(label_lens), B, T, U1, _P(Nl),
+                                          _P(logq), _P(Na), _P(ws), ws_bytes, _stream()), "pk_rnnt_simple_smooth_stats")
+    return Nl, logq, Na
+
+
+def rnnt_simple_tables_smooth(am, lm, am_max, lm_max, S, labels, frame_lens, label_lens, B, T, U1, Nl, logq, Na, lm_only_scale,
+                              am_only_scale):
+    """-> (lpb_skew, lpl_skew) [B, T+U1-1, U1] f32 of the simple joiner smoothed with the LM-only / AM-only terms"""
+    dev = am.device
+    lpb = torch.empty(B, T + U1 - 1, U1, dtype=torch.float32, device=dev)
+    lpl = torch.empty_like(lpb)
+    check(lib.pk_rnnt_simple_tables_smooth(_P(am), _P(lm), am.stride(0), _P(am_max), _P(lm_max), _P(S), S.shape[-1], _P(labels),
+                                           max(labels.stride(0), 1), _P(frame_lens), _P(label_lens), B, T, U1, _P(Nl), _P(logq), _P(Na),
+                                           float(lm_only_scale), float(am_only_scale), _P(lpb), _P(lpl), _stream()),
+          "pk_rnnt_simple_tables_smooth")
+    return lpb, lpl
+
+
+def rnnt_simple_grad_smooth(src, V, rmax, G, n_g, axis, gb, gl, labels, frame_lens, label_lens, scale, logq, lse, lm_only_scale,
+                            am_only_scale, out):
+    """rnnt_simple_grad of the smoothed simple loss (G formed with the scale mu * scale, lse = Na on axis 0, Nl on axis 1)"""
+    B, T, U1 = gb.shape
+    assert out.is_contiguous() and out.shape[-1] == src.stride(0) and G.stride(-1) == 1
+    check(lib.pk_rnnt_simple_grad_smooth(_P(src), src.stride(0), V, _P(rmax), _P(G), G.shape[-1], n_g, axis, _P(gb), _P(gl), _P(labels),
+                                         max(labels.stride(0), 1), _P(frame_lens), _P(label_lens), _P(scale), _P(logq), _P(lse),
+                                         float(lm_only_scale), float(am_only_scale), B, T, U1, _P(out), _dt(out), _stream()),
+          "pk_rnnt_simple_grad_smooth")
+
+
 def rnnt_prune_bounds(ga, gb, frame_lens, label_lens, R):
     """occupancy -(ga + gb) [B,T,U1] (gb may be None) -> bounds [B,T] int32"""
     B, T, U1 = ga.shape

@@ -34,6 +34,11 @@ def prune_loss_scales(args, i):
     return 1.0 - (1.0 - ss) * f, 0.1 + 0.9 * f
 
 
+def smoothing_scales(args):
+    """the simple loss's smoothing keywords of engine.transducer_loss_pruned from --lm_only_scale / --am_only_scale (not ramped)"""
+    return dict(lm_only_scale=float(getattr(args, "lm_only_scale", 0.0)), am_only_scale=float(getattr(args, "am_only_scale", 0.0)))
+
+
 class TrainStep:
     def __init__(self, model, args, frontend, bmuf, optimizer, offset=None, scale=None, spec_augmentor=None):
         self.model, self.args, self.frontend, self.bmuf, self.opt = model, args, frontend, bmuf, optimizer
@@ -65,7 +70,7 @@ class TrainStep:
         if getattr(a, "prune_range", 0) > 0:
             ss, ps = prune_loss_scales(a, a.epoch * a.num_batches_per_epoch + self.num_done)
             simple, costs = engine.transducer_loss_pruned(self.model, feats, batch["target"], len_batch, batch["ali_lens"], a.prune_range,
-                                                          ss, ps, x_len=len_batch, t_out=t_out)
+                                                          ss, ps, x_len=len_batch, t_out=t_out, **smoothing_scales(a))
             self.simple_costs = simple
             loss = (simple * ss + costs * ps).sum()                       # upstream gradients: exactly the scales passed above
         else:

@@ -61,12 +61,13 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
             else:
                 with torch.no_grad():
                     feats = step.features(batch)
-                    from .step import encoder_out_lens, encoder_out_max
+                    from .step import encoder_out_lens, encoder_out_max, smoothing_scales
                     tl = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
                     t_out = encoder_out_max(int(batch["t_max"]), args.model_lctx, args.model_rctx, args.model_stride)
                     if pruned:
                         simple, costs = engine.transducer_loss_pruned(model, feats, batch["target"], tl, batch["ali_lens"],
-                                                                      args.prune_range, args.simple_loss_scale, 1.0, x_len=tl, t_out=t_out)
+                                                                      args.prune_range, args.simple_loss_scale, 1.0, x_len=tl, t_out=t_out,
+                                                                      **smoothing_scales(args))
                     else:
                         costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
             loss = float(costs.sum().item())
@@ -151,7 +152,24 @@ def build_parser():
     parser.add_argument('--prune_warmup_batches', type=int, default=0,
                         help='ramp the pruned loss weight from 0.1 to 1 and the simple loss weight from 1 to --simple_loss_scale '
                              'linearly over this many batches; 0 = off')
+    parser.add_argument('--lm_only_scale', type=float, default=0.0,
+                        help='pruned RNN-T (needs --prune_range): weight of the LM-only log-probs mixed into the simple joiner\'s lattice '
+                             '(DESIGN.md "Pruned RNN-T"); >= 0, and with --am_only_scale < 1; not ramped by --prune_warmup_batches')
+    parser.add_argument('--am_only_scale', type=float, default=0.0,
+                        help='pruned RNN-T (needs --prune_range): weight of the AM-only log-probs (against the batch\'s label unigram) '
+                             'mixed into the simple joiner\'s lattice; >= 0, and with --lm_only_scale < 1')
     return parser
+
+
+def check_smoothing_args(parser, args):
+    """parser.error unless --lm_only_scale / --am_only_scale are both 0, or in range with --prune_range > 0"""
+    lam_l, lam_a = args.lm_only_scale, args.am_only_scale
+    if lam_l == 0.0 and lam_a == 0.0:
+        return
+    if args.prune_range <= 0:
+        parser.error('--lm_only_scale / --am_only_scale smooth the simple loss of the pruned RNN-T loss: they need --prune_range > 0')
+    if not (lam_l >= 0.0 and lam_a >= 0.0 and lam_l + lam_a < 1.0):
+        parser.error('--lm_only_scale and --am_only_scale must be >= 0 with a sum < 1 (got %r, %r)' % (lam_l, lam_a))
 
 
 def main(argv=None):
@@ -160,6 +178,7 @@ def main(argv=None):
     loader_module = importlib.import_module('pika_b200.loader.' + args.loader + '_loader')
     loader_module.register(parser)
     args = parser.parse_args(argv)
+    check_smoothing_args(parser, args)
     args.input_dim = loader_module.get_inputdim(args)
     args.dataloader = loader_module.dataloader
     args.raw_batches = True

@@ -108,6 +108,8 @@ def main(argv=None):
     args = parser.parse_args(argv)
     if args.block_sync != 'bmuf':        # inherited from the RNN-T parser; the MBR trainer runs BmufTrainer only, as the reference's
         parser.error('--block_sync %s: the MBR trainer supports only bmuf' % args.block_sync)
+    if args.lm_only_scale != 0.0 or args.am_only_scale != 0.0:    # inherited from the RNN-T parser; there is no simple loss here
+        parser.error('--lm_only_scale / --am_only_scale: the MBR trainer has no simple loss to smooth')
     if args.lm:
         raise NotImplementedError("pika_b200: --lm (neural LM fusion) is outside the hot path")
     args.input_dim = loader_module.get_inputdim(args)

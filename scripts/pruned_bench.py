@@ -1,12 +1,13 @@
 """Train step with the dense joint against the pruned RNN-T loss (--prune_range R), at the bench's config-2 shape.
 
-    python scripts/pruned_bench.py [--steps 10] [--ranges 4,5,8] [--big-batch 96]
+    python scripts/pruned_bench.py [--steps 10] [--ranges 4,5,8] [--big-batch 96] [--smooth 0.25,0.0 [--smooth-range 5]]
 
 Runs bench.py's training step (B = 32, T = 1000 fbank frames -> T' = 240, U = 150, V = 6000, bf16, SpecAugment on) with the dense
 joint and with the pruned loss at every R, alternating the arms for --rounds rounds in one process.  Prints one JSON line per arm:
 ms per step (CUDA events around --steps steps after warm-up), the in-step durations of the fc2 forward, the loss, the simple loss and
 the bounds (engine._Tap events), and torch.cuda.max_memory_allocated; then the card's name and power limit.  --big-batch adds one
-batch size (default 96) run pruned only, with the dense arm tried first to show whether it fits.  Needs a GPU.
+batch size (default 96) run pruned only, with the dense arm tried first to show whether it fits.  --smooth LM,AM adds one more arm
+to every round: R = --smooth-range with the simple loss smoothed by --lm_only_scale LM and --am_only_scale AM.  Needs a GPU.
 """
 import argparse
 import json
@@ -41,9 +42,10 @@ def card():
 
 
 class Arm:
-    def __init__(self, B, T, U, V, prune_range, dev):
+    def __init__(self, B, T, U, V, prune_range, dev, smooth=(0.0, 0.0)):
         ta = bench.train_args()
         ta.prune_range, ta.simple_loss_scale, ta.prune_warmup_batches = prune_range, 0.5, 0
+        ta.lm_only_scale, ta.am_only_scale = smooth
         torch.manual_seed(777)
         margs = bench.model_args(V)
         margs.prune_range = prune_range
@@ -83,17 +85,17 @@ class Arm:
         return ms, taps
 
 
-def measure(B, R, steps, args, dev):
+def measure(B, R, steps, args, dev, smooth=(0.0, 0.0)):
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats()
+    tag = dict(batch=B, prune_range=R, **(dict(lm_only_scale=smooth[0], am_only_scale=smooth[1]) if any(smooth) else {}))
     try:
-        arm = Arm(B, args.T, args.U, args.V, R, dev)
+        arm = Arm(B, args.T, args.U, args.V, R, dev, smooth)
         ms, taps = arm.run(steps)
-        res = dict(batch=B, prune_range=R, ms_per_step=round(ms, 3), taps_ms=taps,
-                   max_memory_allocated_gb=round(torch.cuda.max_memory_allocated() / 1e9, 2))
+        res = dict(tag, ms_per_step=round(ms, 3), taps_ms=taps, max_memory_allocated_gb=round(torch.cuda.max_memory_allocated() / 1e9, 2))
         del arm
     except torch.cuda.OutOfMemoryError as e:
-        res = dict(batch=B, prune_range=R, error="out of memory: %s" % str(e).split("\n")[0][:160])
+        res = dict(tag, error="out of memory: %s" % str(e).split("\n")[0][:160])
     torch.cuda.empty_cache()
     return res
 
@@ -108,17 +110,21 @@ def main():
     ap.add_argument("--T", type=int, default=1000)
     ap.add_argument("--U", type=int, default=150)
     ap.add_argument("--V", type=int, default=6000)
+    ap.add_argument("--smooth", default="", help="LM,AM: add an arm with the simple loss smoothed by these scales")
+    ap.add_argument("--smooth-range", type=int, default=5)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("pruned_bench.py needs a GPU")
     dev = torch.device("cuda", 0)
     engine.set_precision("bf16")
     engine.set_seed(777)
-    arms = [0] + [int(r) for r in args.ranges.split(",")]
+    arms = [(0, (0.0, 0.0))] + [(int(r), (0.0, 0.0)) for r in args.ranges.split(",")]
+    if args.smooth:
+        arms.append((args.smooth_range, tuple(float(v) for v in args.smooth.split(","))))
     t0 = time.time()
     for rnd in range(args.rounds):
-        for R in arms:
-            print(json.dumps(dict(round=rnd, **measure(args.batch, R, args.steps, args, dev))), flush=True)
+        for R, smooth in arms:
+            print(json.dumps(dict(round=rnd, **measure(args.batch, R, args.steps, args, dev, smooth))), flush=True)
     if args.big_batch:
         for R in (0, 5):
             print(json.dumps(dict(round="big", **measure(args.big_batch, R, max(args.steps // 2, 3), args, dev))), flush=True)
