@@ -229,6 +229,34 @@ int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const 
                         void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * RNN-T forced alignment (pika_b200/csrc/rnnt_loss.cu; DESIGN.md "Forced alignment").  Tables in the layout of pk_rnnt_lattice.
+ * pk_rnnt_tables: the dense loss's first pass alone: logits [B, T, U1, ldv] (as pk_rnnt_loss_fwd_bwd) -> lse [B*T*U1] f32 (the row
+ *   log-sum-exp), lpb_skew, lpl_skew.  row_lse: NULL (the logits are streamed) or the producing GEMM's [n_parts][B*T*U1][2] partials.
+ *   Nodes t >= T_b or u > U_b are not written.  No gradient buffer is touched.
+ * pk_rnnt_pruned_tables: pk_rnnt_pruned_loss's tables alone: logits [B*T*R, ldv] + bounds -> lse [B*T*R], lpb_skew / lpl_skew with -inf
+ *   outside each frame's window of R label positions.
+ * pk_rnnt_lattice_costs: pk_rnnt_lattice without gb / gl: costs [B] = -log P(y | x) only (same workspace).
+ * pk_rnnt_viterbi: best path through the lattice, f64 max-plus: delta(0,0) = 0, delta(t,u) = max(delta(t-1,u) + lpb(t-1,u),
+ *   delta(t,u-1) + lpl(t,u-1)); the label arc is taken only when strictly greater (ties and -inf on both arcs: blank).
+ *   score [B] f32 = delta(T_b-1, U_b) + lpb(T_b-1, U_b), -inf when no path has a finite score (or T_b = 0).
+ *   emit_frames [B][ld_emit] int32 (ld_emit >= U1 - 1): entry u-1 = the frame t of the best path's label arc (t, u-1) -> (t, u) for
+ *   u = 1 .. U_b, non-decreasing in u; -1 from U_b on, and everywhere when score is -inf.
+ *   workspace >= the size pk_rnnt_viterbi_workspace writes to *bytes; on return it holds the decisions: u32 words
+ *   [B][T+U1-1][ceil(U1/32)], bit u % 32 of word (b, t+u, u / 32) = 1 when node (t, u) of a valid utterance came in by its label arc
+ *   (words whose first u is past U_b are not written).  U1 <= 2048; one CTA per utterance, no atomics: deterministic. */
+int pk_rnnt_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, int B, int T, int U1,
+                   int V, int ldv, int ld_labels, const float* row_lse, int n_parts, float* lse, float* lpb_skew, float* lpl_skew,
+                   void* stream);
+int pk_rnnt_pruned_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                          const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* row_lse, int n_parts,
+                          float* lse, float* lpb_skew, float* lpl_skew, void* stream);
+int pk_rnnt_lattice_costs(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew, const float* lpl_skew,
+                          float* costs, void* workspace, long long workspace_bytes, void* stream);
+int pk_rnnt_viterbi_workspace(int B, int T, int U1, long long* bytes);
+int pk_rnnt_viterbi(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew, const float* lpl_skew,
+                    float* score, int* emit_frames, int ld_emit, void* workspace, long long workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Memory-bound layers around the GEMMs (pika_b200/csrc/elementwise.cu).  `dtype` is the
  * activation type (PK_BF16 production, PK_F32 fp32-class parity mode); statistics are f32.
  */

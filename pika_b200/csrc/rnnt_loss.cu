@@ -318,6 +318,7 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
         costs[b] = 0.f;
     }
     __syncthreads();
+    if (gb_out == nullptr) return;             // costs only (pk_rnnt_lattice_costs)
     // ---------------- per-node gradient coefficients (natural [b,t,u] layout); zero for padded nodes
     const float gs = grad_scale ? grad_scale[b] : 1.f;
     const lat_t ll = valid ? s_ll : 0.0;
@@ -338,6 +339,122 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
         }
         gb_out[(size_t)b * nodes + i] = gb;
         gl_out[(size_t)b * nodes + i] = gl;
+    }
+}
+
+// ------------------------------------------------------------------------------------ forced alignment (pk_rnnt_viterbi)
+// The max-plus form of the alpha sweep above, same launch shape (one CTA per utterance, thread j owning u = j, j+G, ..., the previous
+// diagonal ping-ponged in shared memory, the next diagonal's log-probs prefetched before the barrier), in f64:
+//   delta(0,0) = 0,  delta(t,u) = max(delta(t-1,u) + lpb(t-1,u), delta(t,u-1) + lpl(t,u-1)),
+//   score = delta(T-1,U) + lpb(T-1,U).
+// The label arc is taken only when it is strictly greater (ties and -inf on both arcs go to blank).  Each node's choice is one bit,
+// packed 32 label positions per word by __ballot_sync into dec [B][T+U1-1][ceil(U1/32)] (words whose first u is past U are not
+// written).  Then warp 0 walks the bits back from (T-1, U) and writes emit[b][u-1] = t for every label arc: lane k loads the words of
+// diagonal dg-k that can hold the path (u-k .. u spans at most two words), so one round of loads serves 32 steps of the walk.
+__global__ void __launch_bounds__(LAT_MAX_G) rnnt_viterbi_kernel(const int* __restrict__ frame_lens, const int* __restrict__ label_lens,
+                                                               RnntDims d, int G, int cpt, const float* __restrict__ lpb_skew,
+                                                               const float* __restrict__ lpl_skew, unsigned* __restrict__ dec,
+                                                               float* __restrict__ score, int* __restrict__ emit, int ld_emit) {
+    extern __shared__ lat_t sm[];            // 2 diagonals x (U1 + 2)
+    __shared__ lat_t s_score;
+    const int b = blockIdx.x;
+    const int j = threadIdx.x;
+    const int T = frame_lens[b], U = label_lens[b];
+    const int NW = (d.U1 + 31) / 32;
+    const size_t base = (size_t)b * d.ND * d.U1;
+    unsigned* db = dec + (size_t)b * d.ND * NW;
+    int* eb = emit + (size_t)b * ld_emit;
+    const bool valid = (T > 0 && T <= d.T && U >= 0 && U < d.U1);
+    if (!valid) {                            // no lattice: no path
+        for (int i = j; i < ld_emit; i += G) eb[i] = -1;
+        if (j == 0) score[b] = -INFINITY;
+        return;
+    }
+    const int W = d.U1 + 2;
+    lat_t* prev = sm + 1;                    // index -1 .. U1 valid
+    lat_t* cur = prev + W;
+    for (int i = j - 1; i <= d.U1; i += G) { prev[i] = LAT_NEG_INF; cur[i] = LAT_NEG_INF; }
+    __syncthreads();
+    const int last = T - 1 + U;
+    if (j == 0) cur[0] = 0.0;
+    for (int w = j; w <= U / 32; w += G) db[w] = 0u;   // diagonal 0: node (0, 0) has no incoming arc
+    float nb[LAT_MAX_CPT], nl[LAT_MAX_CPT];
+#pragma unroll
+    for (int c = 0; c < LAT_MAX_CPT; ++c) {
+        const int u = j + c * G;
+        nb[c] = (c < cpt && u <= U && last >= 1) ? lpb_skew[base + u] : 0.f;
+        nl[c] = (c < cpt && u >= 1 && u <= U && last >= 1) ? lpl_skew[base + u - 1] : 0.f;
+    }
+    __syncthreads();
+    for (int dg = 1; dg <= last; ++dg) {
+        lat_t* tsw = prev; prev = cur; cur = tsw;
+        const int lo = max(0, dg - (T - 1)), hi = min(U, dg);
+        float pb[LAT_MAX_CPT], pl[LAT_MAX_CPT];
+#pragma unroll
+        for (int c = 0; c < LAT_MAX_CPT; ++c) { pb[c] = nb[c]; pl[c] = nl[c]; }
+        if (dg < last) {
+            const size_t nbase = base + (size_t)dg * d.U1;
+#pragma unroll
+            for (int c = 0; c < LAT_MAX_CPT; ++c) {
+                const int u = j + c * G;
+                if (c < cpt && u <= U) {
+                    nb[c] = lpb_skew[nbase + u];
+                    nl[c] = (u >= 1) ? lpl_skew[nbase + u - 1] : 0.f;
+                }
+            }
+        }
+        unsigned* drow = db + (size_t)dg * NW;
+#pragma unroll
+        for (int c = 0; c < LAT_MAX_CPT; ++c) {
+            if (c < cpt) {                                         // block-uniform: every lane reaches the ballot
+                const int u = j + c * G;
+                bool lab = false;
+                if (u >= lo && u <= hi) {
+                    const lat_t a = (u <= dg - 1) ? prev[u] + pb[c] : LAT_NEG_INF;    // from (t-1, u) via blank
+                    const lat_t l = (u >= 1) ? prev[u - 1] + pl[c] : LAT_NEG_INF;     // from (t, u-1) via label u
+                    lab = l > a;
+                    cur[u] = lab ? l : a;
+                }
+                const unsigned bits = __ballot_sync(0xffffffffu, lab);
+                const int u0 = c * G + (j & ~31);                  // G is a multiple of 32: the warp's 32 u are one word
+                if ((j & 31) == 0 && u0 <= U) drow[u0 >> 5] = bits;
+            }
+        }
+        __syncthreads();
+    }
+    if (j == 0) {
+        const lat_t s = cur[U] + (lat_t)lpb_skew[base + (size_t)last * d.U1 + U];
+        s_score = s;
+        score[b] = (float)s;
+    }
+    __syncthreads();                         // also publishes every warp's decision words to warp 0
+    if (j >= 32) return;
+    const int lane = j;
+    const bool found = s_score != LAT_NEG_INF;
+    for (int i = (found ? U : 0) + lane; i < ld_emit; i += 32) eb[i] = -1;
+    if (!found) return;
+    int t = T - 1, u = U;
+    while (t + u > 0) {
+        const int dg = t + u;
+        const int steps = min(32, dg);                              // diagonals dg .. dg-steps+1; the walk stops at diagonal 0
+        unsigned whi = 0u, wlo = 0u;
+        if (lane < steps) {
+            const unsigned* row = db + (size_t)(dg - lane) * NW;
+            whi = row[u >> 5];
+            wlo = row[max(u - lane, 0) >> 5];
+        }
+        const int uw = u >> 5;
+        for (int s = 0; s < steps; ++s) {                           // the node (t, u) lies on diagonal dg - s
+            const unsigned wh = __shfl_sync(0xffffffffu, whi, s);
+            const unsigned wl = __shfl_sync(0xffffffffu, wlo, s);
+            const unsigned word = (u >> 5) == uw ? wh : wl;
+            if ((word >> (u & 31)) & 1u) {
+                if (lane == 0) eb[u - 1] = t;
+                --u;
+            } else {
+                --t;
+            }
+        }
     }
 }
 
@@ -756,6 +873,35 @@ static int launch_lattice(const int* frame_lens, const int* label_lens, const pk
     return 0;
 }
 
+// pass 1: lse [nodes] and the skewed tables, merged from the producing GEMM's row partials (row_lse) or streamed from the logits
+static int launch_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                         const pk::RnntDims& d, const float* row_lse, int n_parts, float* lse, float* lpb, float* lpl, cudaStream_t stream) {
+    using namespace pk;
+    const long long rows = (long long)d.B * d.T * d.U1;
+    const int warps_per_cta = 8;
+    long long want = (rows + warps_per_cta - 1) / warps_per_cta;
+    const long long cap = (long long)num_sms() * 8 * 4;      // persistent grid-stride: 8 CTAs/SM x 4 waves
+    const int grid = (int)(want < cap ? want : cap);
+    if (row_lse != nullptr) {
+        PK_CHECK_ARG(n_parts >= 1, "n_parts must be >= 1");
+        const int fgrid = (int)((rows + 255) / 256 < (long long)num_sms() * 8 ? (rows + 255) / 256 : (long long)num_sms() * 8);
+        if (dtype == PK_BF16)
+            rnnt_rowfinish_kernel<__nv_bfloat16><<<fgrid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(logits), labels, frame_lens,
+                                                                           label_lens, d, reinterpret_cast<const float2*>(row_lse), n_parts,
+                                                                           lse, lpb, lpl);
+        else
+            rnnt_rowfinish_kernel<float><<<fgrid, 256, 0, stream>>>(reinterpret_cast<const float*>(logits), labels, frame_lens, label_lens, d,
+                                                                   reinterpret_cast<const float2*>(row_lse), n_parts, lse, lpb, lpl);
+    } else if (dtype == PK_BF16)
+        rnnt_rowstats_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(logits), labels,
+                                                                     frame_lens, label_lens, d, lse, lpb, lpl);
+    else
+        rnnt_rowstats_kernel<float><<<grid, 256, 0, stream>>>(reinterpret_cast<const float*>(logits), labels, frame_lens,
+                                                              label_lens, d, lse, lpb, lpl);
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
 static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, const int* frame_lens,
                           const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                           const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
@@ -778,27 +924,10 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
     float* lse = lpl + skew; float* gb = lse + nodes; float* gl = gb + nodes;
 
     const long long rows = (long long)nodes;
-    const int warps_per_cta = 8;
-    long long want = (rows + warps_per_cta - 1) / warps_per_cta;
-    const long long cap = (long long)num_sms() * 8 * 4;      // persistent grid-stride: 8 CTAs/SM x 4 waves
-    const int grid = (int)(want < cap ? want : cap);
-    if (row_lse != nullptr) {
-        PK_CHECK_ARG(n_parts >= 1, "n_parts must be >= 1");
-        const int fgrid = (int)((rows + 255) / 256 < (long long)num_sms() * 8 ? (rows + 255) / 256 : (long long)num_sms() * 8);
-        if (dtype == PK_BF16)
-            rnnt_rowfinish_kernel<__nv_bfloat16><<<fgrid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(logits), labels, frame_lens,
-                                                                           label_lens, d, reinterpret_cast<const float2*>(row_lse), n_parts,
-                                                                           lse, lpb, lpl);
-        else
-            rnnt_rowfinish_kernel<float><<<fgrid, 256, 0, stream>>>(reinterpret_cast<const float*>(logits), labels, frame_lens, label_lens, d,
-                                                                   reinterpret_cast<const float2*>(row_lse), n_parts, lse, lpb, lpl);
-    } else if (dtype == PK_BF16)
-        rnnt_rowstats_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(logits), labels,
-                                                                     frame_lens, label_lens, d, lse, lpb, lpl);
-    else
-        rnnt_rowstats_kernel<float><<<grid, 256, 0, stream>>>(reinterpret_cast<const float*>(logits), labels, frame_lens,
-                                                              label_lens, d, lse, lpb, lpl);
-    PK_CHECK_LAUNCH(); count_launch();
+    {
+        const int rc = launch_tables(logits, dtype, labels, frame_lens, label_lens, d, row_lse, n_parts, lse, lpb, lpl, stream);
+        if (rc) return rc;
+    }
     {
         const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
         if (rc) return rc;
@@ -915,6 +1044,32 @@ extern "C" int pk_rnnt_pruned_loss_workspace(int B, int T, int U1, int R, int ld
     return 0;
 }
 
+// the pruned loss's passes 1 and 2: the row log-sum-exp lse [B*T*R], then tables with -inf outside each frame's window
+static int launch_pruned_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                                 const int* bounds, const pk::RnntDims& d, int R, const float* row_lse, int n_parts, float* lse, float* lpb,
+                                 float* lpl, cudaStream_t stream) {
+    using namespace pk;
+    const long long rows = (long long)d.B * d.T * R;
+    const int wgrid = (int)std::min<long long>((rows + 7) / 8, (long long)num_sms() * 32);
+    const long long nn = (long long)d.B * d.T * d.U1;
+    const int ngrid = (int)std::min<long long>((nn + 255) / 256, (long long)num_sms() * 8);
+    if (dtype == PK_BF16) {
+        using TT = __nv_bfloat16;
+        pruned_row_lse_kernel<TT><<<wgrid, 256, 0, stream>>>((const TT*)logits, frame_lens, label_lens, bounds, d.T, R, d.V, d.ldv, rows,
+                                                            (const float2*)row_lse, n_parts, lse);
+        PK_CHECK_LAUNCH(); count_launch();
+        pruned_tables_kernel<TT><<<ngrid, 256, 0, stream>>>((const TT*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb, lpl);
+    } else {
+        pruned_row_lse_kernel<float><<<wgrid, 256, 0, stream>>>((const float*)logits, frame_lens, label_lens, bounds, d.T, R, d.V, d.ldv,
+                                                               rows, (const float2*)row_lse, n_parts, lse);
+        PK_CHECK_LAUNCH(); count_launch();
+        pruned_tables_kernel<float><<<ngrid, 256, 0, stream>>>((const float*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb,
+                                                               lpl);
+    }
+    PK_CHECK_LAUNCH(); count_launch();
+    return 0;
+}
+
 extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
                                    const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
                                    float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
@@ -938,22 +1093,11 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
     float* gb = lpl + skew; float* gl = gb + nodes;
     float* lse = gl + nodes; float* gb_row = lse + rows; float* gl_row = gb_row + rows;
     int* y_row = reinterpret_cast<int*>(gl_row + rows);
-    const int wgrid = (int)std::min<long long>((rows + 7) / 8, (long long)num_sms() * 32);
-    const long long nn = (long long)B * T * U1;
-    const int ngrid = (int)std::min<long long>((nn + 255) / 256, (long long)num_sms() * 8);
-    if (dtype == PK_BF16) {
-        using TT = __nv_bfloat16;
-        pruned_row_lse_kernel<TT><<<wgrid, 256, 0, stream>>>((const TT*)logits, frame_lens, label_lens, bounds, T, R, V, ldv, rows,
-                                                            (const float2*)row_lse, n_parts, lse);
-        PK_CHECK_LAUNCH(); count_launch();
-        pruned_tables_kernel<TT><<<ngrid, 256, 0, stream>>>((const TT*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb, lpl);
-    } else {
-        pruned_row_lse_kernel<float><<<wgrid, 256, 0, stream>>>((const float*)logits, frame_lens, label_lens, bounds, T, R, V, ldv, rows,
-                                                               (const float2*)row_lse, n_parts, lse);
-        PK_CHECK_LAUNCH(); count_launch();
-        pruned_tables_kernel<float><<<ngrid, 256, 0, stream>>>((const float*)logits, labels, frame_lens, label_lens, bounds, d, R, lse, lpb, lpl);
+    {
+        const int rc = launch_pruned_tables(logits, dtype, labels, frame_lens, label_lens, bounds, d, R, row_lse, n_parts, lse, lpb, lpl,
+                                            stream);
+        if (rc) return rc;
     }
-    PK_CHECK_LAUNCH(); count_launch();
     {
         const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
         if (rc) return rc;
@@ -981,5 +1125,80 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
         colsum_partials_kernel<<<(ldv + 31) / 32, 256, 0, stream>>>(cs_part, ggrid, ldv, dlogits_colsum);
         PK_CHECK_LAUNCH(); count_launch();
     }
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------ forced alignment entry points
+static int check_logits_args(const void* logits, int dtype, int B, int T, int U1, int V, int ldv) {
+    PK_CHECK_ARG(dtype == PK_F32 || dtype == PK_BF16, "bad dtype");
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && V > 1, "bad dims");
+    const int vn = dtype == PK_F32 ? 4 : 8;
+    PK_CHECK_ARG(ldv >= V && ldv % vn == 0, "ldv must be >= V and a multiple of 16 bytes");
+    PK_CHECK_ARG((reinterpret_cast<uintptr_t>(logits) & 15) == 0, "logits not 16B aligned");
+    return 0;
+}
+
+extern "C" int pk_rnnt_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, int B, int T,
+                              int U1, int V, int ldv, int ld_labels, const float* row_lse, int n_parts, float* lse, float* lpb_skew,
+                              float* lpl_skew, void* stream) {
+    const int rc = check_logits_args(logits, dtype, B, T, U1, V, ldv);
+    if (rc) return rc;
+    PK_CHECK_ARG(lse && lpb_skew && lpl_skew, "null pointer");
+    pk::RnntDims d{B, T, U1, V, ldv, ld_labels, T + U1 - 1};
+    return launch_tables(logits, dtype, labels, frame_lens, label_lens, d, row_lse, n_parts, lse, lpb_skew, lpl_skew,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pk_rnnt_pruned_tables(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                                     const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* row_lse,
+                                     int n_parts, float* lse, float* lpb_skew, float* lpl_skew, void* stream) {
+    const int rc = check_logits_args(logits, dtype, B, T, U1, V, ldv);
+    if (rc) return rc;
+    PK_CHECK_ARG(R >= 1, "R must be >= 1");
+    PK_CHECK_ARG(row_lse == nullptr || n_parts >= 1, "n_parts must be >= 1");
+    PK_CHECK_ARG(bounds && lse && lpb_skew && lpl_skew, "null pointer");
+    pk::RnntDims d{B, T, U1, V, ldv, ld_labels, T + U1 - 1};
+    return launch_pruned_tables(logits, dtype, labels, frame_lens, label_lens, bounds, d, R, row_lse, n_parts, lse, lpb_skew, lpl_skew,
+                                reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pk_rnnt_lattice_costs(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
+                                     const float* lpl_skew, float* costs, void* workspace, long long workspace_bytes, void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0, "bad dims");
+    PK_CHECK_ARG(lpb_skew && lpl_skew && costs && workspace, "null pointer");
+    PK_CHECK_ARG(workspace_bytes >= lattice_ws_bytes(B, T, U1), "workspace too small");
+    RnntDims d{B, T, U1, 2, 2, 1, T + U1 - 1};
+    const size_t skew = (size_t)B * d.ND * U1;
+    double* alpha = reinterpret_cast<double*>(workspace);
+    return launch_lattice(frame_lens, label_lens, d, lpb_skew, lpl_skew, alpha, alpha + skew, nullptr, costs, nullptr, nullptr,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+static long long viterbi_ws_bytes(int B, int T, int U1) { return (long long)B * ((long long)T + U1 - 1) * ((U1 + 31) / 32) * 4; }
+extern "C" int pk_rnnt_viterbi_workspace(int B, int T, int U1, long long* bytes) {
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && bytes != nullptr, "bad dims or null pointer");
+    *bytes = viterbi_ws_bytes(B, T, U1);
+    return 0;
+}
+
+extern "C" int pk_rnnt_viterbi(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
+                               const float* lpl_skew, float* score, int* emit_frames, int ld_emit, void* workspace, long long workspace_bytes,
+                               void* stream) {
+    using namespace pk;
+    PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && ld_emit >= 0, "bad dims");
+    PK_CHECK_ARG(lpb_skew && lpl_skew && score && workspace && (emit_frames || ld_emit == 0), "null pointer");
+    PK_CHECK_ARG(ld_emit >= U1 - 1, "ld_emit must be >= U1 - 1");
+    PK_CHECK_ARG(workspace_bytes >= viterbi_ws_bytes(B, T, U1), "workspace too small");
+    int G = ((U1 + 31) / 32) * 32;
+    if (G > LAT_MAX_G) G = LAT_MAX_G;
+    const int cpt = (U1 + G - 1) / G;
+    PK_CHECK_ARG(cpt <= LAT_MAX_CPT, "U too large for the Viterbi kernel (U+1 <= 2048)");
+    RnntDims d{B, T, U1, 2, 2, 1, T + U1 - 1};
+    const int smem = 2 * (U1 + 2) * (int)sizeof(lat_t);           // <= 32.8 KB: no opt-in needed
+    rnnt_viterbi_kernel<<<B, G, smem, reinterpret_cast<cudaStream_t>(stream)>>>(frame_lens, label_lens, d, G, cpt, lpb_skew, lpl_skew,
+                                                                                reinterpret_cast<unsigned*>(workspace), score, emit_frames,
+                                                                                ld_emit);
+    PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }

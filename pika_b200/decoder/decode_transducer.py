@@ -63,6 +63,46 @@ def build_parser():
     return p
 
 
+def load_cmvn(args, dev):
+    """--cmvn_stats -> args.offset / args.scale [D * (lctx + 1 + rctx)] on ``dev`` (decoder/decode_transducer.py:54-71)"""
+    if args.cmvn_stats:
+        cmvn = read_kaldi_text_matrix(args.cmvn_stats)
+        mean = cmvn[0][:-1] / cmvn[0][-1]
+        var = cmvn[1][:-1] / cmvn[0][-1] - mean * mean
+        if min(abs(var)) < 1.0e-20:
+            sys.exit('problematic cmvn_stats, variance too small')
+        rep = args.lctx + args.rctx + 1
+        args.offset = torch.from_numpy(-mean).to(dev).repeat(rep)
+        args.scale = torch.from_numpy(1.0 / np.sqrt(var)).to(dev).repeat(rep)
+
+
+def read_symbols_map(path):
+    """``symbol id`` lines -> {id: symbol} (:103-107)"""
+    sym_map = {}
+    with open(path, 'r', encoding='utf-8') as f:
+        for line in f:
+            entry = line.split(" ")
+            sym_map[int(entry[1])] = entry[0]
+    return sym_map
+
+
+def prepare_batch(data_batch, len_batch, args, dev):
+    """a loader batch -> (features, encoder output lengths): --min_len padding, --cmn / --cmvn_stats, then the model's context and
+    stride (:116-134)"""
+    len_batch = torch.from_numpy(len_batch).to(dev)
+    if int(len_batch.max()) < args.min_len:                                                 # :116-122
+        pad = data_batch[:, -1, :].unsqueeze(1).expand(-1, args.min_len - int(len_batch.max()), -1)
+        data_batch = torch.cat((data_batch, pad), dim=1)
+        len_batch[:] = args.min_len
+    if args.cmvn_stats:                                                                     # :123-129
+        if args.cmn:
+            data_batch = data_batch - data_batch.mean(dim=1, keepdim=True)
+        data_batch = (data_batch + args.offset.to(data_batch.dtype)) * args.scale.to(data_batch.dtype)
+    len_batch = len_batch - args.model_lctx - args.model_rctx                               # :131-134
+    len_batch = len_batch // args.model_stride + torch.ne(len_batch % args.model_stride, 0).int()
+    return data_batch, len_batch
+
+
 def main(argv=None):
     parser = build_parser()
     args, _ = parser.parse_known_args(argv)
@@ -85,15 +125,7 @@ def main(argv=None):
             net.eval().to(dev)
         setattr(args, name, net)
 
-    if args.cmvn_stats:                                                                     # :54-71
-        cmvn = read_kaldi_text_matrix(args.cmvn_stats)
-        mean = cmvn[0][:-1] / cmvn[0][-1]
-        var = cmvn[1][:-1] / cmvn[0][-1] - mean * mean
-        if min(abs(var)) < 1.0e-20:
-            sys.exit('problematic cmvn_stats, variance too small')
-        rep = args.lctx + args.rctx + 1
-        args.offset = torch.from_numpy(-mean).to(dev).repeat(rep)
-        args.scale = torch.from_numpy(1.0 / np.sqrt(var)).to(dev).repeat(rep)
+    load_cmvn(args, dev)
 
     lm_scorer = None
     if args.fst_lm != '':                                                                   # :82-88
@@ -104,25 +136,11 @@ def main(argv=None):
                                       global_scorer=GlobalScorer(), sm_scale=args.sm_scale, lm=None, lm_scale=args.lm_scale,
                                       lm_scorer=lm_scorer, lm_scorer_scale=args.fst_lm_scale, cuda=True, beam_prune=True, args=args)
 
-    sym_map = {}
-    with open(args.symbols_map, 'r', encoding='utf-8') as f:                                # :103-107
-        for line in f:
-            entry = line.split(" ")
-            sym_map[int(entry[1])] = entry[0]
+    sym_map = read_symbols_map(args.symbols_map)
 
     with open(args.output_file, 'w') as f:
         for data_batch, _, len_batch, _ in loader_module.dataloader(args.input_labels, args.input_specifier, False, args):
-            len_batch = torch.from_numpy(len_batch).to(dev)
-            if int(len_batch.max()) < args.min_len:                                         # :116-122
-                pad = data_batch[:, -1, :].unsqueeze(1).expand(-1, args.min_len - int(len_batch.max()), -1)
-                data_batch = torch.cat((data_batch, pad), dim=1)
-                len_batch[:] = args.min_len
-            if args.cmvn_stats:                                                             # :123-129
-                if args.cmn:
-                    data_batch = data_batch - data_batch.mean(dim=1, keepdim=True)
-                data_batch = (data_batch + args.offset.to(data_batch.dtype)) * args.scale.to(data_batch.dtype)
-            len_batch = len_batch - args.model_lctx - args.model_rctx                       # :131-134
-            len_batch = len_batch // args.model_stride + torch.ne(len_batch % args.model_stride, 0).int()
+            data_batch, len_batch = prepare_batch(data_batch, len_batch, args, dev)
             ret, enc_out = trans_decoder.decode_batch(data_batch.float(), len_batch, (len_batch + 100).tolist())
             hyps, scores = ret["predictions"], ret["scores"]
             for i in range(args.batch_size):                                                # :136-178

@@ -1318,6 +1318,37 @@ class SimpleLossFn(torch.autograd.Function):
         return d_enc, d_pred, None, None, None, None, None, None, None, None, None
 
 
+def _pruned_joint_forward(enc, pred, model, bounds, R):
+    """the pruned joint: row (b, t, r) is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd) and fc2 runs on the B*T*R
+    rows, with the row log-sum-exp epilogue in bf16 -> (logits [B*T*R, ldv] act dtype, row_lse or None, saved state)"""
+    B, T, H = enc.shape
+    U1 = pred.shape[1]
+    fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
+    V = fc2.weight.shape[0]
+    ldv = _ldv(V)
+    wx = stage_weight([fc1.weight, fcg.weight])
+    enc_parts = stage_act(enc.reshape(B * T, H))
+    pred_parts = stage_act(pred.reshape(B * U1, H))
+    ex = _new((B * T, 2 * H), like=enc)
+    py = _new((B * U1, 2 * H), like=enc)
+    gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=_cat_bias([fc1.bias, fcg.bias]))
+    gemm_parts([pred_parts], [[p[:, H:] for p in wx]], py)
+    rows = B * T * R
+    h = _new((rows, H), like=enc)
+    K.joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H)
+    w2 = stage_weight(fc2.weight)
+    logits = _new((rows, ldv), like=enc, zero=(ldv != V))
+    h_parts = stage_act(h)
+    del h
+    row_lse = None
+    if _FUSED_LSE and logits.dtype == torch.bfloat16 and V % 8 == 0:
+        row_lse = torch.empty(K.row_lse_parts(rows, V, 256), rows, 2, dtype=torch.float32, device=enc.device)
+    with _Tap("fc2_fwd"):
+        gemm_parts([h_parts], [w2], logits[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
+                   **({"block_n": 256} if row_lse is not None else {}))
+    return logits, row_lse, dict(ex=ex, py=py, h_parts=h_parts, enc_parts=enc_parts, pred_parts=pred_parts, wx=wx, w2=w2)
+
+
 class PrunedJointLossFn(torch.autograd.Function):
     """Pruned joint + RNN-T loss: row (b, t, r) of the joint is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd),
     fc2 runs on the B*T*R rows (with the row log-sum-exp epilogue in bf16), the loss and its gradient come from pk_rnnt_pruned_loss
@@ -1328,30 +1359,13 @@ class PrunedJointLossFn(torch.autograd.Function):
     def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, bounds, R, scale, need_grad):
         B, T, H = enc.shape
         U1 = pred.shape[1]
-        fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
+        fc2 = model.fc2
         V = fc2.weight.shape[0]
         ldv = _ldv(V)
         dev = enc.device
-        wx = stage_weight([fc1.weight, fcg.weight])
-        enc_parts = stage_act(enc.reshape(B * T, H))
-        pred_parts = stage_act(pred.reshape(B * U1, H))
-        ex = _new((B * T, 2 * H), like=enc)
-        py = _new((B * U1, 2 * H), like=enc)
-        gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=_cat_bias([fc1.bias, fcg.bias]))
-        gemm_parts([pred_parts], [[p[:, H:] for p in wx]], py)
         rows = B * T * R
-        h = _new((rows, H), like=enc)
-        K.joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H)
-        w2 = stage_weight(fc2.weight)
-        logits = _new((rows, ldv), like=enc, zero=(ldv != V))
-        h_parts = stage_act(h)
-        del h
-        row_lse = None
-        if _FUSED_LSE and logits.dtype == torch.bfloat16 and V % 8 == 0:
-            row_lse = torch.empty(K.row_lse_parts(rows, V, 256), rows, 2, dtype=torch.float32, device=dev)
-        with _Tap("fc2_fwd"):
-            gemm_parts([h_parts], [w2], logits[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
-                       **({"block_n": 256} if row_lse is not None else {}))
+        logits, row_lse, st = _pruned_joint_forward(enc, pred, model, bounds, R)
+        ex, py, h_parts, w2 = st["ex"], st["py"], st.pop("h_parts"), st["w2"]
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
         if not need_grad:
             return K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=row_lse)
@@ -1371,7 +1385,7 @@ class PrunedJointLossFn(torch.autograd.Function):
         dpy = _new((B * U1, 2 * H), like=enc)
         K.joint_gate_pruned_bwd(ex, py, bounds, dh, dex, dpy, B, T, U1, R, H)
         del dh
-        st = dict(enc_parts=enc_parts, pred_parts=pred_parts, wx=wx, dims=(B, T, U1, H, V, ldv))
+        st = dict(enc_parts=st["enc_parts"], pred_parts=st["pred_parts"], wx=st["wx"], dims=(B, T, U1, H, V, ldv))
         d_enc, d_pred = _gate_input_grads(dex, dpy, st, model, True, True)
         ctx.save_for_backward(d_enc, d_pred)
         return costs
@@ -1419,3 +1433,42 @@ def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, sim
     simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need, lam_l, lam_a)
     pruned_costs = PrunedJointLossFn.apply(enc, pred, model, labels, fl, ll, bounds, R, float(pruned_scale), need)
     return simple_costs, pruned_costs
+
+
+# ------------------------------------------------------------------------------------------------
+# forced alignment (DESIGN.md "Forced alignment")
+def transducer_align(model, x, y, frame_lens, label_lens, x_len=None, t_out=None, prune_range=0):
+    """Viterbi alignment of known transcripts -> (emit_frames [B, Umax] int32, viterbi [B] f32, loglik [B] f32), Umax = y.shape[1].
+    emit_frames[b, u] is the encoder frame on which the best path through the RNN-T lattice emits label u (-1 from label_lens[b] on, and
+    everywhere when no path has a finite score), viterbi[b] that path's log-probability (-inf when there is none) and loglik[b] =
+    log P(y | x) summed over every path.  Runs without gradients; ``x_len`` / ``t_out`` as in transducer_forward.
+    ``prune_range`` R >= 2: the lattice is the pruned loss's, with the simple joiner's windows of R label positions per frame (the model
+    needs simple_am_proj; an utterance with no path inside the windows raises ValueError before any work) and loglik the
+    log-likelihood over the windows.  0: the dense joint."""
+    R = int(prune_range)
+    if R != 0:
+        check_prune_feasible(frame_lens, label_lens, R)
+        if not hasattr(model, "simple_am_proj"):
+            raise ValueError("alignment with prune_range needs the simple joiner: build Net with prune_range > 0")
+    fl, ll = frame_lens.int().contiguous(), label_lens.int().contiguous()
+    labels = y.int().contiguous()
+    with torch.no_grad():
+        enc = model_encoder_forward_act(model, x, x_len, t_out)
+        pred = prednet_forward_act(model, y)
+        B, T, _ = enc.shape
+        U1 = pred.shape[1]
+        V = model.fc2.weight.shape[0]
+        if R:
+            _, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, 1.0, False)
+            logits, row_lse, st = _pruned_joint_forward(enc, pred, model, bounds, R)
+            lpb, lpl = K.rnnt_pruned_tables(logits, labels, fl, ll, bounds, U1, R, V, row_lse=row_lse)
+        else:
+            logits, st = _joint_forward(enc, pred, model, want_lse=True)
+            row_lse = st.pop("row_lse")
+            lpb, lpl = K.rnnt_tables(logits, labels, fl, ll, V=V, row_lse=row_lse)
+        del logits, row_lse, st
+        with _Tap("lattice"):
+            loglik = -K.rnnt_lattice_costs(lpb, lpl, fl, ll, B, T, U1)
+        with _Tap("viterbi"):
+            viterbi, frames = K.rnnt_viterbi(lpb, lpl, fl, ll, B, T, U1, ld_emit=y.shape[1])
+    return frames, viterbi, loglik

@@ -616,3 +616,71 @@ def rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, g
                                   max(labels.stride(0), 1), _P(grad_scale), _P(costs), _P(dlogits), _P(colsum), _P(ws), ws_bytes,
                                   _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _stream()), "pk_rnnt_pruned_loss")
     return costs
+
+
+# ------------------------------------------------------------------------------------------------
+# forced alignment (include/pika_b200.h, "RNN-T forced alignment")
+
+
+def rnnt_tables(logits, labels, frame_lens, label_lens, V=None, row_lse=None):
+    """logits [B,T,U1,ldv] (bf16|f32) -> (lpb_skew, lpl_skew) [B, T+U1-1, U1] f32: the loss's first pass without the lattice.
+    row_lse [n_parts, B*T*U1, 2]: the producing GEMM's row partials (the logits are then not re-read)"""
+    B, T, U1, ldv = logits.shape
+    V = ldv if V is None else V
+    assert logits.is_contiguous() and labels.dtype == torch.int32 and labels.dim() == 2
+    assert frame_lens.dtype == torch.int32 and label_lens.dtype == torch.int32
+    dev = logits.device
+    lse = torch.empty(B * T * U1, dtype=torch.float32, device=dev)
+    lpb = torch.empty(B, T + U1 - 1, U1, dtype=torch.float32, device=dev)
+    lpl = torch.empty_like(lpb)
+    if row_lse is not None:
+        assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (B * T * U1, 2)
+    check(lib.pk_rnnt_tables(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), B, T, U1, V, ldv, max(labels.stride(0), 1),
+                             _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _P(lse), _P(lpb), _P(lpl), _stream()),
+          "pk_rnnt_tables")
+    return lpb, lpl
+
+
+def rnnt_pruned_tables(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=None):
+    """pruned logits [B*T*R, ldv] (row (b,t,r) = node (t, bounds[b,t] + r)) -> (lpb_skew, lpl_skew) [B, T+U1-1, U1] f32, -inf outside
+    the windows"""
+    B, T = bounds.shape
+    rows, ldv = logits.shape
+    assert rows == B * T * R and logits.is_contiguous() and labels.dtype == torch.int32 and bounds.dtype == torch.int32
+    dev = logits.device
+    lse = torch.empty(rows, dtype=torch.float32, device=dev)
+    lpb = torch.empty(B, T + U1 - 1, U1, dtype=torch.float32, device=dev)
+    lpl = torch.empty_like(lpb)
+    if row_lse is not None:
+        assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (rows, 2)
+    check(lib.pk_rnnt_pruned_tables(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), _P(bounds), B, T, U1, R, V, ldv,
+                                    max(labels.stride(0), 1), _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _P(lse),
+                                    _P(lpb), _P(lpl), _stream()), "pk_rnnt_pruned_tables")
+    return lpb, lpl
+
+
+def rnnt_lattice_costs(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1):
+    """rnnt_lattice without the gradient coefficients -> costs [B] = -log P(y | x)"""
+    dev = lpb_skew.device
+    ws_bytes = _ws_query(lib.pk_rnnt_lattice_workspace, "pk_rnnt_lattice_workspace", B, T, U1)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    costs = torch.empty(B, dtype=torch.float32, device=dev)
+    check(lib.pk_rnnt_lattice_costs(_P(frame_lens), _P(label_lens), B, T, U1, _P(lpb_skew), _P(lpl_skew), _P(costs), _P(ws), ws_bytes,
+                                    _stream()), "pk_rnnt_lattice_costs")
+    return costs
+
+
+def rnnt_viterbi(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1, ld_emit=None, want_decisions=False):
+    """best path through the lattice -> (score [B] f32, emit_frames [B, ld_emit] int32 (default U1 - 1)[, decisions
+    [B, T+U1-1, ceil(U1/32)] int32 words: the label-arc bits, see include/pika_b200.h])"""
+    dev = lpb_skew.device
+    ld = U1 - 1 if ld_emit is None else int(ld_emit)
+    ws_bytes = _ws_query(lib.pk_rnnt_viterbi_workspace, "pk_rnnt_viterbi_workspace", B, T, U1)
+    ws = torch.empty(ws_bytes // 4, dtype=torch.int32, device=dev)
+    score = torch.empty(B, dtype=torch.float32, device=dev)
+    emit = torch.empty(B, ld, dtype=torch.int32, device=dev)
+    check(lib.pk_rnnt_viterbi(_P(frame_lens), _P(label_lens), B, T, U1, _P(lpb_skew), _P(lpl_skew), _P(score), _P(emit), ld, _P(ws), ws_bytes,
+                              _stream()), "pk_rnnt_viterbi")
+    if want_decisions:
+        return score, emit, ws.view(B, T + U1 - 1, (U1 + 31) // 32)
+    return score, emit
