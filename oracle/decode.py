@@ -81,7 +81,7 @@ class Beam:
         for i in range(self.size):                                                     # :161-183
             y = int(self.next_ys[-1][i])
             if (y == self.blk and int(t_idx[int(prev_k[i])]) == num_frames - 1) or len(self.next_ys) > self.max_len:
-                s = self.scores[i].clone()
+                s = self.scores[i]                                                     # a view: the final LM term lands in self.scores
                 self.next_ys[-1][i] = EOS
                 if self.lm is not None:                                                # :167-176
                     fin = defaultdict(lambda: float("inf"))
@@ -91,7 +91,7 @@ class Beam:
                             c = self.state_sets[i][state] + cost
                             if c < fin[f_s]:
                                 fin[f_s] = c
-                    s = s + self.lm_scale * (-min(fin.values()))
+                    s += self.lm_scale * (-min(fin.values()))
                 self.finished.append((float(s), len(self.next_ys) - 1, i))             # GlobalScorer.score is the identity (:246-258)
             else:                                                                      # update_partial_hyp :224-232
                 k0 = int(self.prev_ks[-1][i])

@@ -29,6 +29,7 @@ from .. import _lib
 from .._lib import BeamXfState, PikaError, check, lib
 
 _USE_GRAPH = os.environ.get("PK_DECODE_GRAPH", "1") != "0"      # 0: issue every launch of the beam loop from the host (debugging)
+BEAM_SIZES = (1, 2, 4, 8, 16)                                    # the widths beam_advance_kernel is instantiated for (csrc/beam.cu)
 _POLL = 4                                                        # graph replays (= 8 beam steps) between looks at the done counter
 
 
@@ -247,6 +248,9 @@ class TransducerDecoder():
         self.las_rescorer_bw = getattr(args, "las_rescorer_bw", None) if args is not None else None
         if args is not None and getattr(args, "bilas_rescorer", None) is not None:
             self.bilas_rescorer = args.bilas_rescorer
+        # pk_beam_advance has instances for these widths only; refuse others here, before any kernel launch
+        if beam_size not in BEAM_SIZES:
+            raise PikaError("pika_b200: the device beam search supports beam sizes %s (got %d)" % (", ".join(map(str, BEAM_SIZES)), beam_size))
         self.xf = model.decoder_type != "rnn"            # convolutional-transformer prediction net (decoder/transducer_decoder.py:117-120,151-171)
         if self.xf:
             heads = {l.self_attn.head_count for l in model.decoder.transformer}
@@ -321,6 +325,8 @@ class TransducerDecoder():
         m, blk = self.model, self.blk
         dev = x.device if enc_out is None else enc_out.device
         assert dev.type == "cuda", "pika_b200 decodes on the GPU (there is no CPU fallback)"
+        if m.fc2.weight.shape[0] < self.beam_size:
+            raise PikaError("pika_b200: the vocabulary (%d) is smaller than the beam (%d)" % (m.fc2.weight.shape[0], self.beam_size))
         if self.xf:
             # a hypothesis of up to max_len + 1 labels plus SOS; the prediction net's causal mask buffer is max_size (5000) positions long
             n = max(int(v) if v else 10000 for v in max_len) + 2
