@@ -191,8 +191,9 @@ int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, 
  *   holds u, in frame order: one contiguous range because bounds are non-decreasing).  dh must be zero on the masked rows (u > U_b
  *   or t >= T_b), as pk_rnnt_pruned_loss writes it; rows whose u was clamped are not read.
  * pk_rnnt_pruned_loss: logits [B*T*R, ldv] (row (b, t, r) = node (t, bounds[b,t] + r)) -> costs [B], dlogits (may alias logits; NULL =
- *   costs only; masked rows and the padding columns written 0), dlogits_colsum [ldv] (NULL or the fc2 bias gradient, fixed-order
- *   sum).  Nodes outside the windows are -inf.  row_lse: NULL or the producing GEMM's [n_parts][B*T*R][2] partials.
+ *   costs only; masked rows and the padding columns written 0; needs ldv <= 8192, refused before any launch), dlogits_colsum [ldv]
+ *   (NULL or the fc2 bias gradient, fixed-order sum).  Nodes outside the windows are -inf.  An utterance with bounds -1 gets cost +inf
+ *   and zero dlogits rows.  row_lse: NULL or the producing GEMM's [n_parts][B*T*R][2] partials.
  *   workspace >= the size pk_rnnt_pruned_loss_workspace writes to *bytes. */
 int pk_rnnt_simple_prep(const float* src, int ld_src, int V, int nb, int n_in, int n_out, void* hi, void* lo, int ld_out, float* rmax,
                         void* stream);

@@ -1083,6 +1083,7 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
     PK_CHECK_ARG((reinterpret_cast<uintptr_t>(logits) & 15) == 0, "logits not 16B aligned");
     PK_CHECK_ARG(dlogits == nullptr || (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0, "dlogits not 16B aligned");
     PK_CHECK_ARG(row_lse == nullptr || n_parts >= 1, "n_parts must be >= 1");
+    PK_CHECK_ARG(dlogits == nullptr || ldv <= 8192, "V too large for the gradient kernel (V <= 8192)");
     long long cs_off;
     PK_CHECK_ARG(workspace_bytes >= pruned_ws_parts(B, T, U1, R, ldv, &cs_off), "workspace too small");
     RnntDims d{B, T, U1, V, ldv, ld_labels, T + U1 - 1};
@@ -1103,7 +1104,6 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
         if (rc) return rc;
     }
     if (dlogits == nullptr) return 0;
-    PK_CHECK_ARG(ldv <= 8192, "V too large for the gradient kernel (V <= 8192)");
     const int rgrid = (int)std::min<long long>((rows + 255) / 256, (long long)num_sms() * 8);
     pruned_rows_kernel<<<rgrid, 256, 0, stream>>>(labels, frame_lens, label_lens, bounds, d, R, gb, gl, gb_row, gl_row, y_row);
     PK_CHECK_LAUNCH(); count_launch();

@@ -168,3 +168,41 @@ def test_trainer_flags():
     from pika_b200.trainer import train_transducer_bmuf_otfaug as T
     a = T.build_parser().parse_known_args(["transducer", "d", "l", "o"])[0]
     assert (a.prune_range, a.simple_loss_scale, a.prune_warmup_batches) == (0, 0.5, 0)
+
+
+@pytest.mark.parametrize("T,U,windows", [(1, 0, None), (1, 4, None), (6, 0, None), (9, 7, None), (13, 11, 3), (17, 5, 2), (8, 7, 1)])
+def test_diagonal_lattice_equals_the_node_loop(T, U, windows):
+    """alpha_beta_diag (numpy over anti-diagonals) against oracle.rnnt.rnnt_alpha_beta (a loop over nodes), on random tables and on
+    tables that are -inf outside R-wide windows (R = 1: every node off the windows, so no path and an all -inf beta)"""
+    rng = np.random.default_rng(T * 31 + U)
+    lpb = rng.standard_normal((T, U + 1)) * 3 - 2
+    lpl = rng.standard_normal((T, U)) * 3 - 2
+    if windows is not None:
+        R = windows
+        s = np.minimum(np.arange(T) * max(R - 1, 1) // 2, max(U - R + 1, 0))
+        m = P.window_mask(s, T, U, R)
+        lpb = np.where(m, lpb, -np.inf)
+        lpl = np.where(m[:, :U], lpl, -np.inf)
+    a0, b0 = orc.rnnt_alpha_beta(lpb, lpl, T, U)
+    a1, b1 = P.alpha_beta_diag(lpb, lpl, T, U)
+    for x, y in ((a0, a1), (b0, b1)):
+        assert np.array_equal(np.isneginf(x), np.isneginf(y))
+        f = np.isfinite(x)
+        np.testing.assert_allclose(y[f], x[f], rtol=1e-12, atol=1e-12)
+    c0, gb0, gl0 = P.occupancy(lpb, lpl, T, U)
+    c1, gb1, gl1 = P.occupancy(lpb, lpl, T, U, fast=True)
+    assert c0 == c1 or abs(c0 - c1) < 1e-11 * max(1.0, abs(c0))
+    np.testing.assert_allclose(gb1, gb0, rtol=0, atol=1e-12)
+    np.testing.assert_allclose(gl1, gl0, rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("T,U,R", [(1, 0, 2), (7, 0, 3), (9, 12, 3), (12, 11, 2), (20, 17, 5), (6, 3, 9), (30, 60, 4)])
+def test_vectorised_bounds_equal_the_scalar_oracle(T, U, R):
+    rng = np.random.default_rng(T + 7 * U + R)
+    for g in (rng.random((T, U + 1)).astype(np.float32), np.full((T, U + 1), 0.25, np.float32),
+              (rng.random((T, U + 1)) < 0.2).astype(np.float32)):
+        if U > T * (R - 1):
+            with pytest.raises(ValueError):
+                P.prune_bounds_fast(g, T, U, R)
+            continue
+        np.testing.assert_array_equal(P.prune_bounds_fast(g, T, U, R), P.prune_bounds(g, T, U, R))

@@ -266,11 +266,12 @@ def test_pruned_loss_with_full_windows_matches_dense(prec, decoder_type):
 
 @pytest.mark.parametrize("prec", PRECS, indirect=True)
 @pytest.mark.parametrize("decoder_type", ["rnn", "transformer"])
-def test_pruned_step_gradients_match_float64_restatement(prec, decoder_type):
+@pytest.mark.parametrize("V", [61, 64, 520])
+def test_pruned_step_gradients_match_float64_restatement(V, prec, decoder_type):
     """one step of transducer_loss_pruned (sigma_s = 0.5, sigma_p = 1) against float64 torch given the same encoder / prediction-net
     outputs and the GPU's bounds: joint, fc2 and simple-projection gradients"""
     from pika_b200 import engine
-    V, R = 61, 3
+    R = 3
     Ts, Us = (9, 6), (7, 4)
     x, y, fl, ll = _batch(V, Ts, Us)
     engine.set_dropout_enabled(False)
