@@ -258,6 +258,36 @@ int pk_rnnt_viterbi(const int* frame_lens, const int* label_lens, int B, int T, 
                     float* score, int* emit_frames, int ld_emit, void* workspace, long long workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * RNN-T emission regularisation (pika_b200/csrc/rnnt_loss.cu; DESIGN.md "FastEmit and delay penalty").  Each *_reg entry point is
+ * the entry point of the same name without the suffix, with two more arguments, both finite and >= 0 (refused before any launch):
+ *   delay_penalty lambda_d: every label arc (t, u) -> (t, u+1) of utterance b has lambda_d * ((T_b - 1)/2 - t) added to its log-prob,
+ *           in f64 where the lattice reads it (the tables are not changed).  costs are the penalised -log P and gb / gl its exact
+ *           gradient (the term does not depend on the logits).
+ *   fastemit_lambda lambda_f: the label coefficient gl is multiplied by 1 + lambda_f (FastEmit).  The cost is unchanged, so with
+ *           lambda_f > 0 the gradient is not the gradient of the returned cost.
+ * With both 0 the outputs and launches are those of the plain entry point. */
+int pk_rnnt_loss_fwd_bwd_reg(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, int B, int T,
+                             int U1, int V, int ldv, int ld_labels, const float* grad_scale, float* costs, void* dlogits,
+                             float* dlogits_colsum, void* workspace, long long workspace_bytes, float fastemit_lambda, float delay_penalty,
+                             void* stream);
+int pk_rnnt_loss_fwd_bwd_lse_reg(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, int B,
+                                 int T, int U1, int V, int ldv, int ld_labels, const float* grad_scale, float* costs, void* dlogits,
+                                 float* dlogits_colsum, void* workspace, long long workspace_bytes, const float* row_lse, int n_parts,
+                                 float fastemit_lambda, float delay_penalty, void* stream);
+int pk_rnnt_loss_fwd_bwd_compact_reg(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens, int B,
+                                     int T, int U1, int V, int ldv, int ld_labels, const float* grad_scale, float* costs, void* dz_c,
+                                     float* dlogits_colsum, void* workspace, long long workspace_bytes, const float* row_lse, int n_parts,
+                                     const void* h, int H, void* h_c, int* row_map, int* row_count, float fastemit_lambda,
+                                     float delay_penalty, void* stream);
+int pk_rnnt_lattice_reg(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew, const float* lpl_skew,
+                        const float* grad_scale, float* costs, float* gb, float* gl, void* workspace, long long workspace_bytes,
+                        float fastemit_lambda, float delay_penalty, void* stream);
+int pk_rnnt_pruned_loss_reg(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                            const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
+                            float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
+                            const float* row_lse, int n_parts, float fastemit_lambda, float delay_penalty, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Memory-bound layers around the GEMMs (pika_b200/csrc/elementwise.cu).  `dtype` is the
  * activation type (PK_BF16 production, PK_F32 fp32-class parity mode); statistics are f32.
  */

@@ -16,6 +16,7 @@
 //                           (in place if dlogits aliases logits).
 // Algorithmic HBM traffic: 3 * B*T*(U+1)*V * sizeof(elem)  (+ O(nodes) fp32).
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 
 #include "../../include/pika_b200.h"
@@ -201,11 +202,17 @@ PK_DEVICE lat_t lse2(lat_t a, lat_t b) {
 constexpr int LAT_MAX_G = 512;
 constexpr int LAT_MAX_CPT = 4;      // cells per thread => U1 <= 2048
 
+// Emission regularisation (DESIGN.md "FastEmit and delay penalty"), compiled in only when REG: every label arc (t, u) -> (t, u+1)
+// gets lam_d * ((T_b - 1)/2 - t) added to its log-prob where the sweeps read it (the tables are left as they are), and the label
+// coefficient gl is multiplied by fe_scale = 1 + lambda_fastemit where it is written.  REG = false is the plain lattice.
+PK_DEVICE lat_t delay_term(lat_t lam_d, int T, int t) { return lam_d * (0.5 * (lat_t)(T - 1) - (lat_t)t); }
+
+template <bool REG>
 __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
     const int* __restrict__ frame_lens, const int* __restrict__ label_lens, RnntDims d, int G, int cpt,
     const float* __restrict__ lpb_skew, const float* __restrict__ lpl_skew, lat_t* __restrict__ alpha_skew,
     lat_t* __restrict__ beta_skew, const float* __restrict__ grad_scale, float* __restrict__ costs,
-    float* __restrict__ gb_out, float* __restrict__ gl_out) {
+    float* __restrict__ gb_out, float* __restrict__ gl_out, lat_t lam_d, float fe_scale) {
     extern __shared__ lat_t sm[];            // 2 groups x 2 diagonals x (U1 + 2)
     const int b = blockIdx.x;
     const int grp = threadIdx.x >= G ? 1 : 0;
@@ -257,7 +264,10 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
                     if (c < cpt && u >= lo && u <= hi) {
                         lat_t a = LAT_NEG_INF, cc = LAT_NEG_INF;
                         if (u <= dg - 1) a = prev[u] + pb[c];              // from (t-1, u) via blank
-                        if (u >= 1) cc = prev[u - 1] + pl[c];              // from (t, u-1) via label u
+                        if (u >= 1) {                                      // from (t, u-1) via label u, t = dg - u
+                            if (REG) cc = prev[u - 1] + ((lat_t)pl[c] + delay_term(lam_d, T, dg - u));
+                            else cc = prev[u - 1] + pl[c];
+                        }
                         const lat_t v = lse2(a, cc);
                         cur[u] = v;
                         alpha_skew[base + (size_t)dg * d.U1 + u] = v;
@@ -304,7 +314,10 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
                         const int t = dg - u;
                         lat_t a = LAT_NEG_INF, cc = LAT_NEG_INF;
                         if (t + 1 <= T - 1) a = prev[u] + pb[c];            // to (t+1, u) via blank
-                        if (u + 1 <= U) cc = prev[u + 1] + pl[c];           // to (t, u+1) via label u+1
+                        if (u + 1 <= U) {                                   // to (t, u+1) via label u+1
+                            if (REG) cc = prev[u + 1] + ((lat_t)pl[c] + delay_term(lam_d, T, t));
+                            else cc = prev[u + 1] + pl[c];
+                        }
                         const lat_t v = lse2(a, cc);
                         cur[u] = v;
                         beta_skew[base + (size_t)dg * d.U1 + u] = v;
@@ -333,7 +346,14 @@ __global__ void __launch_bounds__(2 * LAT_MAX_G) rnnt_lattice_kernel(
             if (t < T - 1) bn = beta_skew[skew_index(d, b, t + 1, u)];
             else bn = (u == U) ? 0.0 : LAT_NEG_INF;
             gb = (float)(-exp(a + bn + (lat_t)lpb_skew[sk] - ll)) * gs;
-            if (u < U) gl = (float)(-exp(a + beta_skew[skew_index(d, b, t, u + 1)] + (lat_t)lpl_skew[sk] - ll)) * gs;
+            if (u < U) {
+                if (REG) {
+                    const lat_t lpl = (lat_t)lpl_skew[sk] + delay_term(lam_d, T, t);
+                    gl = (float)(-exp(a + beta_skew[skew_index(d, b, t, u + 1)] + lpl - ll)) * gs * fe_scale;
+                } else {
+                    gl = (float)(-exp(a + beta_skew[skew_index(d, b, t, u + 1)] + (lat_t)lpl_skew[sk] - ll)) * gs;
+                }
+            }
             if (!(gb == gb)) gb = 0.f;
             if (!(gl == gl)) gl = 0.f;
         }
@@ -852,8 +872,21 @@ extern "C" long long pk_rnnt_loss_colsum_workspace_bytes(int B, int T, int U1, i
     return (long long)ggrid * ldv * 4;
 }
 
+// lam_d = delay penalty, fe_scale = 1 + FastEmit lambda; (0, 1) launches the plain lattice
+template <bool REG>
+static int lattice_allow_smem() {                    // the two ping-pong diagonals exceed the default 48 KB from U+1 = 1534 on
+    static bool configured = false;
+    if (!configured) {
+        PK_CHECK_CUDA(cudaFuncSetAttribute(pk::rnnt_lattice_kernel<REG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           2 * 2 * (pk::LAT_MAX_G * pk::LAT_MAX_CPT + 2) * (int)sizeof(pk::lat_t)));
+        configured = true;
+    }
+    return 0;
+}
+
 static int launch_lattice(const int* frame_lens, const int* label_lens, const pk::RnntDims& d, const float* lpb, const float* lpl,
-                          double* alpha, double* beta, const float* grad_scale, float* costs, float* gb, float* gl, cudaStream_t stream) {
+                          double* alpha, double* beta, const float* grad_scale, float* costs, float* gb, float* gl, cudaStream_t stream,
+                          float lam_d = 0.f, float fe_scale = 1.f) {
     using namespace pk;
     const int U1 = d.U1;
     const int lat_smem = 2 * 2 * (U1 + 2) * 8;
@@ -861,14 +894,17 @@ static int launch_lattice(const int* frame_lens, const int* label_lens, const pk
     if (G > LAT_MAX_G) G = LAT_MAX_G;
     const int cpt = (U1 + G - 1) / G;
     PK_CHECK_ARG(cpt <= LAT_MAX_CPT, "U too large for the lattice kernel (U+1 <= 2048)");
-    static bool configured = false;                  // the two ping-pong diagonals exceed the default 48 KB from U+1 = 1534 on
-    if (!configured) {
-        PK_CHECK_CUDA(cudaFuncSetAttribute(rnnt_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           2 * 2 * (LAT_MAX_G * LAT_MAX_CPT + 2) * (int)sizeof(lat_t)));
-        configured = true;
+    if (lam_d != 0.f || fe_scale != 1.f) {
+        const int rc = lattice_allow_smem<true>();
+        if (rc) return rc;
+        rnnt_lattice_kernel<true><<<d.B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
+                                                                    costs, gb, gl, (lat_t)lam_d, fe_scale);
+    } else {
+        const int rc = lattice_allow_smem<false>();
+        if (rc) return rc;
+        rnnt_lattice_kernel<false><<<d.B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
+                                                                     costs, gb, gl, 0.0, 1.f);
     }
-    rnnt_lattice_kernel<<<d.B, 2 * G, lat_smem, stream>>>(frame_lens, label_lens, d, G, cpt, lpb, lpl, alpha, beta, grad_scale,
-                                                       costs, gb, gl);
     PK_CHECK_LAUNCH(); count_launch();
     return 0;
 }
@@ -902,13 +938,25 @@ static int launch_tables(const void* logits, int dtype, const int* labels, const
     return 0;
 }
 
+// FastEmit (lambda_f) and the delay penalty (lambda_d) of the *_reg entry points (DESIGN.md "FastEmit and delay penalty"); the plain
+// entry points pass (0, 0), which launches the plain lattice.
+static int check_emission_reg(float fastemit_lambda, float delay_penalty) {
+    PK_CHECK_ARG(std::isfinite(fastemit_lambda) && fastemit_lambda >= 0.f, "fastemit_lambda must be finite and >= 0");
+    PK_CHECK_ARG(std::isfinite(delay_penalty) && delay_penalty >= 0.f, "delay_penalty must be finite and >= 0");
+    return 0;
+}
+
 static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, const int* frame_lens,
                           const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                           const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
                           long long workspace_bytes, const float* row_lse, int n_parts, int* row_map, int* row_count,
-                          const void* h, int H, void* h_c, void* stream_v) {
+                          const void* h, int H, void* h_c, void* stream_v, float fastemit_lambda, float delay_penalty) {
     using namespace pk;
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    {
+        const int rc = check_emission_reg(fastemit_lambda, delay_penalty);
+        if (rc) return rc;
+    }
     PK_CHECK_ARG(dtype == PK_F32 || dtype == PK_BF16, "bad dtype");
     PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && V > 1, "bad dims");
     const int vn = dtype == PK_F32 ? 4 : 8;
@@ -929,7 +977,8 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
         if (rc) return rc;
     }
     {
-        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
+        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream, delay_penalty,
+                                      1.f + fastemit_lambda);
         if (rc) return rc;
     }
     if (dlogits != nullptr) {
@@ -975,21 +1024,56 @@ static int rnnt_loss_impl(const void* logits, int dtype, const int* labels, cons
     return 0;
 }
 
+extern "C" int pk_rnnt_loss_fwd_bwd_reg(const void* logits, int dtype, const int* labels, const int* frame_lens,
+                                        const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
+                                        const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
+                                        long long workspace_bytes, float fastemit_lambda, float delay_penalty, void* stream) {
+    return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
+                          dlogits_colsum, workspace, workspace_bytes, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr, stream,
+                          fastemit_lambda, delay_penalty);
+}
+
 extern "C" int pk_rnnt_loss_fwd_bwd(const void* logits, int dtype, const int* labels, const int* frame_lens,
                                     const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                                     const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
                                     long long workspace_bytes, void* stream) {
+    return pk_rnnt_loss_fwd_bwd_reg(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
+                                    dlogits_colsum, workspace, workspace_bytes, 0.f, 0.f, stream);
+}
+
+extern "C" int pk_rnnt_loss_fwd_bwd_lse_reg(const void* logits, int dtype, const int* labels, const int* frame_lens,
+                                            const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
+                                            const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
+                                            long long workspace_bytes, const float* row_lse, int n_parts, float fastemit_lambda,
+                                            float delay_penalty, void* stream) {
+    PK_CHECK_ARG(row_lse != nullptr, "row_lse is null");
     return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
-                          dlogits_colsum, workspace, workspace_bytes, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr, stream);
+                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, nullptr, nullptr, nullptr, 0, nullptr, stream,
+                          fastemit_lambda, delay_penalty);
 }
 
 extern "C" int pk_rnnt_loss_fwd_bwd_lse(const void* logits, int dtype, const int* labels, const int* frame_lens,
                                         const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
                                         const float* grad_scale, float* costs, void* dlogits, float* dlogits_colsum, void* workspace,
                                         long long workspace_bytes, const float* row_lse, int n_parts, void* stream) {
-    PK_CHECK_ARG(row_lse != nullptr, "row_lse is null");
-    return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dlogits,
-                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, nullptr, nullptr, nullptr, 0, nullptr, stream);
+    return pk_rnnt_loss_fwd_bwd_lse_reg(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs,
+                                        dlogits, dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, 0.f, 0.f, stream);
+}
+
+extern "C" int pk_rnnt_loss_fwd_bwd_compact_reg(const void* logits, int dtype, const int* labels, const int* frame_lens,
+                                                const int* label_lens, int B, int T, int U1, int V, int ldv, int ld_labels,
+                                                const float* grad_scale, float* costs, void* dz_c, float* dlogits_colsum, void* workspace,
+                                                long long workspace_bytes, const float* row_lse, int n_parts, const void* h, int H,
+                                                void* h_c, int* row_map, int* row_count, float fastemit_lambda, float delay_penalty,
+                                                void* stream) {
+    PK_CHECK_ARG(dtype == PK_BF16, "the compacted gradient is bf16 only");
+    PK_CHECK_ARG(dz_c != nullptr && row_map != nullptr && row_count != nullptr && h != nullptr && h_c != nullptr, "null pointer");
+    PK_CHECK_ARG(H > 0 && H % 8 == 0 && H / 8 <= pk::GRAD_THREADS, "H must be a multiple of 8, <= 2048");
+    PK_CHECK_ARG(dz_c != logits, "dz_c must not alias the logits");
+    PK_CHECK_ARG((reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(h_c) & 15) == 0, "h / h_c not 16B aligned");
+    return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dz_c,
+                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, row_map, row_count, h, H, h_c, stream,
+                          fastemit_lambda, delay_penalty);
 }
 
 extern "C" int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const int* labels, const int* frame_lens,
@@ -997,13 +1081,9 @@ extern "C" int pk_rnnt_loss_fwd_bwd_compact(const void* logits, int dtype, const
                                             const float* grad_scale, float* costs, void* dz_c, float* dlogits_colsum, void* workspace,
                                             long long workspace_bytes, const float* row_lse, int n_parts, const void* h, int H,
                                             void* h_c, int* row_map, int* row_count, void* stream) {
-    PK_CHECK_ARG(dtype == PK_BF16, "the compacted gradient is bf16 only");
-    PK_CHECK_ARG(dz_c != nullptr && row_map != nullptr && row_count != nullptr && h != nullptr && h_c != nullptr, "null pointer");
-    PK_CHECK_ARG(H > 0 && H % 8 == 0 && H / 8 <= pk::GRAD_THREADS, "H must be a multiple of 8, <= 2048");
-    PK_CHECK_ARG(dz_c != logits, "dz_c must not alias the logits");
-    PK_CHECK_ARG((reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(h_c) & 15) == 0, "h / h_c not 16B aligned");
-    return rnnt_loss_impl(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs, dz_c,
-                          dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, row_map, row_count, h, H, h_c, stream);
+    return pk_rnnt_loss_fwd_bwd_compact_reg(logits, dtype, labels, frame_lens, label_lens, B, T, U1, V, ldv, ld_labels, grad_scale, costs,
+                                            dz_c, dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, h, H, h_c, row_map,
+                                            row_count, 0.f, 0.f, stream);
 }
 
 static long long lattice_ws_bytes(int B, int T, int U1) { return 2 * (long long)B * ((long long)T + U1 - 1) * U1 * 8; }
@@ -1013,10 +1093,14 @@ extern "C" int pk_rnnt_lattice_workspace(int B, int T, int U1, long long* bytes)
     return 0;
 }
 
-extern "C" int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
-                               const float* lpl_skew, const float* grad_scale, float* costs, float* gb, float* gl, void* workspace,
-                               long long workspace_bytes, void* stream) {
+extern "C" int pk_rnnt_lattice_reg(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
+                                   const float* lpl_skew, const float* grad_scale, float* costs, float* gb, float* gl, void* workspace,
+                                   long long workspace_bytes, float fastemit_lambda, float delay_penalty, void* stream) {
     using namespace pk;
+    {
+        const int rc = check_emission_reg(fastemit_lambda, delay_penalty);
+        if (rc) return rc;
+    }
     PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0, "bad dims");
     PK_CHECK_ARG(lpb_skew && lpl_skew && costs && gb && gl && workspace, "null pointer");
     PK_CHECK_ARG(workspace_bytes >= lattice_ws_bytes(B, T, U1), "workspace too small");
@@ -1024,7 +1108,14 @@ extern "C" int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int
     const size_t skew = (size_t)B * d.ND * U1;
     double* alpha = reinterpret_cast<double*>(workspace);
     return launch_lattice(frame_lens, label_lens, d, lpb_skew, lpl_skew, alpha, alpha + skew, grad_scale, costs, gb, gl,
-                          reinterpret_cast<cudaStream_t>(stream));
+                          reinterpret_cast<cudaStream_t>(stream), delay_penalty, 1.f + fastemit_lambda);
+}
+
+extern "C" int pk_rnnt_lattice(const int* frame_lens, const int* label_lens, int B, int T, int U1, const float* lpb_skew,
+                               const float* lpl_skew, const float* grad_scale, float* costs, float* gb, float* gl, void* workspace,
+                               long long workspace_bytes, void* stream) {
+    return pk_rnnt_lattice_reg(frame_lens, label_lens, B, T, U1, lpb_skew, lpl_skew, grad_scale, costs, gb, gl, workspace, workspace_bytes,
+                               0.f, 0.f, stream);
 }
 
 // workspace of pk_rnnt_pruned_loss: alpha, beta (f64 skew), lpb, lpl (f32 skew), gb, gl (f32 nodes), lse, gb_row, gl_row, y_row
@@ -1070,12 +1161,16 @@ static int launch_pruned_tables(const void* logits, int dtype, const int* labels
     return 0;
 }
 
-extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
-                                   const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
-                                   float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
-                                   const float* row_lse, int n_parts, void* stream_v) {
+extern "C" int pk_rnnt_pruned_loss_reg(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                                       const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
+                                       float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
+                                       const float* row_lse, int n_parts, float fastemit_lambda, float delay_penalty, void* stream_v) {
     using namespace pk;
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    {
+        const int rc = check_emission_reg(fastemit_lambda, delay_penalty);
+        if (rc) return rc;
+    }
     PK_CHECK_ARG(dtype == PK_F32 || dtype == PK_BF16, "bad dtype");
     PK_CHECK_ARG(B > 0 && T > 0 && U1 > 0 && R >= 1 && V > 1, "bad dims");
     const int vn = dtype == PK_F32 ? 4 : 8;
@@ -1100,7 +1195,8 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
         if (rc) return rc;
     }
     {
-        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream);
+        const int rc = launch_lattice(frame_lens, label_lens, d, lpb, lpl, alpha, beta, grad_scale, costs, gb, gl, stream, delay_penalty,
+                                      1.f + fastemit_lambda);
         if (rc) return rc;
     }
     if (dlogits == nullptr) return 0;
@@ -1126,6 +1222,14 @@ extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* lab
         PK_CHECK_LAUNCH(); count_launch();
     }
     return 0;
+}
+
+extern "C" int pk_rnnt_pruned_loss(const void* logits, int dtype, const int* labels, const int* frame_lens, const int* label_lens,
+                                   const int* bounds, int B, int T, int U1, int R, int V, int ldv, int ld_labels, const float* grad_scale,
+                                   float* costs, void* dlogits, float* dlogits_colsum, void* workspace, long long workspace_bytes,
+                                   const float* row_lse, int n_parts, void* stream) {
+    return pk_rnnt_pruned_loss_reg(logits, dtype, labels, frame_lens, label_lens, bounds, B, T, U1, R, V, ldv, ld_labels, grad_scale, costs,
+                                   dlogits, dlogits_colsum, workspace, workspace_bytes, row_lse, n_parts, 0.f, 0.f, stream);
 }
 
 // ------------------------------------------------------------------------------------ forced alignment entry points

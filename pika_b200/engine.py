@@ -898,26 +898,27 @@ class JointLossFn(torch.autograd.Function):
     costs are computed and no gradient buffer is touched."""
 
     @staticmethod
-    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, need_grad=True):
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, need_grad=True, fastemit_lambda=0.0, delay_penalty=0.0):
         logits, st = _joint_forward(enc, pred, model, want_lse=True)
         V = st["dims"][4]
         ctx.need_grad = need_grad
+        reg = dict(fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
         if not need_grad:
-            costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, want_grad=False, row_lse=st.pop("row_lse"))
+            costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, want_grad=False, row_lse=st.pop("row_lse"), **reg)
             return costs
         db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=logits.device)
         compact = None
         if _COMPACT_GRAD and logits.dtype == torch.bfloat16 and len(st["w2"]) == 1 and len(st["h_parts"]) == 1:
             with _Tap("rnnt_loss"):
                 costs, dz_c, h_c, row_map, rows = K.rnnt_loss_compact(logits, labels, frame_lens, label_lens, st["h_parts"][0], V=V,
-                                                                      colsum=db2, row_lse=st.pop("row_lse"))
+                                                                      colsum=db2, row_lse=st.pop("row_lse"), **reg)
             logits, compact = dz_c, (h_c, row_map, rows)          # the logits and h are released here: dz_c and h_c replace them
             del dz_c, h_c
             st.pop("h_parts")
         else:
             with _Tap("rnnt_loss"):
                 costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, dlogits=logits, colsum=db2,
-                                               row_lse=st.pop("row_lse"))
+                                               row_lse=st.pop("row_lse"), **reg)
         d_enc, d_pred = _joint_backward(logits, st, model, db2=db2, compact=compact)
         del compact
         del logits, st
@@ -941,15 +942,16 @@ class JointLossFn(torch.autograd.Function):
                     p.grad.mul_(w[0])
                 d_enc = d_enc * w[0].to(d_enc.dtype)
                 d_pred = d_pred * w[0].to(d_pred.dtype)
-        return d_enc, d_pred, None, None, None, None, None
+        return d_enc, d_pred, None, None, None, None, None, None, None
 
 
 class RNNTLossFn(torch.autograd.Function):
     """warp_rnnt.RNNTLoss.apply-compatible: log_probs [B,T,U1,V] -> costs [B] (reference call site
-    trainer/train_transducer_bmuf_otfaug.py:58,97-98)."""
+    trainer/train_transducer_bmuf_otfaug.py:58,97-98).  ``fastemit_lambda`` / ``delay_penalty``: check_emission_reg."""
 
     @staticmethod
-    def forward(ctx, log_probs, labels, frame_lens, label_lens):
+    def forward(ctx, log_probs, labels, frame_lens, label_lens, fastemit_lambda=0.0, delay_penalty=0.0):
+        fastemit_lambda, delay_penalty = check_emission_reg(fastemit_lambda, delay_penalty)
         lp = log_probs.contiguous()
         B, T, U1, V = lp.shape
         ldv = V if (V % (8 if lp.dtype == torch.bfloat16 else 4) == 0) else None
@@ -959,14 +961,14 @@ class RNNTLossFn(torch.autograd.Function):
             buf[..., :V].copy_(lp)
             lp = buf
         costs, grads = K.rnnt_loss_fwd_bwd(lp, labels.int().contiguous(), frame_lens.int().contiguous(),
-                                           label_lens.int().contiguous(), V=V)
+                                           label_lens.int().contiguous(), V=V, fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
         ctx.save_for_backward(grads[..., :V])
         return costs
 
     @staticmethod
     def backward(ctx, dcosts):
         (g,) = ctx.saved_tensors
-        return g * dcosts.view(-1, 1, 1, 1).to(g.dtype), None, None, None
+        return g * dcosts.view(-1, 1, 1, 1).to(g.dtype), None, None, None, None, None
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1155,13 +1157,26 @@ class LogSoftmaxFn(torch.autograd.Function):
         return out, None
 
 
-def transducer_loss(model, x, y, frame_lens, label_lens, x_len=None, t_out=None):
+def check_emission_reg(fastemit_lambda, delay_penalty):
+    """-> (fastemit_lambda, delay_penalty) as floats; ValueError unless both are finite and >= 0 (DESIGN.md "FastEmit and delay
+    penalty")"""
+    lam_f, lam_d = float(fastemit_lambda), float(delay_penalty)
+    if not (math.isfinite(lam_f) and math.isfinite(lam_d) and lam_f >= 0.0 and lam_d >= 0.0):
+        raise ValueError("emission regularisation needs finite fastemit_lambda >= 0 and delay_penalty >= 0 (got %r, %r)"
+                         % (fastemit_lambda, delay_penalty))
+    return lam_f, lam_d
+
+
+def transducer_loss(model, x, y, frame_lens, label_lens, x_len=None, t_out=None, fastemit_lambda=0.0, delay_penalty=0.0):
     """Fused training path: costs [B] with gradients wired to every parameter.  ``x_len`` / ``t_out`` as in transducer_forward
-    (the trainer passes the encoder output lengths, which are also ``frame_lens``)."""
+    (the trainer passes the encoder output lengths, which are also ``frame_lens``).  ``fastemit_lambda`` / ``delay_penalty``: FastEmit
+    and the delay penalty (DESIGN.md "FastEmit and delay penalty"); the costs are then the delay-penalised ones, and with FastEmit the
+    gradients are not those of the costs.  Out-of-range values raise ValueError before any work."""
+    lam_f, lam_d = check_emission_reg(fastemit_lambda, delay_penalty)
     enc = model_encoder_forward_act(model, x, x_len, t_out)
     pred = prednet_forward_act(model, y)
     return JointLossFn.apply(enc, pred, model, y.int().contiguous(), frame_lens.int().contiguous(), label_lens.int().contiguous(),
-                             torch.is_grad_enabled())
+                             torch.is_grad_enabled(), lam_f, lam_d)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1214,13 +1229,17 @@ def check_smoothing_scales(lm_only_scale, am_only_scale):
     return lam_l, lam_a
 
 
-def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.0, need_grad=True, lm_only_scale=0.0, am_only_scale=0.0):
+def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.0, need_grad=True, lm_only_scale=0.0, am_only_scale=0.0,
+                delay_penalty=0.0):
     """The simple joiner's RNN-T loss from its two projections am [B*T, ldv], lm [B*U1, ldv] (f32, V valid columns) -> (costs [B],
     bounds [B,T] int32 for windows of R, dam, dlm) with dam [B*T, ldv], dlm [B*U1, ldv] (activation dtype, padding columns 0) the
     gradients of sum_b scale * cost_b, or None when ``need_grad`` is False.  R = 0: no bounds (None).
     ``lm_only_scale`` / ``am_only_scale`` (lam_l, lam_a): the lattice's log-probs become mu * full + lam_l * LM-only + lam_a * AM-only,
-    mu = 1 - lam_l - lam_a (DESIGN.md "Pruned RNN-T"); costs and bounds are then the smoothed ones.  Both 0: the unsmoothed kernels."""
+    mu = 1 - lam_l - lam_a (DESIGN.md "Pruned RNN-T"); costs and bounds are then the smoothed ones.  Both 0: the unsmoothed kernels.
+    ``delay_penalty``: the lattice's label arcs carry the delay penalty (DESIGN.md "FastEmit and delay penalty"), so the costs, the bounds
+    and the gradients are the penalised ones."""
     lam_l, lam_a = check_smoothing_scales(lm_only_scale, am_only_scale)
+    _, lam_d = check_emission_reg(0.0, delay_penalty)
     smooth = lam_l > 0.0 or lam_a > 0.0
     ldv = am.shape[1]
     U1p = (U1 + 7) // 8 * 8
@@ -1243,7 +1262,7 @@ def simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale=1.
                                                    Nl, logq, Na, lam_l, lam_a)
         else:
             lpb, lpl = K.rnnt_simple_tables(am, lm, am_max, lm_max, S.view(B * T, U1p), labels, frame_lens, label_lens, B, T, U1)
-        costs, gb, gl = K.rnnt_lattice(lpb, lpl, frame_lens, label_lens, B, T, U1)
+        costs, gb, gl = K.rnnt_lattice(lpb, lpl, frame_lens, label_lens, B, T, U1, delay_penalty=lam_d)
     del lpb, lpl
     bounds = None
     if R:
@@ -1284,10 +1303,11 @@ class SimpleLossFn(torch.autograd.Function):
     log(E.P^T) + the row maxes (pk_rnnt_simple_*), the lattice runs on the resulting tables (pk_rnnt_lattice) and its occupancies give the
     bounds (pk_rnnt_prune_bounds).  The gradients (for an upstream gradient of ``scale`` per utterance) are formed here in forward:
     dam = E (.) (W P) and dlm = P (.) (W^T E) plus the blank / label terms, W = scale * occupancy / (E.P^T).  ``lm_only_scale`` /
-    ``am_only_scale`` smooth the lattice as in simple_loss."""
+    ``am_only_scale`` smooth the lattice and ``delay_penalty`` penalises its label arcs, as in simple_loss."""
 
     @staticmethod
-    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, R, scale, need_grad, lm_only_scale=0.0, am_only_scale=0.0):
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, R, scale, need_grad, lm_only_scale=0.0, am_only_scale=0.0,
+                delay_penalty=0.0):
         B, T, H = enc.shape
         U1 = pred.shape[1]
         am_p, lm_p = model.simple_am_proj, model.simple_lm_proj
@@ -1300,7 +1320,7 @@ class SimpleLossFn(torch.autograd.Function):
         gemm_parts([enc_parts], [stage_weight(am_p.weight)], am[:, :V], bias=am_p.bias.detach())
         gemm_parts([pred_parts], [stage_weight(lm_p.weight)], lm[:, :V], bias=lm_p.bias.detach())
         costs, bounds, dam, dlm = simple_loss(am, lm, V, B, T, U1, labels, frame_lens, label_lens, R, scale, need_grad, lm_only_scale,
-                                              am_only_scale)
+                                              am_only_scale, delay_penalty)
         del am, lm
         ctx.mark_non_differentiable(bounds)
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
@@ -1315,7 +1335,7 @@ class SimpleLossFn(torch.autograd.Function):
         m = ctx.model
         d_enc, d_pred = _scaled_grads_backward(ctx, dcosts, (m.simple_am_proj.weight, m.simple_am_proj.bias, m.simple_lm_proj.weight,
                                                              m.simple_lm_proj.bias), "SimpleLossFn")
-        return d_enc, d_pred, None, None, None, None, None, None, None, None, None
+        return d_enc, d_pred, None, None, None, None, None, None, None, None, None, None
 
 
 def _pruned_joint_forward(enc, pred, model, bounds, R):
@@ -1353,10 +1373,10 @@ class PrunedJointLossFn(torch.autograd.Function):
     """Pruned joint + RNN-T loss: row (b, t, r) of the joint is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd),
     fc2 runs on the B*T*R rows (with the row log-sum-exp epilogue in bf16), the loss and its gradient come from pk_rnnt_pruned_loss
     (in place over the logits), and the joint backward runs at once, as in JointLossFn.  Gradients are formed for an upstream
-    gradient of ``scale`` per utterance."""
+    gradient of ``scale`` per utterance.  ``fastemit_lambda`` / ``delay_penalty`` as in transducer_loss."""
 
     @staticmethod
-    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, bounds, R, scale, need_grad):
+    def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, bounds, R, scale, need_grad, fastemit_lambda=0.0, delay_penalty=0.0):
         B, T, H = enc.shape
         U1 = pred.shape[1]
         fc2 = model.fc2
@@ -1367,13 +1387,14 @@ class PrunedJointLossFn(torch.autograd.Function):
         logits, row_lse, st = _pruned_joint_forward(enc, pred, model, bounds, R)
         ex, py, h_parts, w2 = st["ex"], st["py"], st.pop("h_parts"), st["w2"]
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
+        reg = dict(fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
         if not need_grad:
-            return K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=row_lse)
+            return K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=row_lse, **reg)
         scale_t = torch.full((B,), float(scale), dtype=torch.float32, device=dev)
         db2 = torch.empty(ldv, dtype=torch.float32, device=dev)
         with _Tap("rnnt_loss"):
             costs = K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=scale_t, dlogits=logits,
-                                       colsum=db2, row_lse=row_lse)
+                                       colsum=db2, row_lse=row_lse, **reg)
         del row_lse
         dl_v = [p[:, :V] for p in stage_act(logits)]
         dh = _new((rows, H), like=enc)
@@ -1395,7 +1416,7 @@ class PrunedJointLossFn(torch.autograd.Function):
         m = ctx.model
         d_enc, d_pred = _scaled_grads_backward(ctx, dcosts, (m.fc1.weight, m.fc1.bias, m.fc_gate.weight, m.fc_gate.bias, m.fc2.weight,
                                                              m.fc2.bias), "PrunedJointLossFn")
-        return d_enc, d_pred, None, None, None, None, None, None, None, None
+        return d_enc, d_pred, None, None, None, None, None, None, None, None, None, None
 
 
 def check_prune_feasible(frame_lens, label_lens, prune_range):
@@ -1414,13 +1435,16 @@ def check_prune_feasible(frame_lens, label_lens, prune_range):
 
 
 def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, simple_scale, pruned_scale, x_len=None, t_out=None,
-                           lm_only_scale=0.0, am_only_scale=0.0):
+                           lm_only_scale=0.0, am_only_scale=0.0, fastemit_lambda=0.0, delay_penalty=0.0):
     """Pruned RNN-T training path -> (simple_costs [B], pruned_costs [B]).  The gradients wired to every parameter are those of
     sum_b (simple_scale * simple_b + pruned_scale * pruned_b); back-propagate exactly that sum (TrainStep does).  Refuses, before any
     work, an utterance that has no path inside the windows.  With grad mode off only the costs are computed.  ``model`` needs the
     simple projections (Net with prune_range > 0).  ``lm_only_scale`` / ``am_only_scale`` smooth the simple loss (simple_loss); its
-    costs and the bounds are then the smoothed ones.  Out-of-range scales raise ValueError before any work."""
+    costs and the bounds are then the smoothed ones.  ``delay_penalty`` applies to both losses (so the bounds come from the penalised
+    simple lattice) and ``fastemit_lambda`` to the pruned loss only (DESIGN.md "FastEmit and delay penalty").  Out-of-range scales raise
+    ValueError before any work."""
     lam_l, lam_a = check_smoothing_scales(lm_only_scale, am_only_scale)
+    lam_f, lam_d = check_emission_reg(fastemit_lambda, delay_penalty)
     check_prune_feasible(frame_lens, label_lens, prune_range)
     if not hasattr(model, "simple_am_proj"):
         raise ValueError("the pruned RNN-T loss needs the simple joiner: build Net with prune_range > 0")
@@ -1430,8 +1454,8 @@ def transducer_loss_pruned(model, x, y, frame_lens, label_lens, prune_range, sim
     need = torch.is_grad_enabled()
     enc = model_encoder_forward_act(model, x, x_len, t_out)
     pred = prednet_forward_act(model, y)
-    simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need, lam_l, lam_a)
-    pruned_costs = PrunedJointLossFn.apply(enc, pred, model, labels, fl, ll, bounds, R, float(pruned_scale), need)
+    simple_costs, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, float(simple_scale), need, lam_l, lam_a, lam_d)
+    pruned_costs = PrunedJointLossFn.apply(enc, pred, model, labels, fl, ll, bounds, R, float(pruned_scale), need, lam_f, lam_d)
     return simple_costs, pruned_costs
 
 

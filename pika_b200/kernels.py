@@ -107,14 +107,22 @@ def row_lse_parts(M, N, block_n=0):
     return int(lib.pk_gemm_row_lse_parts(M, N, block_n))
 
 
+def _emission_reg(fastemit_lambda, delay_penalty):
+    """-> the two floats, or None when both are 0 (the plain entry points run)"""
+    lf, ld = float(fastemit_lambda), float(delay_penalty)
+    return None if lf == 0.0 and ld == 0.0 else (lf, ld)
+
+
 def rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=None, grad_scale=None, dlogits=None, want_grad=True, colsum=None,
-                      row_lse=None):
+                      row_lse=None, fastemit_lambda=0.0, delay_penalty=0.0):
     """logits [B,T,U1,ldv] (bf16|f32) -> (costs [B] f32, dlogits).  dlogits may alias logits.
-    row_lse [n_parts, B*T*U1, 2]: per-row log-sum-exp partials written by the producing GEMM (skips the first pass)."""
+    row_lse [n_parts, B*T*U1, 2]: per-row log-sum-exp partials written by the producing GEMM (skips the first pass).
+    fastemit_lambda, delay_penalty: emission regularisation (include/pika_b200.h, *_reg); both 0 is the plain loss."""
     B, T, U1, ldv = logits.shape
     V = ldv if V is None else V
     assert logits.is_contiguous() and labels.dtype == torch.int32 and labels.dim() == 2
     assert frame_lens.dtype == torch.int32 and label_lens.dtype == torch.int32
+    reg = _emission_reg(fastemit_lambda, delay_penalty)
     ws_bytes = int(lib.pk_rnnt_loss_workspace_bytes(B, T, U1))
     if colsum is not None:
         ws_bytes += int(lib.pk_rnnt_loss_colsum_workspace_bytes(B, T, U1, ldv))
@@ -122,21 +130,24 @@ def rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=None, grad_scale
     costs = torch.empty(B, dtype=torch.float32, device=logits.device)
     if want_grad and dlogits is None:
         dlogits = torch.empty_like(logits)
+    args = (_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), B, T, U1, V, ldv, max(labels.stride(0), 1), _P(grad_scale),
+            _P(costs), _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes)
     if row_lse is not None:
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (B * T * U1, 2)
-        check(lib.pk_rnnt_loss_fwd_bwd_lse(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens),
-                                           B, T, U1, V, ldv, max(labels.stride(0), 1), _P(grad_scale), _P(costs),
-                                           _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes,
-                                           _P(row_lse), int(row_lse.shape[0]), _stream()), "pk_rnnt_loss_fwd_bwd_lse")
+        args += (_P(row_lse), int(row_lse.shape[0]))
+        if reg is None:
+            check(lib.pk_rnnt_loss_fwd_bwd_lse(*args, _stream()), "pk_rnnt_loss_fwd_bwd_lse")
+        else:
+            check(lib.pk_rnnt_loss_fwd_bwd_lse_reg(*args, *reg, _stream()), "pk_rnnt_loss_fwd_bwd_lse_reg")
         return costs, dlogits
-    check(lib.pk_rnnt_loss_fwd_bwd(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens),
-                                   B, T, U1, V, ldv, max(labels.stride(0), 1), _P(grad_scale), _P(costs),
-                                   _P(dlogits if want_grad else None), _P(colsum), _P(ws), ws_bytes, _stream()),
-          "pk_rnnt_loss_fwd_bwd")
+    if reg is None:
+        check(lib.pk_rnnt_loss_fwd_bwd(*args, _stream()), "pk_rnnt_loss_fwd_bwd")
+    else:
+        check(lib.pk_rnnt_loss_fwd_bwd_reg(*args, *reg, _stream()), "pk_rnnt_loss_fwd_bwd_reg")
     return costs, dlogits
 
 
-def rnnt_loss_compact(logits, labels, frame_lens, label_lens, h, V=None, colsum=None, row_lse=None):
+def rnnt_loss_compact(logits, labels, frame_lens, label_lens, h, V=None, colsum=None, row_lse=None, fastemit_lambda=0.0, delay_penalty=0.0):
     """bf16 logits [B,T,U1,ldv], joint activations h [B*T*U1, H] -> (costs [B], dz_c [R, ldv], h_c [R, H], row_map [R], row_count [1]).
     Only the rows whose gradient is not all zeros are stored: dz_c / h_c rows [0, row_count) hold them in row order, row_map[r] is the
     row's index there or -1.  dz_c is a new buffer as large as the logits (the two are alive together while the gradient is formed)."""
@@ -158,10 +169,14 @@ def rnnt_loss_compact(logits, labels, frame_lens, label_lens, h, V=None, colsum=
     row_count = torch.empty(1, dtype=torch.int32, device=dev)
     if row_lse is not None:
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (R, 2)
-    check(lib.pk_rnnt_loss_fwd_bwd_compact(_P(logits), PK_BF16, _P(labels), _P(frame_lens), _P(label_lens), B, T, U1, V, ldv,
-                                           max(labels.stride(0), 1), None, _P(costs), _P(dz_c), _P(colsum), _P(ws), ws_bytes,
-                                           _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _P(h), H, _P(h_c),
-                                           _P(row_map), _P(row_count), _stream()), "pk_rnnt_loss_fwd_bwd_compact")
+    args = (_P(logits), PK_BF16, _P(labels), _P(frame_lens), _P(label_lens), B, T, U1, V, ldv, max(labels.stride(0), 1), None, _P(costs),
+            _P(dz_c), _P(colsum), _P(ws), ws_bytes, _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _P(h), H, _P(h_c),
+            _P(row_map), _P(row_count))
+    reg = _emission_reg(fastemit_lambda, delay_penalty)
+    if reg is None:
+        check(lib.pk_rnnt_loss_fwd_bwd_compact(*args, _stream()), "pk_rnnt_loss_fwd_bwd_compact")
+    else:
+        check(lib.pk_rnnt_loss_fwd_bwd_compact_reg(*args, *reg, _stream()), "pk_rnnt_loss_fwd_bwd_compact_reg")
     return costs, dz_c, h_c, row_map, row_count
 
 
@@ -496,7 +511,7 @@ def _ws_query(fn, name, *dims):
     return int(out.value)
 
 
-def rnnt_lattice(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1, grad_scale=None):
+def rnnt_lattice(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1, grad_scale=None, fastemit_lambda=0.0, delay_penalty=0.0):
     """log-prob tables in the lattice's skewed layout [B, T+U1-1, U1] -> (costs [B], gb [B,T,U1], gl [B,T,U1])"""
     dev = lpb_skew.device
     ws_bytes = _ws_query(lib.pk_rnnt_lattice_workspace, "pk_rnnt_lattice_workspace", B, T, U1)
@@ -504,8 +519,12 @@ def rnnt_lattice(lpb_skew, lpl_skew, frame_lens, label_lens, B, T, U1, grad_scal
     costs = torch.empty(B, dtype=torch.float32, device=dev)
     gb = torch.empty(B, T, U1, dtype=torch.float32, device=dev)
     gl = torch.empty_like(gb)
-    check(lib.pk_rnnt_lattice(_P(frame_lens), _P(label_lens), B, T, U1, _P(lpb_skew), _P(lpl_skew), _P(grad_scale), _P(costs), _P(gb),
-                              _P(gl), _P(ws), ws_bytes, _stream()), "pk_rnnt_lattice")
+    args = (_P(frame_lens), _P(label_lens), B, T, U1, _P(lpb_skew), _P(lpl_skew), _P(grad_scale), _P(costs), _P(gb), _P(gl), _P(ws), ws_bytes)
+    reg = _emission_reg(fastemit_lambda, delay_penalty)
+    if reg is None:
+        check(lib.pk_rnnt_lattice(*args, _stream()), "pk_rnnt_lattice")
+    else:
+        check(lib.pk_rnnt_lattice_reg(*args, *reg, _stream()), "pk_rnnt_lattice_reg")
     return costs, gb, gl
 
 
@@ -601,7 +620,8 @@ def joint_gate_pruned_bwd(ex, py, bounds, dh, dex, dpy, B, T, U1, R, H):
           "pk_joint_gate_pruned_bwd")
 
 
-def rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=None, dlogits=None, colsum=None, row_lse=None):
+def rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=None, dlogits=None, colsum=None, row_lse=None,
+                     fastemit_lambda=0.0, delay_penalty=0.0):
     """logits [B*T*R, ldv] (row (b,t,r) = node (t, bounds[b,t] + r)) -> costs [B]; dlogits (may alias logits) and colsum [ldv] filled
     when given"""
     B, T = bounds.shape
@@ -612,9 +632,14 @@ def rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, g
     costs = torch.empty(B, dtype=torch.float32, device=logits.device)
     if row_lse is not None:
         assert row_lse.dtype == torch.float32 and row_lse.is_contiguous() and tuple(row_lse.shape[1:]) == (rows, 2)
-    check(lib.pk_rnnt_pruned_loss(_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), _P(bounds), B, T, U1, R, V, ldv,
-                                  max(labels.stride(0), 1), _P(grad_scale), _P(costs), _P(dlogits), _P(colsum), _P(ws), ws_bytes,
-                                  _P(row_lse), int(row_lse.shape[0]) if row_lse is not None else 0, _stream()), "pk_rnnt_pruned_loss")
+    args = (_P(logits), _dt(logits), _P(labels), _P(frame_lens), _P(label_lens), _P(bounds), B, T, U1, R, V, ldv, max(labels.stride(0), 1),
+            _P(grad_scale), _P(costs), _P(dlogits), _P(colsum), _P(ws), ws_bytes, _P(row_lse),
+            int(row_lse.shape[0]) if row_lse is not None else 0)
+    reg = _emission_reg(fastemit_lambda, delay_penalty)
+    if reg is None:
+        check(lib.pk_rnnt_pruned_loss(*args, _stream()), "pk_rnnt_pruned_loss")
+    else:
+        check(lib.pk_rnnt_pruned_loss_reg(*args, *reg, _stream()), "pk_rnnt_pruned_loss_reg")
     return costs
 
 

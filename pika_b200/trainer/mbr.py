@@ -112,8 +112,10 @@ def alignment_nodes(hyps, seq_grad, Tp, U, blk):
     return cat(ex, np.int32), cat(py, np.int32), cat(tk, np.int32), cat(cf, np.float32)
 
 
-def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, rnnt_scale=1.0, sm_scale=1.0):
-    """Leaves d(rnnt_scale * rnnt_loss + mbr_loss)/d(param) in every ``param.grad``.
+def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, rnnt_scale=1.0, sm_scale=1.0, fastemit_lambda=0.0,
+                         delay_penalty=0.0):
+    """Leaves d(rnnt_scale * rnnt_loss + mbr_loss)/d(param) in every ``param.grad``.  ``fastemit_lambda`` / ``delay_penalty`` apply to
+    the RNN-T branch only, as in engine.transducer_loss; the MBR loss is unchanged.
     feats [bsz,T,D] (already CMVN'd / SpecAugmented), target [bsz,Umax] int64 (padded with padding_idx),
     ret = decode_batch output with n_best == beam.  Returns (mbr_loss, rnnt_loss) as python floats / tensor."""
     dev = feats.device
@@ -149,7 +151,8 @@ def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, 
     gs = torch.full((bsz,), float(rnnt_scale), dtype=torch.float32, device=dev)
     db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=dev)
     costs, _ = K.rnnt_loss_fwd_bwd(logits, target[:, :u_ref].int().contiguous(), len_batch.int().contiguous(),
-                                   ali_lens.int().contiguous(), V=V, grad_scale=gs, dlogits=logits, colsum=db2)
+                                   ali_lens.int().contiguous(), V=V, grad_scale=gs, dlogits=logits, colsum=db2,
+                                   fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
     d_enc, d_pred_ref = engine._joint_backward(logits, st, model, db2=db2)
     del logits, st
 

@@ -39,6 +39,11 @@ def smoothing_scales(args):
     return dict(lm_only_scale=float(getattr(args, "lm_only_scale", 0.0)), am_only_scale=float(getattr(args, "am_only_scale", 0.0)))
 
 
+def emission_reg(args):
+    """the FastEmit / delay-penalty keywords of engine.transducer_loss(_pruned) from --fastemit_lambda / --delay_penalty (not ramped)"""
+    return dict(fastemit_lambda=float(getattr(args, "fastemit_lambda", 0.0)), delay_penalty=float(getattr(args, "delay_penalty", 0.0)))
+
+
 class TrainStep:
     def __init__(self, model, args, frontend, bmuf, optimizer, offset=None, scale=None, spec_augmentor=None):
         self.model, self.args, self.frontend, self.bmuf, self.opt = model, args, frontend, bmuf, optimizer
@@ -70,11 +75,12 @@ class TrainStep:
         if getattr(a, "prune_range", 0) > 0:
             ss, ps = prune_loss_scales(a, a.epoch * a.num_batches_per_epoch + self.num_done)
             simple, costs = engine.transducer_loss_pruned(self.model, feats, batch["target"], len_batch, batch["ali_lens"], a.prune_range,
-                                                          ss, ps, x_len=len_batch, t_out=t_out, **smoothing_scales(a))
+                                                          ss, ps, x_len=len_batch, t_out=t_out, **smoothing_scales(a), **emission_reg(a))
             self.simple_costs = simple
             loss = (simple * ss + costs * ps).sum()                       # upstream gradients: exactly the scales passed above
         else:
-            costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out)
+            costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out,
+                                           **emission_reg(a))
             loss = costs.sum()
         engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1
         try:

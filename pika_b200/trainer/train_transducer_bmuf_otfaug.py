@@ -11,6 +11,7 @@ What runs underneath: raw-PCM loader threads -> GPU front end -> sm_90a model / 
 """
 import argparse
 import importlib
+import math
 import os
 import sys
 
@@ -61,15 +62,16 @@ def run_one_epoch(epoch, model, log_f, args, bmuf_trainer, training):
             else:
                 with torch.no_grad():
                     feats = step.features(batch)
-                    from .step import encoder_out_lens, encoder_out_max, smoothing_scales
+                    from .step import emission_reg, encoder_out_lens, encoder_out_max, smoothing_scales
                     tl = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
                     t_out = encoder_out_max(int(batch["t_max"]), args.model_lctx, args.model_rctx, args.model_stride)
                     if pruned:
                         simple, costs = engine.transducer_loss_pruned(model, feats, batch["target"], tl, batch["ali_lens"],
                                                                       args.prune_range, args.simple_loss_scale, 1.0, x_len=tl, t_out=t_out,
-                                                                      **smoothing_scales(args))
+                                                                      **smoothing_scales(args), **emission_reg(args))
                     else:
-                        costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out)
+                        costs = engine.transducer_loss(model, feats, batch["target"], tl, batch["ali_lens"], x_len=tl, t_out=t_out,
+                                                       **emission_reg(args))
             loss = float(costs.sum().item())
             simple_loss = float(simple.sum().item()) if pruned else 0.0
         else:                                                 # empty batch (:100-101)
@@ -158,6 +160,13 @@ def build_parser():
     parser.add_argument('--am_only_scale', type=float, default=0.0,
                         help='pruned RNN-T (needs --prune_range): weight of the AM-only log-probs (against the batch\'s label unigram) '
                              'mixed into the simple joiner\'s lattice; >= 0, and with --lm_only_scale < 1')
+    parser.add_argument('--fastemit_lambda', type=float, default=0.0,
+                        help='FastEmit (DESIGN.md "FastEmit and delay penalty"): scale the gradient of every label arc of the RNN-T '
+                             'loss (the pruned loss with --prune_range) by 1 + this; the logged loss is unchanged.  >= 0, 0 = off')
+    parser.add_argument('--delay_penalty', type=float, default=0.0,
+                        help='delay penalty: add this x ((T-1)/2 - t) to the log-prob of every label arc emitted on frame t, in the '
+                             'RNN-T loss and (with --prune_range) the simple loss too; the logged losses are the penalised ones.  '
+                             '>= 0, 0 = off; not ramped by --prune_warmup_batches')
     return parser
 
 
@@ -172,6 +181,14 @@ def check_smoothing_args(parser, args):
         parser.error('--lm_only_scale and --am_only_scale must be >= 0 with a sum < 1 (got %r, %r)' % (lam_l, lam_a))
 
 
+def check_emission_reg_args(parser, args):
+    """parser.error unless --fastemit_lambda and --delay_penalty are finite and >= 0"""
+    for name in ('fastemit_lambda', 'delay_penalty'):
+        v = getattr(args, name)
+        if not (math.isfinite(v) and v >= 0.0):
+            parser.error('--%s must be finite and >= 0 (got %r)' % (name, v))
+
+
 def main(argv=None):
     parser = build_parser()
     args, _ = parser.parse_known_args(argv)
@@ -179,6 +196,7 @@ def main(argv=None):
     loader_module.register(parser)
     args = parser.parse_args(argv)
     check_smoothing_args(parser, args)
+    check_emission_reg_args(parser, args)
     args.input_dim = loader_module.get_inputdim(args)
     args.dataloader = loader_module.dataloader
     args.raw_batches = True

@@ -28,7 +28,7 @@ from .bmuf import BmufTrainer
 from .flat import FlatParams, SgdNesterovClip, lr_at
 from .mbr import mbr_forward_backward
 from .step import TrainStep, encoder_out_lens
-from .train_transducer_bmuf_otfaug import build_parser as build_rnnt_parser
+from .train_transducer_bmuf_otfaug import build_parser as build_rnnt_parser, check_emission_reg_args
 
 MASTER_NODE = 0
 
@@ -66,7 +66,7 @@ def run_one_epoch(epoch, log_f, model, args, bmuf_trainer):
             if spec is not None:                                              # SpecAugment on the training forward only (:134-135)
                 spec.apply(feats)
             mbr, costs = mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=args.blk, rnnt_scale=args.rnnt_scale,
-                                              sm_scale=args.sm_scale)
+                                              sm_scale=args.sm_scale, fastemit_lambda=args.fastemit_lambda, delay_penalty=args.delay_penalty)
             optimizer.step()                                                  # clip_grad_norm_(inf) + SGD(nesterov) (:236-240)
             mbr_loss, rnnt_loss = float(mbr), float(costs.sum().item())
         try:                                                                  # (:245-257) for every loader item, data or not
@@ -110,6 +110,7 @@ def main(argv=None):
         parser.error('--block_sync %s: the MBR trainer supports only bmuf' % args.block_sync)
     if args.lm_only_scale != 0.0 or args.am_only_scale != 0.0:    # inherited from the RNN-T parser; there is no simple loss here
         parser.error('--lm_only_scale / --am_only_scale: the MBR trainer has no simple loss to smooth')
+    check_emission_reg_args(parser, args)        # inherited: applied to the RNN-T branch, not to the MBR loss
     if args.lm:
         raise NotImplementedError("pika_b200: --lm (neural LM fusion) is outside the hot path")
     args.input_dim = loader_module.get_inputdim(args)
