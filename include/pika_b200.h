@@ -330,6 +330,22 @@ int pk_attention_bwd_bits(const void* q, const void* k, const void* v, long long
                           const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
                           long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
                           void* stream);
+/* Chunk-masked (streaming) self-attention, keep-bits form (DESIGN.md "Chunked attention").  Frame t lies in chunk
+ * (t + chunk_off) / chunk_len; query i sees key j iff chunk(i) - left_chunks <= chunk(j) <= chunk(i), with no lower limit when
+ * left_chunks = -1.  A frame always sees itself.  Arguments otherwise as pk_attention_fwd_bits / pk_attention_bwd_bits, with the same
+ * dropout decisions for every pair; keep_bits may be NULL only when drop_p == 0.  The kernels skip every 64-wide key tile (the dK/dV
+ * kernel: query tile) that no row of the 128-row block sees, and never write or read the keep bits of a skipped tile.  The lse padding
+ * entries are written as without the mask.  A mask that lets every query see every key runs the unmasked kernels.
+ * Refused before any launch: chunk_len < 1, chunk_off < 0, left_chunks < -1. */
+int pk_attention_fwd_chunk(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                           int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits,
+                           int chunk_len, int chunk_off, int left_chunks, void* stream);
+int pk_attention_bwd_chunk(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                           const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                           long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
+                           int chunk_len, int chunk_off, int left_chunks, void* stream);
+/* 1 when that mask lets every query of a T-frame sequence see every key, 0 when it does not, -1 on bad arguments (a pure host function) */
+int pk_attention_chunk_admits_all(int T, int chunk_len, int chunk_off, int left_chunks);
 /* nn.BatchNorm1d over rows [rows, C] (trainer/model/rnnt_tdnn_transformer.py:41,58-59,69,76-82,85):
  * train: batch statistics incl. padded frames, running stats updated with the given momentum (unbiased variance); eval: running
  * stats.  stats_ws: pk_colstats_ws_floats(C) + 2*C floats scratch.  mean/rstd [C] are saved for the backward.
@@ -359,6 +375,10 @@ int pk_softmax_fwd(const float* S, long long ld_s, void* P, void* Pd, int dtype,
  * (key_pad: uint8 [sequences][n] or NULL).  The backward is pk_softmax_bwd (a dropped key has P = 0). */
 int pk_softmax_masked_fwd(const float* S, long long ld_s, void* P, void* Pd, int dtype, long long ld_p, long long rows, int n,
                           int q_len, int heads, int causal, const uint8_t* key_pad, float drop_p, uint32_t seed, void* stream);
+/* chunk-masked self-attention forward (the chunk mask of pk_attention_fwd_chunk): rows = sequences * heads * n, query i = row % n keeps
+ * the keys its chunk allows (always i itself).  The backward is pk_softmax_bwd.  Bad chunk arguments are refused before any launch. */
+int pk_softmax_chunk_fwd(const float* S, long long ld_s, void* P, void* Pd, int dtype, long long ld_p, long long rows, int n,
+                         int chunk_len, int chunk_off, int left_chunks, float drop_p, uint32_t seed, void* stream);
 int pk_softmax_bwd(const float* dPd, long long ld_d, const void* P, long long ld_p, void* dS, int dtype, long long rows,
                    int n, float drop_p, uint32_t seed, void* stream);
 /* Relative-position self-attention (Shaw et al.; trainer/model/modules/multi_headed_attn.py:9-41,186-229), max_rel = m > 0:

@@ -21,6 +21,12 @@
 // (pk_attention_fwd_bits / _bwd_bits): the forward alone hashes and writes each decision as one bit (layout in
 // include/pika_b200.h), and the backward reads them -- MODE 1 one word per thread and tile straight from global memory, MODE 2 the
 // transposed 64 x 128 block through the loader's ring.
+//
+// Chunk mask (template CHUNK; pk_attention_fwd_chunk / _bwd_chunk, DESIGN.md "Chunked attention"): frame t lies in chunk
+// (t + chunk_off) / chunk_len, and query i sees key j iff chunk(i) - left_chunks <= chunk(j) <= chunk(i) (left_chunks = -1: no lower
+// limit).  A row's allowed streamed indices form one interval whose ends never decrease with the row, so a CTA streams only the tiles
+// between the first row's lower end and the last row's upper end (the loader and both consumer warpgroups derive the same trip
+// count from the same rows), and the per-element mask runs only on tiles that some row of the warpgroup does not see whole.
 #include <cstdlib>
 #include <cstring>
 
@@ -58,7 +64,21 @@ struct AttnTcParams {
     int B, T, heads, Tpad, Tp2, nkb;
     float alpha;
     uint32_t thresh16; float drop_scale; uint32_t seed;
+    int chunk_len, chunk_off, left_chunks;        // CHUNK only
 };
+
+// stationary row -> its allowed streamed interval in MODE (0 / 1: keys of a query, 2: queries of a key)
+template <int MODE> PK_DEVICE int chunk_lo(const AttnTcParams& p, int r) {
+    return MODE == 2 ? chunk_query_lo(r, p.T, p.chunk_len, p.chunk_off) : chunk_key_lo(r, p.T, p.chunk_len, p.chunk_off, p.left_chunks);
+}
+template <int MODE> PK_DEVICE int chunk_hi(const AttnTcParams& p, int r) {
+    return MODE == 2 ? chunk_query_hi(r, p.T, p.chunk_len, p.chunk_off, p.left_chunks) : chunk_key_hi(r, p.T, p.chunk_len, p.chunk_off);
+}
+// the 64-wide streamed tiles [jb, je) that stationary rows [row_base, row_base + 128) of the CTA visit; never empty (a frame sees itself)
+template <int MODE> PK_DEVICE void chunk_tiles(const AttnTcParams& p, int row_base, int& jb, int& je) {
+    jb = chunk_lo<MODE>(p, row_base) / TA_BC;
+    je = (chunk_hi<MODE>(p, min(row_base + TA_BR, p.T) - 1) + TA_BC - 1) / TA_BC;
+}
 
 // A-operand fragment k-block kk (16 streamed indices) of a 64 x 64 register tile
 PK_DEVICE void frag_a(const float (&x)[32], int kk, uint32_t (&a)[4]) {
@@ -87,7 +107,7 @@ PK_DEVICE void store_tile(const float (&x)[32], __nv_bfloat16* base, long long l
 
 // DROP: TA_DROP_NONE (p = 0: no mask code at all), TA_DROP_HASH (every mode hashes the mask from the seed) or TA_DROP_BITS (MODE 0
 // hashes it and writes the keep bits, MODES 1 / 2 read them)
-template <int MODE, int DROP>
+template <int MODE, int DROP, bool CHUNK = false>
 __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __grid_constant__ AttnTcParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -101,7 +121,8 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     const int T = p.T;
     const int bh = blockIdx.y, b = bh / p.heads, h = bh - b * p.heads;
     const int row_base = blockIdx.x * TA_BR;
-    const int n_tiles = (T + TA_BC - 1) / TA_BC;
+    int j_begin = 0, j_end = (T + TA_BC - 1) / TA_BC;
+    if (CHUNK) chunk_tiles<MODE>(p, row_base, j_begin, j_end);
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.q); tma_prefetch_desc(&p.k); tma_prefetch_desc(&p.v);
@@ -129,10 +150,20 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
         constexpr bool kb_load = MODE == 2 && DROP == TA_DROP_BITS;
         int stage = 0;
         uint32_t phase = 0;
-        for (int j = 0; j < n_tiles; ++j) {
+        for (int j = j_begin; j < j_end; ++j) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* x1 = smem + TA_OFF_RING + stage * 2 * TA_TILE_X;
-            mbar_arrive_expect_tx_p(&full_bar[stage], 2 * TA_TILE_X + (MODE == 2 ? 2 * TA_BC * 4 : 0) + (kb_load ? 2 * TA_KB_BLOCK : 0), lead);
+            // CHUNK: the forward wrote the keep bits of key block 2 * blockIdx.x + half for query tile j only if the forward CTA of
+            // query rows [(j / 2) * 128, +128) visited it; a block it skipped is not read (every pair of it is masked)
+            bool kb_half[2] = {kb_load, kb_load};
+            if (CHUNK && kb_load) {
+                int qb, qe;
+                chunk_tiles<0>(p, (j >> 1) * TA_BR, qb, qe);
+                kb_half[0] = 2 * (int)blockIdx.x >= qb && 2 * (int)blockIdx.x < qe;
+                kb_half[1] = 2 * (int)blockIdx.x + 1 >= qb && 2 * (int)blockIdx.x + 1 < qe;
+            }
+            mbar_arrive_expect_tx_p(&full_bar[stage], 2 * TA_TILE_X + (MODE == 2 ? 2 * TA_BC * 4 : 0) + ((int)kb_half[0] + (int)kb_half[1]) * TA_KB_BLOCK,
+                                    lead);
             tma_load_3d_p(x1, mx1, &full_bar[stage], h * 64, j * TA_BC, b, lead);
             tma_load_3d_p(x1 + TA_TILE_X, mx2, &full_bar[stage], h * 64, j * TA_BC, b, lead);
             if (MODE == 2) {
@@ -140,9 +171,16 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
                 bulk_load_p(vec + (stage * 2 + 0) * TA_BC, p.lse + off, TA_BC * 4, &full_bar[stage], lead);
                 bulk_load_p(vec + (stage * 2 + 1) * TA_BC, p.dsum + off, TA_BC * 4, &full_bar[stage], lead);
                 // streamed query block j x the CTA's two key blocks: adjacent in the layout, so one 1 KB copy
-                if (kb_load)
+                if (kb_load && (!CHUNK || (kb_half[0] && kb_half[1])))
                     bulk_load_p(smem + TA_OFF_KB + stage * 2 * TA_KB_BLOCK, p.keep_bits + kb_block(p, bh, j, 2 * blockIdx.x), 2 * TA_KB_BLOCK,
                                 &full_bar[stage], lead);
+                else if (CHUNK && kb_load) {
+#pragma unroll
+                    for (int half = 0; half < 2; ++half)
+                        if (kb_half[half])
+                            bulk_load_p(smem + TA_OFF_KB + (stage * 2 + half) * TA_KB_BLOCK, p.keep_bits + kb_block(p, bh, j, 2 * blockIdx.x + half),
+                                        TA_KB_BLOCK, &full_bar[stage], lead);
+                }
             }
             if (++stage == TA_NST) { stage = 0; phase ^= 1; }
         }
@@ -169,9 +207,16 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     const int kb_word = (et >> 5) * 32 + (lane & 3) * 8 + (lane >> 2);
     uint32_t row_salt[2];                             // MODE 0 / 1: the probability rows are this thread's rows
     float lse2[2] = {0.f, 0.f}, dsum_r[2] = {0.f, 0.f};
+    int c_lo[2] = {0, 0}, c_hi[2] = {0, 0};           // CHUNK: allowed streamed interval of this thread's rows
+    int wg_lo = 0, wg_hi = 0;                         // CHUNK: tiles inside [wg_lo, wg_hi) are seen whole by every row of the warpgroup
+    if (CHUNK) {
+        wg_lo = chunk_lo<MODE>(p, srow0 + 63);
+        wg_hi = chunk_hi<MODE>(p, srow0);
+    }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
         const int srow = srow0 + r0 + 8 * hh;
+        if (CHUNK) { c_lo[hh] = chunk_lo<MODE>(p, srow); c_hi[hh] = chunk_hi<MODE>(p, srow); }
         if (MODE == 0 || (MODE == 1 && !KB)) row_salt[hh] = drop_row_salt(stat_row0 + (uint64_t)srow, p.seed);
         if (MODE == 1 && srow < T) {
             lse2[hh] = p.lse[(size_t)bh * p.Tpad + srow] * TA_LOG2E;
@@ -188,7 +233,7 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     if (MODE == 0) {
         int stage = 0;
         uint32_t phase = 0;
-        for (int j = 0; j < n_tiles; ++j) {
+        for (int j = j_begin; j < j_end; ++j) {
             const int col0 = j * TA_BC;
             const int nvalid = min(TA_BC, T - col0);  // streamed indices of this tile inside the sequence
             mbar_wait(&full_bar[stage], phase);
@@ -201,7 +246,15 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
             wgmma_commit();
             wgmma_wait<0>();
             wgmma_fence_acc(s);
-            if (nvalid < TA_BC) {                     // last tile only (uniform): keys beyond the sequence get probability 0
+            if (CHUNK) {
+                if (col0 < wg_lo || col0 + TA_BC > wg_hi) {   // uniform; covers the keys beyond the sequence too (c_hi <= T)
+#pragma unroll
+                    for (int c = 0; c < 32; ++c) {
+                        const int col = col0 + (c >> 2) * 8 + cq + (c & 1);
+                        if (col < c_lo[(c >> 1) & 1] || col >= c_hi[(c >> 1) & 1]) s[c] = -INFINITY;
+                    }
+                }
+            } else if (nvalid < TA_BC) {              // last tile only (uniform): keys beyond the sequence get probability 0
 #pragma unroll
                 for (int c = 0; c < 32; ++c) if ((c >> 2) * 8 + cq + (c & 1) >= nvalid) s[c] = -INFINITY;
             }
@@ -212,14 +265,17 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
                 float mx = -INFINITY;
 #pragma unroll
                 for (int nb = 0; nb < 8; ++nb) mx = fmaxf(mx, fmaxf(s[nb * 4 + 2 * hh], s[nb * 4 + 2 * hh + 1]));
-                const float m_new = fmaxf(m_run[hh], quad_max(mx) * c2);   // finite: every tile holds a valid column
-                corr[hh] = ex2_approx(m_run[hh] - m_new);                    // 0 on the first tile
+                const float m_new = fmaxf(m_run[hh], quad_max(mx) * c2);   // finite unless CHUNK: every tile holds a valid column
+                // CHUNK: a row that has seen only masked keys keeps m = -inf; its exponents use 0 instead, so that no
+                // exp(-inf - (-inf)) is formed (its probabilities and corr are then exactly 0)
+                const float m_use = (CHUNK && m_new == -INFINITY) ? 0.f : m_new;
+                corr[hh] = ex2_approx(m_run[hh] - m_use);                    // 0 on the first tile
                 float sum = 0.f;
 #pragma unroll
                 for (int nb = 0; nb < 8; ++nb) {
                     float* pr = &s[nb * 4 + 2 * hh];
-                    pr[0] = ex2_approx(fmaf(pr[0], c2, -m_new));
-                    pr[1] = ex2_approx(fmaf(pr[1], c2, -m_new));
+                    pr[0] = ex2_approx(fmaf(pr[0], c2, -m_use));
+                    pr[1] = ex2_approx(fmaf(pr[1], c2, -m_use));
                     sum += pr[0] + pr[1];
                     if (use_drop) {
                         const uint32_t km = drop_pair(row_salt[hh], (uint32_t)((col0 + nb * 8 + cq) >> 1), p.thresh16);
@@ -252,8 +308,9 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
     } else {
         int stage = 0;
         uint32_t phase = 0;
-        for (int j = 0; j < n_tiles; ++j) {
+        for (int j = j_begin; j < j_end; ++j) {
             const int col0 = j * TA_BC;
+            const bool part = CHUNK && (col0 < wg_lo || col0 + TA_BC > wg_hi);   // uniform: some pair of the tile is masked
             uint32_t kw = 0u;                             // MODE 1: keep bits of this tile, loaded under the wgmma below
             if (MODE == 1 && KB && use_drop) kw = __ldg(p.keep_bits + kb_block(p, bh, 2 * blockIdx.x + wg, j) + kb_word);
             mbar_wait(&full_bar[stage], phase);
@@ -319,7 +376,8 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
                             const int cl = nb * 8 + cq + e;           // streamed index inside the tile
                             const float l2 = (MODE == 1) ? lse2[hh] : lse_t[cl] * TA_LOG2E;
                             const float dd = (MODE == 1) ? dsum_r[hh] : dsum_t[cl];
-                            const float pr = ex2_approx(fmaf(s[c], c2, -l2));
+                            float pr = ex2_approx(fmaf(s[c], c2, -l2));
+                            if (CHUNK && part && (col0 + cl < c_lo[hh] || col0 + cl >= c_hi[hh])) pr = 0.f;
                             const bool kp = (keep >> e) & 1u;
                             const float dpe = kp ? dp[c] * p.drop_scale : 0.f;
                             ds[c] = pr * (dpe - dd);
@@ -361,7 +419,8 @@ __global__ void __launch_bounds__(TA_THREADS, 1) attention_tc_kernel(const __gri
             const int srow = srow0 + r0 + 8 * hh;
             // rows in [T, Tpad) (zero queries: lse = ln(T)) are written too, so that the dK/dV mode, which streams whole 64-query
             // tiles of lse, never reads a value the caller left there (a NaN would reach dK / dV through 0 * NaN)
-            if ((lane & 3) == 0 && srow < p.Tpad) p.lse[(size_t)bh * p.Tpad + srow] = (m_run[hh] + log2f(l)) * TA_LN2;
+            // CHUNK: a padding row may see no key at all (l = 0); its lse is written as 0 (the backward masks it)
+            if ((lane & 3) == 0 && srow < p.Tpad) p.lse[(size_t)bh * p.Tpad + srow] = (CHUNK && l == 0.f) ? 0.f : (m_run[hh] + log2f(l)) * TA_LN2;
         }
 #pragma unroll
         for (int c = 0; c < 32; ++c) acc0[c] *= inv[(c >> 1) & 1];
@@ -411,8 +470,8 @@ static int attn_maps(AttnTcParams& p, const void* q, const void* k, const void* 
     return 0;
 }
 
-template <int MODE, int DROP> static int launch_attn_drop(const AttnTcParams& p, cudaStream_t st) {
-    auto kern = attention_tc_kernel<MODE, DROP>;
+template <int MODE, int DROP, bool CHUNK> static int launch_attn_drop(const AttnTcParams& p, cudaStream_t st) {
+    auto kern = attention_tc_kernel<MODE, DROP, CHUNK>;
     static bool configured = false;
     if (!configured) {
         PK_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TA_SMEM));
@@ -424,8 +483,12 @@ template <int MODE, int DROP> static int launch_attn_drop(const AttnTcParams& p,
     return 0;
 }
 template <int MODE> static int launch_attn(const AttnTcParams& p, cudaStream_t st) {
-    if (p.thresh16 == 0u) return launch_attn_drop<MODE, TA_DROP_NONE>(p, st);
-    return p.keep_bits ? launch_attn_drop<MODE, TA_DROP_BITS>(p, st) : launch_attn_drop<MODE, TA_DROP_HASH>(p, st);
+    if (p.chunk_len > 0) {                        // chunk mask: keep-bits form only
+        if (p.thresh16 == 0u) return launch_attn_drop<MODE, TA_DROP_NONE, true>(p, st);
+        return launch_attn_drop<MODE, TA_DROP_BITS, true>(p, st);
+    }
+    if (p.thresh16 == 0u) return launch_attn_drop<MODE, TA_DROP_NONE, false>(p, st);
+    return p.keep_bits ? launch_attn_drop<MODE, TA_DROP_BITS, false>(p, st) : launch_attn_drop<MODE, TA_DROP_HASH, false>(p, st);
 }
 
 }  // namespace pk
@@ -449,8 +512,20 @@ extern "C" long long pk_attention_keep_bits_bytes(int B, int T, int heads) {
     PK_CHECK_ARG(drop_p == 0.f || (keep_bits != nullptr && ((uintptr_t)keep_bits & 15) == 0),                               \
                  "keep_bits must be a 16-byte aligned buffer of pk_attention_keep_bits_bytes when drop_p > 0")
 
+#define CHUNK_CHECKS()                                                                                                     \
+    PK_CHECK_ARG(chunk_len >= 1 && chunk_off >= 0 && left_chunks >= -1, "chunk mask: chunk_len >= 1, chunk_off >= 0, left_chunks >= -1")
+
+/* 1 when the chunk mask (chunk_len, chunk_off, left_chunks) lets every query of a T-frame sequence see every key: the last query's
+   lowest key is 0 and the first query's highest key is T - 1 (both ends are monotone in the query) */
+extern "C" int pk_attention_chunk_admits_all(int T, int chunk_len, int chunk_off, int left_chunks) {
+    CHUNK_CHECKS();
+    PK_CHECK_ARG(T > 0, "bad dims");
+    return pk::chunk_key_lo(T - 1, T, chunk_len, chunk_off, left_chunks) == 0 && pk::chunk_key_hi(0, T, chunk_len, chunk_off) == T;
+}
+
 static int attention_fwd(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
-                         int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits, void* stream) {
+                         int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits, void* stream,
+                         int chunk_len = 0, int chunk_off = 0, int left_chunks = -1) {
     using namespace pk;
     ATTN_CHECKS();
     static thread_local AttnTcParams p;
@@ -460,6 +535,7 @@ static int attention_fwd(const void* q, const void* k, const void* v, long long 
     int rc = attn_maps(p, q, k, v, ld_qkv, nullptr, 0);
     if (rc) return rc;
     p.out = (__nv_bfloat16*)out; p.ld_o = ld_out; p.lse = lse;
+    p.chunk_len = chunk_len; p.chunk_off = chunk_off; p.left_chunks = left_chunks;
     p.alpha = alpha;
     p.thresh16 = drop_thresh16_of(drop_p); p.drop_scale = drop_scale16_of(p.thresh16); p.seed = seed;
     return launch_attn<0>(p, STREAM(stream));
@@ -471,7 +547,7 @@ static int attention_fwd(const void* q, const void* k, const void* v, long long 
 static int attention_bwd(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
                          const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
                          long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed,
-                         const uint32_t* keep_bits, void* stream) {
+                         const uint32_t* keep_bits, void* stream, int chunk_len = 0, int chunk_off = 0, int left_chunks = -1) {
     using namespace pk;
     ATTN_CHECKS();
     PK_CHECK_ARG(ld_dout % 8 == 0 && ld_dqkv % 8 == 0, "row strides must be multiples of 8 elements (16 bytes)");
@@ -483,6 +559,7 @@ static int attention_bwd(const void* q, const void* k, const void* v, long long 
     if (rc) return rc;
     p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv; p.ld_dqkv = ld_dqkv;
     p.lse = const_cast<float*>(lse); p.dsum = dsum_ws;
+    p.chunk_len = chunk_len; p.chunk_off = chunk_off; p.left_chunks = left_chunks;
     p.alpha = alpha;
     p.thresh16 = drop_thresh16_of(drop_p); p.drop_scale = drop_scale16_of(p.thresh16); p.seed = seed;
     const long long n = (long long)B * T * heads;
@@ -519,4 +596,27 @@ extern "C" int pk_attention_bwd_bits(const void* q, const void* k, const void* v
     KEEP_BITS_CHECK();
     return attention_bwd(q, k, v, ld_qkv, out, ld_out, dout, ld_dout, lse, dsum_ws, dq, dk, dv, ld_dqkv, B, T, heads, dh, alpha, drop_p, 0u,
                          keep_bits, stream);
+}
+
+/* chunk-masked forms; a mask that admits every key runs the unmasked kernels */
+extern "C" int pk_attention_fwd_chunk(const void* q, const void* k, const void* v, long long ld_qkv, void* out, long long ld_out, float* lse,
+                                      int B, int T, int heads, int dh, float alpha, float drop_p, uint32_t seed, uint32_t* keep_bits,
+                                      int chunk_len, int chunk_off, int left_chunks, void* stream) {
+    CHUNK_CHECKS();
+    KEEP_BITS_CHECK();
+    ATTN_CHECKS();
+    if (pk_attention_chunk_admits_all(T, chunk_len, chunk_off, left_chunks)) chunk_len = 0;
+    return attention_fwd(q, k, v, ld_qkv, out, ld_out, lse, B, T, heads, dh, alpha, drop_p, seed, keep_bits, stream, chunk_len, chunk_off,
+                         left_chunks);
+}
+extern "C" int pk_attention_bwd_chunk(const void* q, const void* k, const void* v, long long ld_qkv, const void* out, long long ld_out,
+                                      const void* dout, long long ld_dout, const float* lse, float* dsum_ws, void* dq, void* dk, void* dv,
+                                      long long ld_dqkv, int B, int T, int heads, int dh, float alpha, float drop_p, const uint32_t* keep_bits,
+                                      int chunk_len, int chunk_off, int left_chunks, void* stream) {
+    CHUNK_CHECKS();
+    KEEP_BITS_CHECK();
+    ATTN_CHECKS();
+    if (pk_attention_chunk_admits_all(T, chunk_len, chunk_off, left_chunks)) chunk_len = 0;
+    return attention_bwd(q, k, v, ld_qkv, out, ld_out, dout, ld_dout, lse, dsum_ws, dq, dk, dv, ld_dqkv, B, T, heads, dh, alpha, drop_p, 0u,
+                         keep_bits, stream, chunk_len, chunk_off, left_chunks);
 }

@@ -99,6 +99,19 @@ __host__ __device__ inline uint32_t drop_thresh16_of(float p) {
 }
 __host__ __device__ inline float drop_scale16_of(uint32_t thresh16) { return thresh16 ? 1.f / (1.f - (float)thresh16 / 65536.f) : 1.f; }
 
+// Chunk mask of streaming self-attention (DESIGN.md "Chunked attention"): frame t lies in chunk (t + off) / len, and query i sees key j
+// iff chunk(i) - left <= chunk(j) <= chunk(i) (left = -1: no lower limit).  Allowed keys [lo, hi) of query i and allowed queries
+// [lo, hi) of key j, clipped to [0, T); each end is monotone in i (j).
+__host__ __device__ inline int chunk_clip(long long v, int T) { return (int)(v < 0 ? 0 : v > T ? T : v); }
+__host__ __device__ inline int chunk_key_lo(int i, int T, int len, int off, int left) {
+    return left < 0 ? 0 : chunk_clip(((long long)((i + (long long)off) / len) - left) * len - off, T);
+}
+__host__ __device__ inline int chunk_key_hi(int i, int T, int len, int off) { return chunk_clip(((i + (long long)off) / len + 1) * len - off, T); }
+__host__ __device__ inline int chunk_query_lo(int j, int T, int len, int off) { return chunk_clip((j + (long long)off) / len * len - off, T); }
+__host__ __device__ inline int chunk_query_hi(int j, int T, int len, int off, int left) {
+    return left < 0 ? T : chunk_clip(((j + (long long)off) / len + left + 1) * len - off, T);
+}
+
 PK_DEVICE float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -451,15 +451,18 @@ PK_DEVICE void ld8f(const float* p, float (&f)[8]) {
     const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
     f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
-template <typename T, int SM_CH>
+template <typename T, int SM_CH, bool CHUNK = false>
 __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restrict__ S, long long ld_s, T* __restrict__ P,
                                                           T* __restrict__ Pd, long long ld_p, long long rows, int n,
                                                           uint32_t drop_thresh, float drop_scale, uint32_t seed, int q_len = 0,
-                                                          int heads = 1, int causal = 0, const uint8_t* __restrict__ key_pad = nullptr) {
+                                                          int heads = 1, int causal = 0, const uint8_t* __restrict__ key_pad = nullptr,
+                                                          int chunk_len = 1, int chunk_off = 0, int left_chunks = -1) {
     // masked form (q_len > 0; the transformer prediction net, trainer/model/rnnt_conv_transformer_lm.py:66-70): row r is query
     // i = r % q_len of sequence r / (heads * q_len); key c is dropped when c > i (causal) or key_pad[seq, c] != 0.  A dropped score
     // becomes -inf where the reference fills -1e18 (multi_headed_attn.py:214-216): both give probability exactly 0 as long as one key
     // survives, which the causal diagonal guarantees.
+    // CHUNK (pk_softmax_chunk_fwd; q_len = n, self-attention): query i keeps the keys [chunk_key_lo, chunk_key_hi) of the chunk mask
+    // (common.cuh), which always hold i itself.
     const int lane = threadIdx.x & 31;
     const long long warp = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
@@ -467,9 +470,13 @@ __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restric
         const float* sr = S + r * ld_s;
         float v[SM_CH][8];
         float m = -INFINITY;
-        int lim = n;
+        int lim = n, lo = 0;
         const uint8_t* kp = nullptr;
-        if (q_len > 0) {
+        if (CHUNK) {
+            const int i = (int)(r % q_len);
+            lo = chunk_key_lo(i, n, chunk_len, chunk_off, left_chunks);
+            lim = chunk_key_hi(i, n, chunk_len, chunk_off);
+        } else if (q_len > 0) {
             if (causal) lim = min(n, (int)(r % q_len) + 1);
             if (key_pad) kp = key_pad + (r / ((long long)heads * q_len)) * n;
         }
@@ -479,7 +486,7 @@ __global__ void __launch_bounds__(256) softmax_fwd_kernel(const float* __restric
             if (c0 < (int)ld_p) ld8f(sr + c0, v[k]);
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
-                if (c0 + e >= lim || (kp && kp[c0 + e])) v[k][e] = -INFINITY;
+                if (c0 + e >= lim || (CHUNK && c0 + e < lo) || (kp && kp[c0 + e])) v[k][e] = -INFINITY;
                 m = fmaxf(m, v[k][e]);
             }
         }
@@ -1326,6 +1333,18 @@ extern "C" int pk_softmax_masked_fwd(const float* S, long long ld_s, void* P, vo
     const float sc = drop_scale16_of(th);
     if (ld_p <= 1024) { PK_DISPATCH_T(dtype, (softmax_fwd_kernel<T, 4><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, q_len, heads, causal, key_pad))); }
     else { PK_DISPATCH_T(dtype, (softmax_fwd_kernel<T, 8><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, q_len, heads, causal, key_pad))); }
+    DONE();
+}
+extern "C" int pk_softmax_chunk_fwd(const float* S, long long ld_s, void* P, void* Pd, int dtype, long long ld_p, long long rows, int n,
+                                    int chunk_len, int chunk_off, int left_chunks, float drop_p, uint32_t seed, void* stream) {
+    PK_CHECK_ARG(rows > 0 && n > 0 && ld_p >= n && ld_s >= ld_p && ld_p <= 2048 && ld_p % 8 == 0 && ld_s % 8 == 0, "softmax rows: ld % 8 == 0, <= 2048 wide");
+    PK_CHECK_ARG(rows % n == 0, "chunked softmax: rows = sequences * heads * n");
+    PK_CHECK_ARG(chunk_len >= 1 && chunk_off >= 0 && left_chunks >= -1, "chunk mask: chunk_len >= 1, chunk_off >= 0, left_chunks >= -1");
+    const int grid = grid_for(rows, 8);
+    const uint32_t th = drop_thresh16_of(drop_p);
+    const float sc = drop_scale16_of(th);
+    if (ld_p <= 1024) { PK_DISPATCH_T(dtype, (softmax_fwd_kernel<T, 4, true><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, n, 1, 0, nullptr, chunk_len, chunk_off, left_chunks))); }
+    else { PK_DISPATCH_T(dtype, (softmax_fwd_kernel<T, 8, true><<<grid, 256, 0, STREAM(stream)>>>(S, ld_s, (T*)P, (T*)Pd, ld_p, rows, n, th, sc, seed, n, 1, 0, nullptr, chunk_len, chunk_off, left_chunks))); }
     DONE();
 }
 extern "C" int pk_softmax_bwd(const float* dPd, long long ld_d, const void* P, long long ld_p, void* dS, int dtype, long long rows,

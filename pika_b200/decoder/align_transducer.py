@@ -19,7 +19,7 @@ import sys
 
 import torch
 
-from .decode_transducer import load_cmvn, prepare_batch, read_symbols_map
+from .decode_transducer import add_chunk_args, apply_chunk_args, load_cmvn, prepare_batch, read_symbols_map
 
 
 def build_parser():
@@ -43,6 +43,7 @@ def build_parser():
                    help='align in the pruned lattice: R >= 2 label positions per frame chosen by the simple joiner (0: dense)')
     p.add_argument('--frame_shift_ms', type=float, default=10.0, help='frame shift of the features in milliseconds')
     p.add_argument('--scores', type=str, default=None, help="write 'uttid T' U viterbi loglik viterbi/T'' lines to this file")
+    add_chunk_args(p)
     return p
 
 
@@ -81,6 +82,7 @@ def main(argv=None):
     torch.cuda.set_device(dev)
     engine.set_precision(args.precision)
     model = torch.load(args.model, map_location="cpu", weights_only=False)
+    apply_chunk_args(parser, args, model)
     model.eval().to(dev)
     if args.prune_range and not hasattr(model, "simple_am_proj"):
         sys.exit("pika_b200.decoder.align_transducer: --prune_range needs a model trained with the pruned loss (simple_am_proj)")

@@ -60,7 +60,31 @@ def build_parser():
     p.add_argument('--model_lctx', type=int, default=0, help='model left context')
     p.add_argument('--model_rctx', type=int, default=0, help='model right context')
     p.add_argument('--model_stride', type=int, default=1, help='model stride, ie., subsampling in the model')
+    add_chunk_args(p)
     return p
+
+
+def add_chunk_args(p):
+    """--chunk_size / --left_chunks: override the TDNN-Transformer encoder's chunk setting (DESIGN.md "Chunked attention")"""
+    p.add_argument('--chunk_size', type=int, default=None,
+                   help='run the encoder with self-attention limited to chunks of this many output frames; 0 = full context; '
+                        'default: as trained')
+    p.add_argument('--left_chunks', type=int, default=None, help='earlier chunks a frame may attend to (-1 = all); default: as trained')
+
+
+def apply_chunk_args(parser, args, model):
+    """sets the model encoder's chunk_size / left_chunks from the flags that were given; parser.error when they are out of range or
+    the model's encoder cannot be chunked"""
+    if args.chunk_size is None and args.left_chunks is None:
+        return
+    if (args.chunk_size is not None and args.chunk_size < 0) or (args.left_chunks is not None and args.left_chunks < -1):
+        parser.error('--chunk_size must be >= 0 and --left_chunks >= -1')
+    if not hasattr(model.encoder, 'chunk_masks'):
+        parser.error('--chunk_size / --left_chunks apply to the TDNN-Transformer encoder only')
+    if args.chunk_size is not None:
+        model.encoder.chunk_size = args.chunk_size
+    if args.left_chunks is not None:
+        model.encoder.left_chunks = args.left_chunks
 
 
 def load_cmvn(args, dev):
@@ -116,6 +140,7 @@ def main(argv=None):
     torch.cuda.set_device(dev)
 
     model = torch.load(args.model, map_location="cpu", weights_only=False)                # :19-20
+    apply_chunk_args(parser, args, model)
     model.eval().to(dev)
     for name in ("las_rescorer", "las_rescorer_bw", "bilas_rescorer"):                      # :22-38
         path = getattr(args, name + "_model")

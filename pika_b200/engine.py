@@ -443,15 +443,19 @@ class AttentionFn(torch.autograd.Function):
     186-229), shared by the key and the value relations; it always takes the materialised path.  The band kernels
     (pk_softmax_masked_relpos_fwd / pk_softmax_relpos_bwd) add QR = (alpha Q) R^T to the scores and reduce Pd / dS onto the 2m+1
     buckets (Pb / dSb, token-major rows); the rest is GEMMs: out += Pb R, G = dO R^T, dQ += alpha dSb R, dR = dSb^T (alpha Q) + Pb^T dO.
-    dR is written into ``grad_of(rel)`` (the engine's gradient contract), so no gradient is returned for it."""
+    dR is written into ``grad_of(rel)`` (the engine's gradient contract), so no gradient is returned for it.
+    ``chunk`` = (chunk_len, chunk_off, left_chunks): the streaming encoder's chunk mask (DESIGN.md "Chunked attention"), on the fused
+    kernels' chunk instantiations (head dim 64, bf16) or the chunk-masked softmax; not combined with the other masks."""
 
     @staticmethod
-    def forward(ctx, qkv, heads, drop_p, seed, causal=False, key_pad=None, rel=None):
+    def forward(ctx, qkv, heads, drop_p, seed, causal=False, key_pad=None, rel=None, chunk=None):
         B, T, D3 = qkv.shape
         D = D3 // 3
         dh = D // heads
         masked = causal or key_pad is not None
-        ctx.rel = rel
+        if chunk is not None and (masked or rel is not None):
+            raise NotImplementedError("pika_b200: the chunk mask does not combine with causal / key_pad / relative positions")
+        ctx.rel, ctx.chunk = rel, chunk
         ctx.fused = _FUSED_ATTN and qkv.dtype == torch.bfloat16 and dh == 64 and not masked and rel is None
         if ctx.fused:
             # scores / probabilities never leave the SM (pika_b200/csrc/attention_tc.cu)
@@ -460,7 +464,7 @@ class AttentionFn(torch.autograd.Function):
             lse = torch.zeros(B * heads * K.attention_lse_stride(T), dtype=torch.float32, device=qkv.device)   # pad entries finite
             alpha = 1.0 / math.sqrt(dh)
             keep_bits = K.attention_keep_bits(B, T, heads, drop_p, qkv.device)   # dropout decisions, for the backward
-            K.attention_fwd(qkv, out, lse, heads, alpha, drop_p, seed, keep_bits=keep_bits)
+            K.attention_fwd(qkv, out, lse, heads, alpha, drop_p, seed, keep_bits=keep_bits, chunk=chunk)
             ctx.save_for_backward(qkv, out, lse, keep_bits)
             ctx.meta = (B, T, D, heads, dh, 0, drop_p, seed, alpha)
             return out
@@ -496,6 +500,8 @@ class AttentionFn(torch.autograd.Function):
             ctx.r_parts, ctx.qc, ctx.pb_parts = r_parts, qc, pb_parts
         elif masked:
             K.softmax_masked_fwd(S, P, Pd, T, T, heads, causal, key_pad, drop_p, seed)
+        elif chunk is not None:
+            K.softmax_chunk_fwd(S, P, Pd, T, chunk, drop_p, seed)
         else:
             K.softmax_fwd(S, P, Pd, T, drop_p, seed)
         del S
@@ -513,8 +519,8 @@ class AttentionFn(torch.autograd.Function):
             qkv, out, lse, keep_bits = ctx.saved_tensors
             B, T, D, heads, dh, _, drop_p, seed, alpha = ctx.meta
             dqkv = torch.empty_like(qkv)
-            K.attention_bwd(qkv, out, dout.contiguous(), lse, dqkv, heads, alpha, drop_p, seed, keep_bits=keep_bits)
-            return dqkv, None, None, None, None, None, None
+            K.attention_bwd(qkv, out, dout.contiguous(), lse, dqkv, heads, alpha, drop_p, seed, keep_bits=keep_bits, chunk=ctx.chunk)
+            return dqkv, None, None, None, None, None, None, None
         qkv, P = ctx.saved_tensors
         B, T, D, heads, dh, Tp, drop_p, seed, alpha = ctx.meta
         dout = dout.contiguous()
@@ -554,7 +560,7 @@ class AttentionFn(torch.autograd.Function):
         # dQ = alpha * dS K ; dK = alpha * dS^T Q
         gemm_parts([ds_parts], [k], head_view(dqkv, 0), b_mn=True, alpha=alpha, **rel_dq)
         gemm_parts([ds_parts], [q], head_view(dqkv, 1), a_mn=True, b_mn=True, alpha=alpha)
-        return dqkv, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None
 
 
 class EmbeddingFn(torch.autograd.Function):
@@ -985,16 +991,18 @@ def _to_act(x):
     return x.float()
 
 
-def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None):
-    """x2 [B*T, D] -> [B*T, D]   (pre-LN attention block + position-wise FFN); ``causal`` / ``key_pad`` and the layer's relative-position
-    table (when it has one): see AttentionFn."""
+def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None, chunk=None):
+    """x2 [B*T, D] -> [B*T, D]   (pre-LN attention block + position-wise FFN); ``causal`` / ``key_pad``, ``chunk`` and the layer's
+    relative-position table (when it has one): see AttentionFn.  A chunk mask that admits every key runs the unmasked path."""
+    if chunk is not None and K.attention_chunk_admits_all(T, chunk):
+        chunk = None
     att, ff = layer.self_attn, layer.feed_forward
     p = _drop(layer.dropout_p, training)
     ln = LayerNormFn.apply(x2, layer.layer_norm, layer.layer_norm.weight, layer.layer_norm.bias)
     qkv = linear(ln, [att.linear_query.weight, att.linear_keys.weight, att.linear_values.weight],
                  [att.linear_query.bias, att.linear_keys.bias, att.linear_values.bias])
     rel = att.relative_positions_embeddings.weight if getattr(att, "max_relative_positions", 0) > 0 else None
-    ctxv = AttentionFn.apply(qkv.view(B, T, -1), att.head_count, p, _next_seed() if p > 0 else 0, causal, key_pad, rel)
+    ctxv = AttentionFn.apply(qkv.view(B, T, -1), att.head_count, p, _next_seed() if p > 0 else 0, causal, key_pad, rel, chunk)
     h1 = linear(ctxv.view(B * T, -1), att.final_linear.weight, att.final_linear.bias, drop_p=p, residual=x2)
     ln2 = LayerNormFn.apply(h1, ff.layer_norm, ff.layer_norm.weight, ff.layer_norm.bias)
     fold = ln2.dtype == torch.bfloat16
@@ -1006,7 +1014,8 @@ def transformer_layer(layer, x2, B, T, training, causal=False, key_pad=None):
 
 def encoder_forward_act(enc, x, x_len=None, t_out=None):
     """x [B,T,D] -> [B,T',H] in the activation dtype.  An nn.LSTM encoder runs over the packed lengths ``x_len`` (see
-    lstm_encoder_forward_act); the TDNN-Transformer encoder ignores them, as the reference does (pack_seq is False)."""
+    lstm_encoder_forward_act); the TDNN-Transformer encoder ignores them, as the reference does (pack_seq is False).  Its attention
+    layers run under the chunk masks of ``enc.chunk_size`` / ``enc.left_chunks`` (Net.chunk_masks; full context at chunk_size 0)."""
     if isinstance(enc, torch.nn.LSTM):
         return lstm_encoder_forward_act(enc, x, x_len, t_out)
     training = enc.training
@@ -1014,6 +1023,7 @@ def encoder_forward_act(enc, x, x_len=None, t_out=None):
     C = enc.tdnn_nhid
     if T < 43:
         raise ValueError("encoder input has %d frames; the TDNN stack needs at least 43 (receptive field 21+1+21)" % T)
+    chunks = enc.chunk_masks()
     # ReLU masks ride in the BatchNorm backward (pk_bn_bwd relu_mask) instead of separate passes
     h = linear(_to_act(x).view(B * T, D), enc.fc_in.weight, enc.fc_in.bias, act=True, premasked=True)
     h = BatchNormFn.apply(h, enc.bn_in, training, enc.bn_in.weight, enc.bn_in.bias, True)
@@ -1023,7 +1033,7 @@ def encoder_forward_act(enc, x, x_len=None, t_out=None):
         T = h3.shape[1]
         h = BatchNormFn.apply(h3.view(B * T, C), bn, training, bn.weight, bn.bias, True)
         if (l + 1) % 3 == 0:
-            h = transformer_layer(enc.transformer[l // 3], h, B, T, training)
+            h = transformer_layer(enc.transformer[l // 3], h, B, T, training, chunk=chunks[l // 3])
     h = BatchNormFn.apply(h, enc.bn_final, training, enc.bn_final.weight, enc.bn_final.bias)
     h = linear(h, enc.fc_out.weight, enc.fc_out.bias)
     return h.view(B, T, -1)

@@ -205,15 +205,26 @@ def attention_keep_bits(B, T, heads, drop_p, device):
     return torch.empty(int(lib.pk_attention_keep_bits_bytes(B, T, heads)) // 4, dtype=torch.int32, device=device)
 
 
-def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0, keep_bits=None):
+def attention_chunk_admits_all(T, chunk):
+    """True when the chunk mask ``chunk`` = (chunk_len, chunk_off, left_chunks) lets every query of a T-frame sequence see every key"""
+    rc = int(lib.pk_attention_chunk_admits_all(T, *chunk))
+    check(min(rc, 0), "pk_attention_chunk_admits_all")
+    return rc == 1
+
+
+def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0, keep_bits=None, chunk=None):
     """qkv [B,T,3D] bf16 (q | k | v column blocks) -> out [B,T,D], lse [B*heads*T] f32 (fused attention, head dim 64).
-    keep_bits (attention_keep_bits): also write the dropout decisions there, for attention_bwd to read."""
+    keep_bits (attention_keep_bits): also write the dropout decisions there, for attention_bwd to read.  chunk = (chunk_len,
+    chunk_off, left_chunks): the chunk mask of pk_attention_fwd_chunk (keep_bits then needed whenever drop_p > 0)."""
     B, T, D3 = qkv.shape
     D = D3 // 3
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and out.is_contiguous() and out.shape == (B, T, D)
     assert lse.dtype == torch.float32 and lse.numel() == B * heads * attention_lse_stride(T)
     base, es = qkv.data_ptr(), 2
     args = (base, base + D * es, base + 2 * D * es, D3, _P(out), D, _P(lse), B, T, heads, D // heads, alpha, drop_p, seed & 0xFFFFFFFF)
+    if chunk is not None:
+        check(lib.pk_attention_fwd_chunk(*args, _P(keep_bits), *chunk, _stream()), "pk_attention_fwd_chunk")
+        return
     if keep_bits is None:
         check(lib.pk_attention_fwd(*args, _stream()), "pk_attention_fwd")
         return
@@ -221,8 +232,9 @@ def attention_fwd(qkv, out, lse, heads, alpha, drop_p=0.0, seed=0, keep_bits=Non
     check(lib.pk_attention_fwd_bits(*args, _P(keep_bits), _stream()), "pk_attention_fwd_bits")
 
 
-def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0, keep_bits=None):
-    """dqkv <- gradient of attention_fwd; with keep_bits (the forward's) the mask is read from them, otherwise drawn from seed"""
+def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0, keep_bits=None, chunk=None):
+    """dqkv <- gradient of attention_fwd; with keep_bits (the forward's) the mask is read from them, otherwise drawn from seed.
+    chunk: the forward's chunk mask (pk_attention_bwd_chunk; reads keep_bits)."""
     B, T, D3 = qkv.shape
     D = D3 // 3
     assert dout.is_contiguous() and dqkv.is_contiguous() and dqkv.shape == qkv.shape and dout.dtype == torch.bfloat16
@@ -230,7 +242,9 @@ def attention_bwd(qkv, out, dout, lse, dqkv, heads, alpha, drop_p=0.0, seed=0, k
     base, gb, es = qkv.data_ptr(), dqkv.data_ptr(), 2
     args = (base, base + D * es, base + 2 * D * es, D3, _P(out), D, _P(dout), D, _P(lse), _P(ws),
             gb, gb + D * es, gb + 2 * D * es, D3, B, T, heads, D // heads, alpha, drop_p)
-    if keep_bits is None:
+    if chunk is not None:
+        check(lib.pk_attention_bwd_chunk(*args, _P(keep_bits), *chunk, _stream()), "pk_attention_bwd_chunk")
+    elif keep_bits is None:
         check(lib.pk_attention_bwd(*args, seed & 0xFFFFFFFF, _stream()), "pk_attention_bwd")
     else:
         check(lib.pk_attention_bwd_bits(*args, _P(keep_bits), _stream()), "pk_attention_bwd_bits")
@@ -290,6 +304,14 @@ def softmax_masked_fwd(S, P, Pd, n, q_len, heads, causal, key_pad, drop_p, seed)
         assert key_pad.dtype == torch.uint8 and key_pad.is_contiguous() and key_pad.shape[-1] == n
     check(lib.pk_softmax_masked_fwd(_P(S), S.shape[-1], _P(P), _P(Pd), _dt(P), P.shape[-1], rows, n, q_len, heads, int(bool(causal)),
                                     _P(key_pad), drop_p, seed & 0xFFFFFFFF, _stream()), "pk_softmax_masked_fwd")
+
+
+def softmax_chunk_fwd(S, P, Pd, n, chunk, drop_p, seed):
+    """rows of S = (sequence, head, query i < n); query i keeps the keys its chunk allows (chunk = (chunk_len, chunk_off, left_chunks),
+    the mask of pk_attention_fwd_chunk)"""
+    rows = S.numel() // S.shape[-1]
+    check(lib.pk_softmax_chunk_fwd(_P(S), S.shape[-1], _P(P), _P(Pd), _dt(P), P.shape[-1], rows, n, *chunk, drop_p, seed & 0xFFFFFFFF,
+                                   _stream()), "pk_softmax_chunk_fwd")
 
 
 def softmax_bwd(dPd, P, dS, n, drop_p, seed):

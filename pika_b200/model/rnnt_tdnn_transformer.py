@@ -7,6 +7,8 @@ that a seeded construction yields the reference's initial weights bit for bit.  
 live in ordinary torch containers; ``forward`` runs on the hand-written sm_90a kernels
 (pika_b200/engine.py) -- there is no torch-op compute path.
 """
+import math
+
 import torch.nn as nn
 
 
@@ -60,6 +62,10 @@ class Net(nn.Module):
     TDNN_DIL_STRIDE = [(1, 1)] * 3 + [(3, 1)] * 5 + [(3, 4)]
     HEADS = [16, 16, 8]
     XF_DROPOUT = 0.2        # hard-wired in the reference (:65)
+    # streaming (DESIGN.md "Chunked attention"): chunk width in output frames (0 = full context) and how many earlier chunks a frame
+    # may attend to (-1 = all).  Plain attributes, not state: state_dict keys do not change, and pickles without them read these.
+    chunk_size = 0
+    left_chunks = -1
 
     def __init__(self, input_dim, input_ctx, output_dim, tdnn_nhid, tdnn_layers, bn_dim=0):
         super().__init__()
@@ -78,6 +84,32 @@ class Net(nn.Module):
             [_TransformerLayerParams(tdnn_nhid, self.HEADS[i], tdnn_nhid * 4, self.XF_DROPOUT) for i in range(3)])
         self.bn_final = nn.BatchNorm1d(tdnn_nhid)
         self.fc_out = nn.Linear(tdnn_nhid, output_dim)
+
+    def attention_geometry(self):
+        """[(s_l, o_l)] of the attention layers: frame i of attention layer l reads input frames up to s_l * i + o_l (each TDNN is a
+        valid convolution: output i reads inputs s*i + k*d, k < filter_size)"""
+        geo, s, o = [], 1, 0
+        for l, (dil, stride) in enumerate(self.TDNN_DIL_STRIDE):
+            o += s * (self.filter_size - 1) * dil
+            s *= stride
+            if (l + 1) % 3 == 0:
+                geo.append((s, o))
+        return geo
+
+    def chunk_masks(self, chunk_size=None, left_chunks=None):
+        """per attention layer, the chunk mask (chunk_len, chunk_off, left_chunks) of ``chunk_size`` output frames (default: the
+        attributes), or None everywhere for full context.  A frame belongs to the chunk that holds its rightmost input frame, so a chunk
+        of C output frames is W = C * (product of the strides) input frames, and layer l's frame i is in chunk (i + o_l // s_l) //
+        (W // s_l)."""
+        C = self.chunk_size if chunk_size is None else int(chunk_size)
+        left = self.left_chunks if left_chunks is None else int(left_chunks)
+        if C < 0 or left < -1:
+            raise ValueError("chunk_size must be >= 0 and left_chunks >= -1 (got %d, %d)" % (C, left))
+        geo = self.attention_geometry()
+        if C == 0:
+            return [None] * len(geo)
+        W = C * math.prod(stride for _, stride in self.TDNN_DIL_STRIDE)
+        return [(W // s, o // s, left) for s, o in geo]
 
     def forward(self, x, frame_offset=0):
         from pika_b200 import engine

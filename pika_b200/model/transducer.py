@@ -35,6 +35,8 @@ class Net(nn.Module):
         else:
             self.encoder = encoder_tdnn(input_dim=input_dim, input_ctx=0, output_dim=self.hid_dim,
                                         tdnn_nhid=1024, tdnn_layers=9)
+            self.encoder.chunk_size = getattr(opt, "chunk_size", 0)              # streaming (chunk-limited attention)
+            self.encoder.left_chunks = getattr(opt, "left_chunks", -1)
             self.pack_seq = False
         self.embed = nn.Embedding(output_dim + 1, opt.embd_dim, padding_idx=opt.padding_idx)
         if opt.decoder_type == "rnn":

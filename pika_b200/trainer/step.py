@@ -5,6 +5,10 @@ encoder / prediction net / fused joint+loss forward and backward -> inf-norm cli
 BMUF block sync every ``sync_period`` batches.
 """
 
+import contextlib
+
+import numpy as np
+
 from .. import engine
 from ..frontend import noise_rir_kwargs
 from .flat import lr_at
@@ -44,6 +48,35 @@ def emission_reg(args):
     return dict(fastemit_lambda=float(getattr(args, "fastemit_lambda", 0.0)), delay_penalty=float(getattr(args, "delay_penalty", 0.0)))
 
 
+def chunk_for_batch(args, index):
+    """with --dynamic_chunk_max M, the encoder's chunk size for global batch ``index``: full context (0) with probability 1/2 and otherwise
+    uniform in [1, M], from a generator of its own seeded by (--seed, rank, index), so the loader's, SpecAugment's and torch's random
+    streams do not move.  None without the flag: the encoder keeps its own setting."""
+    M = int(getattr(args, "dynamic_chunk_max", 0))
+    if M <= 0:
+        return None
+    rng = np.random.default_rng([int(args.seed) & 0xFFFFFFFF, int(getattr(args, "local_rank", 0) or 0), int(index)])
+    if rng.random() < 0.5:
+        return 0
+    return int(rng.integers(1, M + 1))
+
+
+@contextlib.contextmanager
+def encoder_chunk(model, chunk_size):
+    """runs the block with the TDNN-Transformer encoder's chunk_size set to ``chunk_size`` (None: unchanged), and restores it after (so a
+    checkpoint of a dynamically chunked model records its static setting)"""
+    enc = model.encoder
+    if chunk_size is None or not hasattr(enc, "chunk_masks"):
+        yield
+        return
+    old = enc.chunk_size
+    enc.chunk_size = chunk_size
+    try:
+        yield
+    finally:
+        enc.chunk_size = old
+
+
 class TrainStep:
     def __init__(self, model, args, frontend, bmuf, optimizer, offset=None, scale=None, spec_augmentor=None):
         self.model, self.args, self.frontend, self.bmuf, self.opt = model, args, frontend, bmuf, optimizer
@@ -72,6 +105,19 @@ class TrainStep:
         len_batch = encoder_out_lens(self.frontend.out_lens(batch["n_frames"]), a.model_lctx, a.model_rctx, a.model_stride)
         t_out = encoder_out_max(int(batch["t_max"]), a.model_lctx, a.model_rctx, a.model_stride)
         self.simple_costs = None
+        with encoder_chunk(self.model, chunk_for_batch(a, a.epoch * a.num_batches_per_epoch + self.num_done)):
+            costs, loss = self._loss(feats, batch, len_batch, t_out)
+        engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1
+        try:
+            loss.backward()
+        finally:
+            engine.assume_unit_loss_grad(False)
+        self.opt.step()                                                   # clip_grad_norm_(inf) + SGD(nesterov)
+        self.end_of_item()
+        return costs
+
+    def _loss(self, feats, batch, len_batch, t_out):
+        a = self.args
         if getattr(a, "prune_range", 0) > 0:
             ss, ps = prune_loss_scales(a, a.epoch * a.num_batches_per_epoch + self.num_done)
             simple, costs = engine.transducer_loss_pruned(self.model, feats, batch["target"], len_batch, batch["ali_lens"], a.prune_range,
@@ -82,14 +128,7 @@ class TrainStep:
             costs = engine.transducer_loss(self.model, feats, batch["target"], len_batch, batch["ali_lens"], x_len=len_batch, t_out=t_out,
                                            **emission_reg(a))
             loss = costs.sum()
-        engine.assume_unit_loss_grad(True)                                # loss = costs.sum() (:99): upstream gradient is exactly 1
-        try:
-            loss.backward()
-        finally:
-            engine.assume_unit_loss_grad(False)
-        self.opt.step()                                                   # clip_grad_norm_(inf) + SGD(nesterov)
-        self.end_of_item()
-        return costs
+        return costs, loss
 
     def skip(self):
         """An empty loader item (every utterance filtered, :100-101): no forward / backward / optimiser step, but the item

@@ -167,7 +167,34 @@ def build_parser():
                         help='delay penalty: add this x ((T-1)/2 - t) to the log-prob of every label arc emitted on frame t, in the '
                              'RNN-T loss and (with --prune_range) the simple loss too; the logged losses are the penalised ones.  '
                              '>= 0, 0 = off; not ramped by --prune_warmup_batches')
+    parser.add_argument('--chunk_size', type=int, default=0,
+                        help='streaming TDNN-Transformer encoder (DESIGN.md "Chunked attention"): self-attention limited to chunks of this '
+                             'many encoder output frames and earlier ones; 0 = full context')
+    parser.add_argument('--left_chunks', type=int, default=-1,
+                        help='with --chunk_size / --dynamic_chunk_max: how many earlier chunks a frame may attend to; -1 = all')
+    parser.add_argument('--dynamic_chunk_max', type=int, default=0,
+                        help='per batch, full context with probability 1/2, otherwise a chunk size drawn uniformly from [1, this]; '
+                             '0 = off.  Checkpoints record chunk size 0')
     return parser
+
+
+def check_chunk_args(parser, args):
+    """parser.error unless --chunk_size / --left_chunks / --dynamic_chunk_max are in range, consistent, and on the TDNN-Transformer"""
+    C, left, M = args.chunk_size, args.left_chunks, args.dynamic_chunk_max
+    if C < 0 or M < 0 or left < -1:
+        parser.error('--chunk_size and --dynamic_chunk_max must be >= 0 and --left_chunks >= -1 (got %d, %d, %d)' % (C, M, left))
+    if C > 0 and M > 0:
+        parser.error('--chunk_size and --dynamic_chunk_max exclude each other')
+    if left != -1 and C == 0 and M == 0:
+        parser.error('--left_chunks needs --chunk_size or --dynamic_chunk_max')
+    if args.encoder_type == 'rnn' and (C or M or left != -1):
+        parser.error('--chunk_size / --left_chunks / --dynamic_chunk_max apply to the TDNN-Transformer encoder (--encoder_type transformer)')
+
+
+def apply_chunk_args(model, args):
+    """the encoder's static chunk setting from the flags (also for an --init_model)"""
+    if hasattr(model.encoder, 'chunk_masks'):
+        model.encoder.chunk_size, model.encoder.left_chunks = args.chunk_size, args.left_chunks
 
 
 def check_smoothing_args(parser, args):
@@ -197,6 +224,7 @@ def main(argv=None):
     args = parser.parse_args(argv)
     check_smoothing_args(parser, args)
     check_emission_reg_args(parser, args)
+    check_chunk_args(parser, args)
     args.input_dim = loader_module.get_inputdim(args)
     args.dataloader = loader_module.dataloader
     args.raw_batches = True
@@ -226,6 +254,7 @@ def main(argv=None):
             add_simple_joiner(model, model.fc2.weight.shape[1], model.fc2.weight.shape[0])   # drawn after the seed above
     if args.prune_range == 1 or args.prune_range < 0:
         parser.error('--prune_range must be 0 (off) or >= 2')
+    apply_chunk_args(model, args)
     model.to(dev)
     flat = FlatParams(model)
     if args.block_sync == 'bmuf_adam':

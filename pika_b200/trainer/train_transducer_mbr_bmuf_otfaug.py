@@ -27,8 +27,8 @@ from .. import engine
 from .bmuf import BmufTrainer
 from .flat import FlatParams, SgdNesterovClip, lr_at
 from .mbr import mbr_forward_backward
-from .step import TrainStep, encoder_out_lens
-from .train_transducer_bmuf_otfaug import build_parser as build_rnnt_parser, check_emission_reg_args
+from .step import TrainStep, chunk_for_batch, encoder_chunk, encoder_out_lens
+from .train_transducer_bmuf_otfaug import apply_chunk_args, build_parser as build_rnnt_parser, check_chunk_args, check_emission_reg_args
 
 MASTER_NODE = 0
 
@@ -59,14 +59,17 @@ def run_one_epoch(epoch, log_f, model, args, bmuf_trainer):
             ali_lens = ali_lens_cpu.to(dev)
             feats = step.features(batch)                                      # CMN / CMVN, no SpecAugment yet (:109-115)
             len_batch = encoder_out_lens(args.frontend.out_lens(batch["n_frames"]), args.model_lctx, args.model_rctx, args.model_stride)
-            model.eval()                                                      # N-best generation (:117-123)
-            ret, _ = decoder.decode_batch(feats, len_batch.cpu(), [int(t) + int(u) + 3 for t, u in zip(len_batch.cpu(), ali_lens_cpu)])
-            model.train()
-            optimizer.flat.zero_grad()
-            if spec is not None:                                              # SpecAugment on the training forward only (:134-135)
-                spec.apply(feats)
-            mbr, costs = mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=args.blk, rnnt_scale=args.rnnt_scale,
-                                              sm_scale=args.sm_scale, fastemit_lambda=args.fastemit_lambda, delay_penalty=args.delay_penalty)
+            # one chunk size for the item's N-best generation and its training forward
+            with encoder_chunk(model, chunk_for_batch(args, epoch * args.num_batches_per_epoch + step.num_done)):
+                model.eval()                                                  # N-best generation (:117-123)
+                ret, _ = decoder.decode_batch(feats, len_batch.cpu(), [int(t) + int(u) + 3 for t, u in zip(len_batch.cpu(), ali_lens_cpu)])
+                model.train()
+                optimizer.flat.zero_grad()
+                if spec is not None:                                          # SpecAugment on the training forward only (:134-135)
+                    spec.apply(feats)
+                mbr, costs = mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=args.blk, rnnt_scale=args.rnnt_scale,
+                                                  sm_scale=args.sm_scale, fastemit_lambda=args.fastemit_lambda,
+                                                  delay_penalty=args.delay_penalty)
             optimizer.step()                                                  # clip_grad_norm_(inf) + SGD(nesterov) (:236-240)
             mbr_loss, rnnt_loss = float(mbr), float(costs.sum().item())
         try:                                                                  # (:245-257) for every loader item, data or not
@@ -111,6 +114,7 @@ def main(argv=None):
     if args.lm_only_scale != 0.0 or args.am_only_scale != 0.0:    # inherited from the RNN-T parser; there is no simple loss here
         parser.error('--lm_only_scale / --am_only_scale: the MBR trainer has no simple loss to smooth')
     check_emission_reg_args(parser, args)        # inherited: applied to the RNN-T branch, not to the MBR loss
+    check_chunk_args(parser, args)               # inherited: the encoder of the N-best generation and of both branches
     if args.lm:
         raise NotImplementedError("pika_b200: --lm (neural LM fusion) is outside the hot path")
     args.input_dim = loader_module.get_inputdim(args)
@@ -137,6 +141,7 @@ def main(argv=None):
         model = nnet_module.Net(args, args.input_dim, args.output_dim)
     else:
         model = torch.load(args.init_model, map_location=lambda storage, loc: storage, weights_only=False)
+    apply_chunk_args(model, args)
     model.to(dev)
     flat = FlatParams(model)
     bmuf_trainer = BmufTrainer(MASTER_NODE, args.local_rank, world_size, model, args.block_momentum, args.block_lr, flat=flat)
