@@ -470,14 +470,17 @@ int pk_bmuf_adam_update(float* glob, float* local, float* delta_prev, float* exp
  *   pcm [B, ld_pcm] int16; n_samples, new_len (= int(n/rate)) [B] int32
  *   n_frames [B] int32: fbank frames of new_len samples; snip_edges: 0 if new_len < frame_len, else 1+(new_len-frame_len)/frame_shift;
  *     otherwise (new_len + frame_shift/2) / frame_shift, frame t starting at t*frame_shift + frame_shift/2 - frame_len/2 with the
- *     samples outside [0, new_len) reflected about the edges (Kaldi's ExtractWindow)
+ *     samples outside [0, new_len) reflected about the edges (Kaldi's ExtractWindow).  Precondition the host cannot check (the
+ *     lengths live on the device): with snip_edges = 0, new_len[b] >= 1 wherever n_frames[b] > 0 -- reflection about an empty
+ *     signal never ends.  The same holds for n_samples of pk_fbank / pk_mfcc.
  *   t_max: output rows; stride: output row t is spliced fbank frame min(t, ceil(n_frames/stride)-1)*stride, i.e.
  *     splice(feats)[::stride] padded with its last row.  Workspace queries take t_max*stride, the fbank frames held in between.
  *   rate, target_db [B] f32 (host-drawn, as the reference draws them in the loader thread)
  *   window [frame_len], twiddle [N/2 x (re,im)] = exp(-2 pi i k / N), mel_w [n_mel, N/2], mel_lo/hi [n_mel]: host-built tables for
  *     the FFT size N = 2^log2_nfft, 128 <= N <= 2048, 1 <= frame_len <= N; n_max >= frame_len when snip_edges is set
  *   remove_dc: subtract each window's mean (Kaldi --remove-dc-offset); preemph: --preemphasis-coefficient
- *   offset/scale [D] CMVN (NULL = off); cmn: subtract the per-utterance mean over the PADDED time axis
+ *   offset/scale [D] CMVN (NULL = off); cmn: subtract the per-utterance mean over the PADDED time axis, summed in a fixed order
+ *     (row order within blocks of 64 rows, then block order), so that repeated runs give the same bits
  *   (f0,fs,t0,ts): SpecAugment freq/time mask start and span (span 0 = off), shared by the batch
  *   out [B, t_max, D] f32|bf16; wave_i16_out [B, n_max] optional copy of the augmented samples
  *   err_flag: set to 1 if a gain above 300 dB was requested (the reference raises ValueError)
@@ -508,7 +511,9 @@ int pk_fbank(const float* wave, long long ld_wave, const int* n_samples, const i
  *   noise_rms_db [n_noise] f64: rms_db of each whole segment (float32 samples, as AudioSegment.rms_db)
  *   rir          int16 bank of concatenated RIRs (device), or null for no reverberation
  *   rir_off      [n_rir] int64 start, rir_len [n_rir] int32 length (>= 1), rir_idx [B] int32 RIR of each utterance
- *   rir_max_len  host-side bound >= every rir_len[rir_idx[b]], in [1, 65536] (pass 1 without RIRs); sets the FFT block length
+ *   rir_max_len  host-side bound >= every rir_len[rir_idx[b]], in [1, 65536] (pass 1 without RIRs); sets the FFT block length.
+ *                Precondition the host cannot check (the lengths live on the device): a drawn RIR longer than rir_max_len is
+ *                silently truncated to its first ceil(rir_max_len / Lb) blocks of Lb samples
  * The convolution is fftconvolve(x, h, "same") in float64 (uniformly partitioned overlap-save); on the rate == 1.0 branch the
  * result is rounded to float32, like the reference's float32 samples.  err_flag also reports a renormalisation gain above 300 dB.
  * Workspace: pk_frontend_noise_rir_workspace_bytes (< 0 when rir_max_len is outside [1, 65536]; no device access). */

@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(AUG_THREADS) aug_resample_kernel(const short* 
             const float sq = s * s;                                      // numpy: float32 array ** 2
             acc += (double)sq;
         } else {
-            const double x = (j == L - 1) ? (double)N : __dmul_rn((double)j, step);
+            const double x = (j == L - 1 && L > 1) ? (double)N : __dmul_rn((double)j, step);   // linspace(0, N, 1) = [0]
             if (x >= (double)(N - 1)) {
                 v = (double)((float)src[N - 1] * (1.0f / 32768.0f));     // right of the last knot: fp[-1]
             } else {
@@ -576,9 +576,11 @@ PK_DEVICE float spliced_value(const float* __restrict__ fb, int n_frames, int n_
     src = max(0, min(n_frames - 1, src));
     return fb[(long long)src * n_mel + c];
 }
+// CMN column sums in a fixed order, so that the mean does not depend on the order in which CTAs finish: each CTA sums its 64 rows
+// in row order into partial [B, parts, D] (parts = gridDim.x), then splice_colmerge adds the parts in block order
 template <bool STRIDED>
 __global__ void splice_colsum_kernel(const float* __restrict__ feats, long long ld_b, const int* __restrict__ n_frames, int n_mel,
-                                     int lctx, int stride, int D, int t_max, float* __restrict__ sums) {
+                                     int lctx, int stride, int D, int t_max, float* __restrict__ partial) {
     const int b = blockIdx.y, col = threadIdx.x;
     if (col >= D || n_frames[b] <= 0) return;
     const int t0 = blockIdx.x * 64, t1 = min(t_max, t0 + 64);
@@ -586,7 +588,17 @@ __global__ void splice_colsum_kernel(const float* __restrict__ feats, long long 
     const int nf = n_frames[b], n_out = STRIDED ? (nf + stride - 1) / stride : nf;
     float s = 0.f;
     for (int t = t0; t < t1; ++t) s += spliced_value<STRIDED>(fb, nf, n_out, n_mel, lctx, stride, t, col);
-    atomicAdd(&sums[(long long)b * D + col], s);
+    partial[((long long)b * gridDim.x + blockIdx.x) * D + col] = s;
+}
+// sums [B, D] <- the parts of splice_colsum added in block order (0 for an utterance without frames, whose parts are not written)
+__global__ void splice_colmerge_kernel(const float* __restrict__ partial, int parts, const int* __restrict__ n_frames, int D,
+                                       float* __restrict__ sums) {
+    const int b = blockIdx.x, col = threadIdx.x;
+    if (col >= D) return;
+    float s = 0.f;
+    if (n_frames[b] > 0)
+        for (int p = 0; p < parts; ++p) s += partial[((long long)b * parts + p) * D + col];
+    sums[(long long)b * D + col] = s;
 }
 template <typename T, bool STRIDED>
 __global__ void splice_finalize_kernel(const float* __restrict__ feats, long long ld_b, const int* __restrict__ n_frames, int n_mel,
@@ -611,14 +623,16 @@ __global__ void splice_finalize_kernel(const float* __restrict__ feats, long lon
 using namespace pk;
 
 /* Workspace layout of pk_frontend_fwd: resampled f64 [B, n_max] | partial f64 [B, parts] | wave f32 [B, n_max] |
- * feats f32 [B, t_max, n_mel] | sums f32 [B, D] | err int.  t_max here counts fbank frames, before the splice's stride. */
+ * feats f32 [B, t_max, n_mel] | sums f32 [B, D] | CMN partials f32 [B, ceil(t_max / 64), D] | err int.  t_max here counts fbank
+ * frames, before the splice's stride, so it bounds the output rows the CMN sums run over. */
 static const int kAugParts = 64;
+static long long cmn_parts(long long t_max) { return (t_max + 63) / 64; }
 extern "C" long long pk_frontend_workspace_bytes(int B, int n_max, int t_max, int n_mel, int D) {
     long long b = 0;
     b += (long long)B * n_max * 8 + (long long)B * kAugParts * 8;
     b += (long long)B * n_max * 4;
     b += (long long)B * t_max * n_mel * 4;
-    b += (long long)B * D * 4 + 256;
+    b += (long long)B * D * 4 + (long long)B * cmn_parts(t_max) * D * 4 + 256;
     return b + 1024;
 }
 
@@ -771,12 +785,20 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
     PK_CHECK_ARG(stride >= 1 && (long long)t_max * stride <= 0x7fffffffLL, "bad splice stride");
     const int t_fb = t_max * stride;
     PK_CHECK_ARG(workspace_bytes >= pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D), "frontend workspace too small");
+    ConvGeom g{};
+    if (nr) {
+        PK_CHECK_ARG(nr->rir_max_len >= 1 && nr->rir_max_len <= kRirMaxLen, "rir_max_len must be in [1, 65536]");
+        PK_CHECK_ARG(workspace_bytes >= align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D)) +
+                                            noise_rir_extra_bytes(B, n_max, nr->rir_max_len, &g),
+                     "frontend workspace too small");
+    }
     unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
     double* resampled = reinterpret_cast<double*>(w); w += (long long)B * n_max * 8;
     double* partial = reinterpret_cast<double*>(w);   w += (long long)B * kAugParts * 8;
     float* wave = reinterpret_cast<float*>(w);        w += (long long)B * n_max * 4;
     float* feats = reinterpret_cast<float*>(w);       w += (long long)B * t_fb * n_feat * 4;
-    float* sums = reinterpret_cast<float*>(w);
+    float* sums = reinterpret_cast<float*>(w);        w += (long long)B * D * 4;
+    float* cmn_part = reinterpret_cast<float*>(w);
     dim3 ga(kAugParts, B);
     aug_resample_kernel<<<ga, AUG_THREADS, 0, st>>>(pcm, ld_pcm, n_samples, rate, new_len, resampled, n_max, partial, kAugParts);
     PK_CHECK_LAUNCH(); count_launch();
@@ -785,10 +807,7 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
                                                    n_max, err_flag);
         PK_CHECK_LAUNCH(); count_launch();
     } else {
-        PK_CHECK_ARG(nr->rir_max_len >= 1 && nr->rir_max_len <= kRirMaxLen, "rir_max_len must be in [1, 65536]");
-        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D));
-        ConvGeom g;
-        PK_CHECK_ARG(workspace_bytes >= base + noise_rir_extra_bytes(B, n_max, nr->rir_max_len, &g), "frontend workspace too small");
+        const long long base = align256(pk_frontend_workspace_bytes(B, n_max, t_fb, n_feat, D));    // checked above, with g
         unsigned char* x = reinterpret_cast<unsigned char*>(workspace) + base;
         double* part_gain = reinterpret_cast<double*>(x);  x += align256((long long)B * kAugParts * 8);
         double* part_noisy = reinterpret_cast<double*>(x); x += align256((long long)B * kAugParts * 8);
@@ -815,13 +834,15 @@ static int frontend_launch(const short* pcm, long long ld_pcm, const int* n_samp
         return -1;
     const long long ld_fb = (long long)t_fb * n_feat;
     if (cmn) {
-        PK_CHECK_CUDA(cudaMemsetAsync(sums, 0, sizeof(float) * B * D, st));
-        const dim3 grid((t_max + 63) / 64, B);
+        const int parts = (int)cmn_parts(t_max);
+        const dim3 grid(parts, B);
         const int threads = ((D + 31) / 32) * 32;
         if (stride == 1)
-            splice_colsum_kernel<false><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums);
+            splice_colsum_kernel<false><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, cmn_part);
         else
-            splice_colsum_kernel<true><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, sums);
+            splice_colsum_kernel<true><<<grid, threads, 0, st>>>(feats, ld_fb, n_frames, n_feat, lctx, stride, D, t_max, cmn_part);
+        PK_CHECK_LAUNCH(); count_launch();
+        splice_colmerge_kernel<<<B, threads, 0, st>>>(cmn_part, parts, n_frames, D, sums);
         PK_CHECK_LAUNCH(); count_launch();
     }
     const dim3 grid((int)(((long long)t_max * D + 255) / 256), B);
