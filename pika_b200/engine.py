@@ -780,86 +780,145 @@ class _Tap:
             EVENT_TAPS.setdefault(self.name, []).append((self.s, e))
 
 
-def _joint_forward(enc, pred, model, want_lse=False):
-    """factored gated joint -> (logits [B,T,U1,ldv] act dtype, saved state).  ``want_lse``: the fc2 GEMM also
-    reduces every logits row to per-tile (max, sum-exp) pairs (state["row_lse"]) for the fused loss."""
-    B, T, H = enc.shape
-    U1 = pred.shape[1]
-    V = model.fc2.weight.shape[0]
-    ldv = _ldv(V)
+def joint_forward(enc, pred, model, want_lse=False, bounds=None, R=0, nodes=None):
+    """The factored gated joint (trainer/model/transducer.py:96-108) over one of three row layouts -> (logits [rows, ldv] act dtype,
+    saved state for ``joint_backward``):
+      * the dense (b, t, u) grid (default): rows = B*T*U1 and the logits are shaped [B,T,U1,ldv];
+      * ``bounds`` [B,T] int32 and ``R``: row (b, t, r) is the joint at (t, bounds[b,t] + r), rows = B*T*R (the pruned loss's windows);
+      * ``nodes`` = (ex_idx, py_idx), int32 [rows]: row i joins row ex_idx[i] of enc [B,T,H] with row py_idx[i] of pred [B',U1,H] (the
+        MBR alignment nodes); the logits are zero-filled.
+    ``want_lse``: the fc2 GEMM also reduces every logits row to per-tile (max, sum-exp) pairs (state["row_lse"], else None) for the
+    fused loss, in bf16 when V % 8 == 0."""
+    H = enc.shape[-1]
     fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
+    V = fc2.weight.shape[0]
+    ldv = _ldv(V)
     wx = stage_weight([fc1.weight, fcg.weight])                       # [2H, 2H]; x half = cols [0,H), y half = [H,2H)
-    enc_parts = stage_act(enc.reshape(B * T, H))
-    pred_parts = stage_act(pred.reshape(B * U1, H))
-    ex = _new((B * T, 2 * H), like=enc)
-    py = _new((B * U1, 2 * H), like=enc)
+    enc_parts = stage_act(enc.reshape(-1, H))
+    pred_parts = stage_act(pred.reshape(-1, H))
+    ex = _new((enc_parts[0].shape[0], 2 * H), like=enc)
+    py = _new((pred_parts[0].shape[0], 2 * H), like=enc)
     gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=_cat_bias([fc1.bias, fcg.bias]))
     gemm_parts([pred_parts], [[p[:, H:] for p in wx]], py)
-    R = B * T * U1
-    h = _new((R, H), like=enc)
-    K.joint_gate_fwd(ex, py, h, B, T, U1, H)
+    B, T, U1 = enc.shape[0], enc.shape[1], pred.shape[1]
+    rows = nodes[0].shape[0] if nodes is not None else B * T * (R if bounds is not None else U1)
+    h = _new((rows, H), like=enc)
+    if nodes is not None:
+        ex_g, py_g = _new((rows, 2 * H), like=enc), _new((rows, 2 * H), like=enc)
+        K.gather_rows(ex, nodes[0], ex_g)
+        K.gather_rows(py, nodes[1], py_g)
+        ex, py = ex_g, py_g
+        K.joint_gate_fwd(ex, py, h, rows, 1, 1, H)
+    elif bounds is not None:
+        K.joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H)
+    else:
+        K.joint_gate_fwd(ex, py, h, B, T, U1, H)
     w2 = stage_weight(fc2.weight)
-    logits = _new((B, T, U1, ldv), like=enc, zero=(ldv != V))
+    dense = nodes is None and bounds is None
+    logits = _new((B, T, U1, ldv) if dense else (rows, ldv), like=enc, zero=(ldv != V or nodes is not None))
     h_parts = stage_act(h)
+    del h
     row_lse = None
     if want_lse and _FUSED_LSE and logits.dtype == torch.bfloat16 and V % 8 == 0:
-        row_lse = torch.empty(K.row_lse_parts(R, V, 256), R, 2, dtype=torch.float32, device=enc.device)
+        row_lse = torch.empty(K.row_lse_parts(rows, V, 256), rows, 2, dtype=torch.float32, device=enc.device)
     with _Tap("fc2_fwd"):
-        gemm_parts([h_parts], [w2], logits.view(R, ldv)[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
+        gemm_parts([h_parts], [w2], logits.view(rows, ldv)[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
                    **({"block_n": 256} if row_lse is not None else {}))
-    state = dict(row_lse=row_lse, ex=ex, py=py, h_parts=h_parts, enc_parts=enc_parts, pred_parts=pred_parts, wx=wx, w2=w2, dims=(B, T, U1, H, V, ldv))
+    state = dict(row_lse=row_lse, ex=ex, py=py, h_parts=h_parts, enc_parts=enc_parts, pred_parts=pred_parts, wx=wx,
+                 enc_shape=enc.shape, pred_shape=pred.shape, bounds=bounds, R=R, nodes=nodes)
     return logits, state
 
 
-def _joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None, compact=None):
-    """dlogits [B,T,U1,ldv] (padding columns zero) -> (d_enc, d_pred); parameter grads written in place.
-    compact = (h_c, row_map, row_count) of rnnt_loss_compact: dlogits and h_c hold only the kept rows, the GEMMs run over row_count
-    of them and the gate backward reads dh through row_map."""
-    B, T, U1, H, V, ldv = st["dims"]
-    R = B * T * U1
-    fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
-    dl_parts = [p.view(R, ldv) for p in stage_act(dlogits)]
-    dl_v = [p[:, :V] for p in dl_parts]
-    dh = _new((R, H), like=dlogits)
-    h_parts, row_map, rows = st.get("h_parts"), None, None
+def joint_backward(dlogits, st, model, need_enc=True, need_pred=True, db2=None, compact=None, accumulate=False):
+    """dlogits (``joint_forward``'s logits shape, padding columns zero) -> (d_enc, d_pred) shaped like enc and pred; the joint's
+    parameter gradients are written in place, or added to them with ``accumulate``.  db2: the column sums of dlogits when the loss
+    kernel already formed them.  compact = (h_c, row_map, row_count) of rnnt_loss_compact (dense layout): dlogits and h_c hold only
+    the kept rows, the fc2 GEMMs run over row_count of them and the gate backward reads dh through row_map.  The fc2 input is taken
+    out of ``st`` and released before the gate backward."""
+    h_parts, row_map, rows = st.pop("h_parts", None), None, None
     if compact is not None:
         h_c, row_map, rows = compact
         h_parts = [h_c]
-    gemm_parts([dl_v], [st["w2"]], dh, b_mn=True, a_rows_dev=rows)
-    gemm_parts([dl_v], [h_parts], grad_of(fc2.weight), a_mn=True, b_mn=True, a_rows_dev=rows)
-    if db2 is None:
-        db2 = torch.empty(ldv, dtype=torch.float32, device=dlogits.device)
-        K.colsum(dlogits.view(R, ldv), db2)
-    grad_of(fc2.bias).copy_(db2[:V])
-    dex = _new((B * T, 2 * H), like=dlogits)
-    dpy = _new((B * U1, 2 * H), like=dlogits)
-    K.joint_gate_bwd(st["ex"], st["py"], dh, dex, dpy, B, T, U1, H, dh_map=row_map)
+    dh = _vocab_proj_backward(dlogits.view(-1, dlogits.shape[-1]), h_parts, model.fc2, db2, rows, accumulate)
+    del h_parts
+    dex, dpy = _gate_backward(st, dh, row_map)
     del dh
-    return _gate_input_grads(dex, dpy, st, model, need_enc, need_pred)
+    return _gate_input_grads(dex, dpy, st, model, need_enc, need_pred, accumulate)
 
 
-def _gate_input_grads(dex, dpy, st, model, need_enc, need_pred):
-    """gate-input gradients dex [B*T, 2H], dpy [B*U1, 2H] -> (d_enc, d_pred); the fc1 / fc_gate gradients written in place"""
-    B, T, U1, H = st["dims"][:4]
+def _write_grad(p, g, accumulate):
+    """p.grad = g, or p.grad += g with ``accumulate``"""
+    if accumulate:
+        K.add(p.grad, g, p.grad)
+    else:
+        grad_of(p).copy_(g)
+
+
+def _vocab_proj_backward(d, x_parts, lin, db=None, a_rows_dev=None, accumulate=False):
+    """d [rows, ldv] (act dtype, padding columns 0) = d(loss)/d(x W^T + b) of a projection ``lin`` to V, x staged as ``x_parts`` ->
+    dx [rows, K]; dW and db written in place, or added to them with ``accumulate``.  db: the column sums of d if already formed;
+    a_rows_dev: int32 device tensor [1], only that many leading rows of d and x take part."""
+    V = lin.weight.shape[0]
+    d_v = [p[:, :V] for p in stage_act(d)]
+    dx = _new((d.shape[0], lin.weight.shape[1]), like=d)
+    gemm_parts([d_v], [stage_weight(lin.weight)], dx, b_mn=True, a_rows_dev=a_rows_dev)
+    gemm_parts([d_v], [x_parts], grad_of(lin.weight), a_mn=True, b_mn=True, a_rows_dev=a_rows_dev, accumulate=accumulate,
+               k_splits=1 if accumulate else 0)
+    if db is None:
+        db = torch.empty(d.shape[1], dtype=torch.float32, device=d.device)
+        K.colsum(d, db)
+    _write_grad(lin.bias, db[:V], accumulate)
+    return dx
+
+
+def _gate_backward(st, dh, dh_map=None):
+    """dh [rows, H] -> the gate-input gradients dex [B*T, 2H], dpy [B'*U1, 2H] through ``joint_forward``'s row layout (f32 for the
+    node layout, whose rows are scatter-added; act dtype otherwise).  dh_map: the compacted rows' map (rnnt_loss_compact)."""
+    ex, py, nodes = st["ex"], st["py"], st["nodes"]
+    B, T, H = st["enc_shape"]
+    U1 = st["pred_shape"][1]
+    n_ex, n_py = st["enc_parts"][0].shape[0], st["pred_parts"][0].shape[0]
+    if nodes is not None:
+        rows = dh.shape[0]
+        dex_g, dpy_g = _new((rows, 2 * H), like=dh), _new((rows, 2 * H), like=dh)
+        K.joint_gate_bwd(ex, py, dh, dex_g, dpy_g, rows, 1, 1, H)
+        dex = torch.zeros(n_ex, 2 * H, dtype=torch.float32, device=dh.device)
+        dpy = torch.zeros(n_py, 2 * H, dtype=torch.float32, device=dh.device)
+        K.scatter_add_rows(dex_g, nodes[0], dex)
+        K.scatter_add_rows(dpy_g, nodes[1], dpy)
+        return dex, dpy
+    dex, dpy = _new((n_ex, 2 * H), like=dh), _new((n_py, 2 * H), like=dh)
+    if st["bounds"] is not None:
+        K.joint_gate_pruned_bwd(ex, py, st["bounds"], dh, dex, dpy, B, T, U1, st["R"], H)
+    else:
+        K.joint_gate_bwd(ex, py, dh, dex, dpy, B, T, U1, H, dh_map=dh_map)
+    return dex, dpy
+
+
+def _gate_input_grads(dex, dpy, st, model, need_enc, need_pred, accumulate):
+    """gate-input gradients dex [B*T, 2H], dpy [B'*U1, 2H] -> (d_enc, d_pred); the fc1 / fc_gate gradients written in place, or
+    added to them with ``accumulate``.  The GEMMs read dex / dpy in the activation dtype, the bias column sum as given."""
+    H = st["enc_shape"][-1]
     fc1, fcg = model.fc1, model.fc_gate
-    dex_parts, dpy_parts = stage_act(dex), stage_act(dpy)
+    dex_parts, dpy_parts = stage_act(_to_act(dex)), stage_act(_to_act(dpy))
     g1, gg = grad_of(fc1.weight), grad_of(fcg.weight)
+    acc = dict(accumulate=accumulate, k_splits=1 if accumulate else 0)
     for (dparts, xparts, lo) in ((dex_parts, st["enc_parts"], 0), (dpy_parts, st["pred_parts"], H)):
-        gemm_parts([[p[:, :H] for p in dparts]], [xparts], g1[:, lo:lo + H], a_mn=True, b_mn=True)
-        gemm_parts([[p[:, H:] for p in dparts]], [xparts], gg[:, lo:lo + H], a_mn=True, b_mn=True)
+        gemm_parts([[p[:, :H] for p in dparts]], [xparts], g1[:, lo:lo + H], a_mn=True, b_mn=True, **acc)
+        gemm_parts([[p[:, H:] for p in dparts]], [xparts], gg[:, lo:lo + H], a_mn=True, b_mn=True, **acc)
     dbx = torch.empty(2 * H, dtype=torch.float32, device=dex.device)
     K.colsum(dex, dbx)
-    grad_of(fc1.bias).copy_(dbx[:H])
-    grad_of(fcg.bias).copy_(dbx[H:])
+    _write_grad(fc1.bias, dbx[:H], accumulate)
+    _write_grad(fcg.bias, dbx[H:], accumulate)
     d_enc = d_pred = None
     if need_enc:
-        d_enc = _new((B * T, H), like=dex)
+        d_enc = _new((dex.shape[0], H), like=dex)
         gemm_parts([dex_parts], [[p[:, :H] for p in st["wx"]]], d_enc, b_mn=True)
-        d_enc = d_enc.view(B, T, H)
+        d_enc = d_enc.view(st["enc_shape"])
     if need_pred:
-        d_pred = _new((B * U1, H), like=dex)
+        d_pred = _new((dpy.shape[0], H), like=dex)
         gemm_parts([dpy_parts], [[p[:, H:] for p in st["wx"]]], d_pred, b_mn=True)
-        d_pred = d_pred.view(B, U1, H)
+        d_pred = d_pred.view(st["pred_shape"])
     return d_enc, d_pred
 
 
@@ -868,13 +927,14 @@ class JointFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, pred, model):
-        logits, st = _joint_forward(enc, pred, model)
+        logits, st = joint_forward(enc, pred, model)
         ctx.st, ctx.model = st, model
         return logits
 
     @staticmethod
     def backward(ctx, dlogits):
-        d_enc, d_pred = _joint_backward(dlogits.contiguous(), ctx.st, ctx.model, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        # a copy: joint_backward takes the fc2 input out of the state it is given, and a retained graph may run this again
+        d_enc, d_pred = joint_backward(dlogits.contiguous(), dict(ctx.st), ctx.model, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         return d_enc, d_pred, None
 
 
@@ -905,8 +965,8 @@ class JointLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, need_grad=True, fastemit_lambda=0.0, delay_penalty=0.0):
-        logits, st = _joint_forward(enc, pred, model, want_lse=True)
-        V = st["dims"][4]
+        logits, st = joint_forward(enc, pred, model, want_lse=True)
+        V = model.fc2.weight.shape[0]
         ctx.need_grad = need_grad
         reg = dict(fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
         if not need_grad:
@@ -914,7 +974,7 @@ class JointLossFn(torch.autograd.Function):
             return costs
         db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=logits.device)
         compact = None
-        if _COMPACT_GRAD and logits.dtype == torch.bfloat16 and len(st["w2"]) == 1 and len(st["h_parts"]) == 1:
+        if _COMPACT_GRAD and logits.dtype == torch.bfloat16:
             with _Tap("rnnt_loss"):
                 costs, dz_c, h_c, row_map, rows = K.rnnt_loss_compact(logits, labels, frame_lens, label_lens, st["h_parts"][0], V=V,
                                                                       colsum=db2, row_lse=st.pop("row_lse"), **reg)
@@ -925,7 +985,7 @@ class JointLossFn(torch.autograd.Function):
             with _Tap("rnnt_loss"):
                 costs, _ = K.rnnt_loss_fwd_bwd(logits, labels, frame_lens, label_lens, V=V, dlogits=logits, colsum=db2,
                                                row_lse=st.pop("row_lse"), **reg)
-        d_enc, d_pred = _joint_backward(logits, st, model, db2=db2, compact=compact)
+        d_enc, d_pred = joint_backward(logits, st, model, db2=db2, compact=compact)
         del compact
         del logits, st
         ctx.save_for_backward(d_enc, d_pred)
@@ -1216,20 +1276,6 @@ def _scaled_grads_backward(ctx, dcosts, params, who):
     return d_enc, d_pred
 
 
-def _proj_backward(d, x_parts, lin, V):
-    """d [rows, ldv] (act dtype, padding columns 0) = d(loss)/d(x W^T + b) of a projection to V -> dx [rows, H]; dW, db written"""
-    d_parts = stage_act(d)
-    d_v = [p[:, :V] for p in d_parts]
-    w_parts = stage_weight(lin.weight)
-    dx = _new((d.shape[0], lin.weight.shape[1]), like=d)
-    gemm_parts([d_v], [w_parts], dx, b_mn=True)
-    gemm_parts([d_v], [x_parts], grad_of(lin.weight), a_mn=True, b_mn=True)
-    db = torch.empty(d.shape[1], dtype=torch.float32, device=d.device)
-    K.colsum(d, db)
-    grad_of(lin.bias).copy_(db[:V])
-    return dx
-
-
 def check_smoothing_scales(lm_only_scale, am_only_scale):
     """-> (lm_only_scale, am_only_scale) as floats; ValueError unless both are >= 0 and their sum is < 1"""
     lam_l, lam_a = float(lm_only_scale), float(am_only_scale)
@@ -1335,8 +1381,8 @@ class SimpleLossFn(torch.autograd.Function):
         ctx.mark_non_differentiable(bounds)
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
         if need_grad:
-            d_enc = _proj_backward(dam, enc_parts, am_p, V).view(B, T, H)
-            d_pred = _proj_backward(dlm, pred_parts, lm_p, V).view(B, U1, H)
+            d_enc = _vocab_proj_backward(dam, enc_parts, am_p).view(B, T, H)
+            d_pred = _vocab_proj_backward(dlm, pred_parts, lm_p).view(B, U1, H)
             ctx.save_for_backward(d_enc, d_pred)
         return costs, bounds
 
@@ -1348,37 +1394,6 @@ class SimpleLossFn(torch.autograd.Function):
         return d_enc, d_pred, None, None, None, None, None, None, None, None, None, None
 
 
-def _pruned_joint_forward(enc, pred, model, bounds, R):
-    """the pruned joint: row (b, t, r) is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd) and fc2 runs on the B*T*R
-    rows, with the row log-sum-exp epilogue in bf16 -> (logits [B*T*R, ldv] act dtype, row_lse or None, saved state)"""
-    B, T, H = enc.shape
-    U1 = pred.shape[1]
-    fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
-    V = fc2.weight.shape[0]
-    ldv = _ldv(V)
-    wx = stage_weight([fc1.weight, fcg.weight])
-    enc_parts = stage_act(enc.reshape(B * T, H))
-    pred_parts = stage_act(pred.reshape(B * U1, H))
-    ex = _new((B * T, 2 * H), like=enc)
-    py = _new((B * U1, 2 * H), like=enc)
-    gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=_cat_bias([fc1.bias, fcg.bias]))
-    gemm_parts([pred_parts], [[p[:, H:] for p in wx]], py)
-    rows = B * T * R
-    h = _new((rows, H), like=enc)
-    K.joint_gate_pruned_fwd(ex, py, bounds, h, B, T, U1, R, H)
-    w2 = stage_weight(fc2.weight)
-    logits = _new((rows, ldv), like=enc, zero=(ldv != V))
-    h_parts = stage_act(h)
-    del h
-    row_lse = None
-    if _FUSED_LSE and logits.dtype == torch.bfloat16 and V % 8 == 0:
-        row_lse = torch.empty(K.row_lse_parts(rows, V, 256), rows, 2, dtype=torch.float32, device=enc.device)
-    with _Tap("fc2_fwd"):
-        gemm_parts([h_parts], [w2], logits[:, :V], bias=fc2.bias.detach(), row_lse=row_lse,
-                   **({"block_n": 256} if row_lse is not None else {}))
-    return logits, row_lse, dict(ex=ex, py=py, h_parts=h_parts, enc_parts=enc_parts, pred_parts=pred_parts, wx=wx, w2=w2)
-
-
 class PrunedJointLossFn(torch.autograd.Function):
     """Pruned joint + RNN-T loss: row (b, t, r) of the joint is the gated joint at (t, bounds[b,t] + r) (pk_joint_gate_pruned_fwd),
     fc2 runs on the B*T*R rows (with the row log-sum-exp epilogue in bf16), the loss and its gradient come from pk_rnnt_pruned_loss
@@ -1387,37 +1402,21 @@ class PrunedJointLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, pred, model, labels, frame_lens, label_lens, bounds, R, scale, need_grad, fastemit_lambda=0.0, delay_penalty=0.0):
-        B, T, H = enc.shape
         U1 = pred.shape[1]
-        fc2 = model.fc2
-        V = fc2.weight.shape[0]
-        ldv = _ldv(V)
-        dev = enc.device
-        rows = B * T * R
-        logits, row_lse, st = _pruned_joint_forward(enc, pred, model, bounds, R)
-        ex, py, h_parts, w2 = st["ex"], st["py"], st.pop("h_parts"), st["w2"]
+        V = model.fc2.weight.shape[0]
+        logits, st = joint_forward(enc, pred, model, want_lse=True, bounds=bounds, R=R)
+        row_lse = st.pop("row_lse")
         ctx.need_grad, ctx.scale, ctx.model = need_grad, float(scale), model
         reg = dict(fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
         if not need_grad:
             return K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, row_lse=row_lse, **reg)
-        scale_t = torch.full((B,), float(scale), dtype=torch.float32, device=dev)
-        db2 = torch.empty(ldv, dtype=torch.float32, device=dev)
+        scale_t = torch.full((enc.shape[0],), float(scale), dtype=torch.float32, device=enc.device)
+        db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=enc.device)
         with _Tap("rnnt_loss"):
             costs = K.rnnt_pruned_loss(logits, labels, frame_lens, label_lens, bounds, U1, R, V, grad_scale=scale_t, dlogits=logits,
                                        colsum=db2, row_lse=row_lse, **reg)
         del row_lse
-        dl_v = [p[:, :V] for p in stage_act(logits)]
-        dh = _new((rows, H), like=enc)
-        gemm_parts([dl_v], [w2], dh, b_mn=True)
-        gemm_parts([dl_v], [h_parts], grad_of(fc2.weight), a_mn=True, b_mn=True)
-        grad_of(fc2.bias).copy_(db2[:V])
-        del dl_v, logits, h_parts
-        dex = _new((B * T, 2 * H), like=enc)
-        dpy = _new((B * U1, 2 * H), like=enc)
-        K.joint_gate_pruned_bwd(ex, py, bounds, dh, dex, dpy, B, T, U1, R, H)
-        del dh
-        st = dict(enc_parts=st["enc_parts"], pred_parts=st["pred_parts"], wx=st["wx"], dims=(B, T, U1, H, V, ldv))
-        d_enc, d_pred = _gate_input_grads(dex, dpy, st, model, True, True)
+        d_enc, d_pred = joint_backward(logits, st, model, db2=db2)
         ctx.save_for_backward(d_enc, d_pred)
         return costs
 
@@ -1494,13 +1493,12 @@ def transducer_align(model, x, y, frame_lens, label_lens, x_len=None, t_out=None
         V = model.fc2.weight.shape[0]
         if R:
             _, bounds = SimpleLossFn.apply(enc, pred, model, labels, fl, ll, R, 1.0, False)
-            logits, row_lse, st = _pruned_joint_forward(enc, pred, model, bounds, R)
-            lpb, lpl = K.rnnt_pruned_tables(logits, labels, fl, ll, bounds, U1, R, V, row_lse=row_lse)
+            logits, st = joint_forward(enc, pred, model, want_lse=True, bounds=bounds, R=R)
+            lpb, lpl = K.rnnt_pruned_tables(logits, labels, fl, ll, bounds, U1, R, V, row_lse=st["row_lse"])
         else:
-            logits, st = _joint_forward(enc, pred, model, want_lse=True)
-            row_lse = st.pop("row_lse")
-            lpb, lpl = K.rnnt_tables(logits, labels, fl, ll, V=V, row_lse=row_lse)
-        del logits, row_lse, st
+            logits, st = joint_forward(enc, pred, model, want_lse=True)
+            lpb, lpl = K.rnnt_tables(logits, labels, fl, ll, V=V, row_lse=st["row_lse"])
+        del logits, st
         with _Tap("lattice"):
             loglik = -K.rnnt_lattice_costs(lpb, lpl, fl, ll, B, T, U1)
         with _Tap("viterbi"):

@@ -1,8 +1,8 @@
 """Generic transducer -- drop-in for trainer/model/transducer.py (reference).
 
 ``Net(opt, input_dim, output_dim)`` / ``forward(x, y, x_len, softmax)`` and the sub-module names
-``encoder, embed, decoder, fc1, fc_gate, fc2`` (reached into by the decoder and the MBR trainer)
-are the reference's.  Either encoder of the reference: the LSTM (``encoder_type == 'rnn'``, optionally bidirectional,
+``encoder, embed, decoder, fc1, fc_gate, fc2`` are the reference's.  The joint's layers are run by engine.joint_forward /
+joint_backward (the MBR trainer too) and, for the graph-replayed beam search, read by the decoder.  Either encoder of the reference: the LSTM (``encoder_type == 'rnn'``, optionally bidirectional,
 run over the packed lengths ``x_len``) or the TDNN-Transformer; and either prediction net: the LSTM stack
 (``decoder_type == 'rnn'``) or the convolutional transformer (``'transformer'``, trainer/model/rnnt_conv_transformer_lm.py).
 Modules are created in the reference's order, so ``torch.manual_seed(s); Net(...)`` draws the reference's initial weights.

@@ -124,7 +124,6 @@ def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, 
     bb = bsz * beam
     pad = model.embed.padding_idx
     V = model.fc2.weight.shape[0]
-    H = model.hid_dim
     tgt_cpu = target.cpu().numpy()
     al_cpu = ali_lens.cpu().numpy()
     nonblk, prob, dist, seq_grad, mbr_loss = nbest_risk(hyps, scores, tgt_cpu, al_cpu, blk)
@@ -147,78 +146,28 @@ def mbr_forward_backward(model, feats, target, len_batch, ali_lens, ret, blk=0, 
 
     # ---- RNN-T branch (fused joint + loss, gradients scaled by rnnt_scale)
     pred_ref = pred_d[:bsz, :u_ref + 1].contiguous()
-    logits, st = engine._joint_forward(enc_d, pred_ref, model)
+    logits, st = engine.joint_forward(enc_d, pred_ref, model)
     gs = torch.full((bsz,), float(rnnt_scale), dtype=torch.float32, device=dev)
     db2 = torch.empty(logits.shape[-1], dtype=torch.float32, device=dev)
     costs, _ = K.rnnt_loss_fwd_bwd(logits, target[:, :u_ref].int().contiguous(), len_batch.int().contiguous(),
                                    ali_lens.int().contiguous(), V=V, grad_scale=gs, dlogits=logits, colsum=db2,
                                    fastemit_lambda=fastemit_lambda, delay_penalty=delay_penalty)
-    d_enc, d_pred_ref = engine._joint_backward(logits, st, model, db2=db2)
+    d_enc, d_pred_ref = engine.joint_backward(logits, st, model, db2=db2)
     del logits, st
 
-    # ---- MBR branch: alignment nodes of every hypothesis
-    U1 = U + 1
+    # ---- MBR branch: the joint on the alignment nodes of every hypothesis, its gradients added to the RNN-T branch's
     ex_idx, py_idx, toks, coef = alignment_nodes(hyps, seq_grad, Tp, U, blk)
-    rows = int(toks.shape[0])
     ex_idx_t, py_idx_t, tok_t = (torch.from_numpy(v).to(dev) for v in (ex_idx, py_idx, toks))
     coef_t = torch.from_numpy(coef).to(dev)
-    fc1, fcg, fc2 = model.fc1, model.fc_gate, model.fc2
-    wx = engine.stage_weight([fc1.weight, fcg.weight])
-    w2 = engine.stage_weight(fc2.weight)
-    adt = enc_d.dtype
-    enc2 = enc_d.reshape(bsz * Tp, H)
-    pred_hyp2 = pred_d[bsz:].reshape(bb * U1, H)
-    enc_parts, ph_parts = engine.stage_act(enc2), engine.stage_act(pred_hyp2)
-    ex = torch.empty(bsz * Tp, 2 * H, dtype=adt, device=dev)
-    py = torch.empty(bb * U1, 2 * H, dtype=adt, device=dev)
-    engine.gemm_parts([enc_parts], [[p[:, :H] for p in wx]], ex, bias=engine._cat_bias([fc1.bias, fcg.bias]))
-    engine.gemm_parts([ph_parts], [[p[:, H:] for p in wx]], py)
-    ex_g = torch.empty(rows, 2 * H, dtype=adt, device=dev)
-    py_g = torch.empty(rows, 2 * H, dtype=adt, device=dev)
-    K.gather_rows(ex, ex_idx_t, ex_g)
-    K.gather_rows(py, py_idx_t, py_g)
-    hj = torch.empty(rows, H, dtype=adt, device=dev)
-    K.joint_gate_fwd(ex_g, py_g, hj, rows, 1, 1, H)
-    ldv = engine._ldv(V)
-    z = torch.zeros(rows, ldv, dtype=adt, device=dev)
-    h_parts = engine.stage_act(hj)
-    engine.gemm_parts([h_parts], [w2], z[:, :V], bias=fc2.bias.detach())
+    z, st = engine.joint_forward(enc_d, pred_d[bsz:], model, nodes=(ex_idx_t, py_idx_t))
     K.ce_grad(z, tok_t, coef_t, float(sm_scale), z, V)                         # in place: z := d(mbr)/d(logits)
-    dz_parts = engine.stage_act(z)
-    dz_v = [p[:, :V] for p in dz_parts]
-    dh = torch.empty(rows, H, dtype=adt, device=dev)
-    engine.gemm_parts([dz_v], [w2], dh, b_mn=True)
-    engine.gemm_parts([dz_v], [h_parts], engine.grad_of(fc2.weight), a_mn=True, b_mn=True, accumulate=True, k_splits=1)
-    tmpb = torch.empty(ldv, dtype=torch.float32, device=dev)
-    K.colsum(z, tmpb)
-    K.add(fc2.bias.grad, tmpb[:V].contiguous(), fc2.bias.grad)
-    dex_g = torch.empty(rows, 2 * H, dtype=adt, device=dev)
-    dpy_g = torch.empty(rows, 2 * H, dtype=adt, device=dev)
-    K.joint_gate_bwd(ex_g, py_g, dh, dex_g, dpy_g, rows, 1, 1, H)
-    dex = torch.zeros(bsz * Tp, 2 * H, dtype=torch.float32, device=dev)
-    dpy = torch.zeros(bb * U1, 2 * H, dtype=torch.float32, device=dev)
-    K.scatter_add_rows(dex_g, ex_idx_t, dex)
-    K.scatter_add_rows(dpy_g, py_idx_t, dpy)
-    dex_parts, dpy_parts = engine.stage_act(dex if adt == torch.float32 else engine._to_act(dex)), \
-        engine.stage_act(dpy if adt == torch.float32 else engine._to_act(dpy))
-    g1, gg = engine.grad_of(fc1.weight), engine.grad_of(fcg.weight)
-    for (dparts, xparts, lo) in ((dex_parts, enc_parts, 0), (dpy_parts, ph_parts, H)):
-        engine.gemm_parts([[p[:, :H] for p in dparts]], [xparts], g1[:, lo:lo + H], a_mn=True, b_mn=True, accumulate=True, k_splits=1)
-        engine.gemm_parts([[p[:, H:] for p in dparts]], [xparts], gg[:, lo:lo + H], a_mn=True, b_mn=True, accumulate=True, k_splits=1)
-    dbx = torch.empty(2 * H, dtype=torch.float32, device=dev)                  # bias gradient of the x-side pre-activations
-    K.colsum(dex, dbx)
-    K.add(fc1.bias.grad, dbx[:H].contiguous(), fc1.bias.grad)
-    K.add(fcg.bias.grad, dbx[H:].contiguous(), fcg.bias.grad)
-    d_enc_m = torch.empty(bsz * Tp, H, dtype=adt, device=dev)
-    d_pred_h = torch.empty(bb * U1, H, dtype=adt, device=dev)
-    engine.gemm_parts([dex_parts], [[p[:, :H] for p in wx]], d_enc_m, b_mn=True)
-    engine.gemm_parts([dpy_parts], [[p[:, H:] for p in wx]], d_pred_h, b_mn=True)
+    d_enc_m, d_pred_h = engine.joint_backward(z, st, model, accumulate=True)
 
     # ---- one backward through encoder and prediction net with the summed gradients
     d_enc_tot = torch.empty_like(enc_d)
     K.add(d_enc.reshape(-1), d_enc_m.reshape(-1), d_enc_tot.reshape(-1))
     d_pred_all = torch.zeros_like(pred_d)
     d_pred_all[:bsz, :u_ref + 1] = d_pred_ref
-    d_pred_all[bsz:] = d_pred_h.view(bb, U1, H)
+    d_pred_all[bsz:] = d_pred_h
     torch.autograd.backward([enc, pred_all], [d_enc_tot, d_pred_all])
     return mbr_loss, costs * float(rnnt_scale)
